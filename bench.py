@@ -21,8 +21,16 @@ N = 8 is exactly BASELINE configs[3] (1024^3 ComplexF64, process grid (4,2)).
 
   python bench.py [--gpus N] [--steps K] [--warmup W]        # this framework
   python bench.py --impl reference ...                       # CPU port of the reference path
+
+--dump-outputs DIR writes, after the timed steps, what the last step left in the
+three arrays of the chain (x, y and z pencils: the arrays a caller of transpose!
+receives) as DIR/<pencil>_rank<r>.npy: a fixed, seeded sample of SAMPLE_ELEMS / N
+elements per array and rank (linear indices into the parent array, drawn by
+sample_indices), ComplexF64 as float64 (re, im) pairs, Float32 as float32.
+The inputs are seeded as well, so two builds can be compared output for output.
 """
 import argparse
+import atexit
 import ctypes as C
 import json
 import math
@@ -36,6 +44,7 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 GIB = float(1 << 30)
+SAMPLE_ELEMS = 1 << 20              # --dump-outputs: elements per array over all ranks (<= 48 MiB)
 PER_GPU = (512, 512, 512)           # ComplexF64 shard per GPU: 2 GiB
 CHAIN = [((2, 3), None), ((1, 3), (2, 1, 3)), ((1, 2), (3, 2, 1))]  # x, y, z pencils
 LEGS = ["x->y", "y->z", "z->y", "y->x"]
@@ -62,7 +71,7 @@ def measured_peak():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "fallback: H100 SXM data sheet HBM3 bandwidth, not measured"
 
 
 class ClockSampler:
@@ -86,6 +95,7 @@ class ClockSampler:
                 ["nvidia-smi", "-i", str(self.index), f"--query-gpu={self.Q}",
                  "--format=csv,noheader,nounits", "-lms", "10"],
                 stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
+            atexit.register(self.proc.kill)  # never outlive the benchmark
             self.th = threading.Thread(target=self._read, daemon=True)
             self.th.start()
             t = time.time()
@@ -313,7 +323,7 @@ def cpu_baseline(wl):
                       f"OpenMP over {threads} threads, fastest of {cands})"}
 
 
-# ------------------------------------------------------------------------- B200 arm
+# ------------------------------------------------------------------------- GPU arm
 def time_launches(fn, reps, torch):
     for _ in range(2):
         fn()
@@ -331,7 +341,7 @@ def baseline_kernels(pa, torch, peak):
     (4,2) grid sees them (geometry only: `Comm(0, 8)` has no data plane), and
     r2c-shaped (odd leading extent) permutes, launched through the C ABI exactly as
     pa_transpose launches them; CUDA events around back-to-back launches, arrays of
-    1-2 GiB (>> 126 MB L2)."""
+    1-2 GiB (>> 50 MB L2)."""
     from pencilarrays_b200._lib import lib, check
     from pencilarrays_b200.transpositions import _Plan
     st = C.c_void_p(torch.cuda.current_stream().cuda_stream)
@@ -427,7 +437,7 @@ def configs1_256cubed(pa, torch, peak):
     """BASELINE configs[1]: 256^3 Float64, 1 GPU, x->y for every permutation = one
     fused K3 launch per transpose!.  Two timings: `rotating` -- 24 back-to-back
     launches cycling over 6 source/destination pairs (1.5 GiB touched between two
-    uses of the same array: nothing is served from the 126 MB L2, and launch gaps
+    uses of the same array: nothing is served from the 50 MB L2, and launch gaps
     are hidden as they are in a real chain); `flushed` -- one launch at a time,
     each after a 256 MiB memset (cold L2 and an idle GPU: includes launch latency)."""
     res = {}
@@ -437,7 +447,7 @@ def configs1_256cubed(pa, torch, peak):
     srcs = [pa.PencilArray.undef(torch.float64, q1) for _ in range(NP)]
     for a in srcs:
         a.data.normal_()
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")  # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")  # > 50 MB L2
     nb = 2 * srcs[0].data.numel() * 8
     for perm in ((2, 1, 3), (2, 3, 1), (3, 2, 1), (3, 1, 2), (1, 3, 2), None):
         q2 = pa.Pencil(q1, decomp_dims=(1, 3),
@@ -502,6 +512,26 @@ def pcie_peaks(torch, nbytes):
            "both_directions_GBps_each": round(run(True, True), 1)}
     del h1, h2, d1, d2
     return out
+
+
+def sample_indices(numel, k, torch):
+    """The fixed sample of --dump-outputs: k sorted linear indices into an array of numel."""
+    if numel <= k:
+        return torch.arange(numel)
+    g = torch.Generator().manual_seed(20261015)
+    return torch.randint(0, numel, (k,), generator=g).sort().values
+
+
+def dump_outputs(path, arrays, rank, n, torch):
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    for name, u in arrays.items():
+        flat = u.data.reshape(-1)
+        idx = sample_indices(flat.numel(), SAMPLE_ELEMS // n, torch).to(flat.device)
+        vals = flat[idx]
+        if vals.is_complex():
+            vals = torch.view_as_real(vals)
+        np.save(os.path.join(path, f"{name}_rank{rank}.npy"), vals.cpu().numpy())
 
 
 def run_b200(args):
@@ -647,6 +677,8 @@ def run_b200(args):
             leg_ms[i] += legs[k][i].elapsed_time(legs[k][i + 1]) / args.steps
     leg_ms = [max_over_ranks(x) for x in leg_ms]
     ok = bool(torch.equal(ux.data.view(torch.uint8), orig.view(torch.uint8)))
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"x": ux, "y": uy, "z": uz}, rank, n, torch)
     gbytes = math.prod(dims) * isz
     value = 4 * gbytes / GIB / (ms * 1e-3)
 
@@ -701,8 +733,7 @@ def run_b200(args):
         if args.variants:
             variants = [v for i, v in enumerate(variants) if str(i) in args.variants.split(",")]
         elif not args.all_variants:
-            # (chunked NCCL sends cost ~0.1 ms per operation: 2-3x slower at N=8, measured in
-            #  profiles/r2_bench_n8.json -- kept out of the default run)
+            # (chunked NCCL sends pay a fixed cost per operation -- kept out of the default run)
             variants = [v for v in variants if not (set(v[1]) & {"p2p_chunks", "self_first", "remote_ctas",
                                                                   "oneside_self_ctas"})]
         defaults = {"p2p_chunks": args.p2p_chunks or 1, "ipc_exchange": 1 if args.ipc_exchange else 0,
@@ -783,21 +814,6 @@ def run_b200(args):
     dom = min(base.items(), key=lambda kv: kv[1]["GBps"]) if base else None
     rest = {k: v for k, v in kern.items() if not v.get("baseline_shape")}
     low = min(rest.items(), key=lambda kv: kv[1]["GBps"]) if rest else None
-    def traffic_of(kernel_name):
-        """DRAM bytes per launch of that kernel from the committed ncu capture
-        (profiles/traffic.json, which names the file and the date); None when the selected
-        kernel has no capture."""
-        try:
-            with open(os.path.join(ROOT, "profiles", "traffic.json")) as f:
-                tj = json.load(f)
-            for key, ent in tj.get("by_kernel", {}).items():
-                if key in kernel_name:
-                    return ent.get("bytes_per_launch"), {k: ent.get(k) for k in (
-                        "kernel", "file", "date", "algorithmic_bytes_per_launch")}
-        except Exception:
-            pass
-        return None, None
-
     # ---- BASELINE configs[1] beside it (N == 1): 256^3 Float64, 1 GPU, pack/unpack kernel only ----
     cfg1 = configs1_256cubed(pa, torch, peak) if (n == 1 and args.workload == "cfg4" and not args.quick) else None
     fused = None
@@ -886,7 +902,8 @@ def run_b200(args):
                                "unpack_ms": round(tm.unpack_ms, 3), "total_ms": round(tm.total_ms, 3),
                                "send_bytes": info.send_bytes,
                                "nvlink_GBps_out": round(info.send_bytes / max(tm.exchange_ms, 1e-6) / 1e6, 1),
-                               "nvlink_frac_of_770": round(info.send_bytes / max(tm.exchange_ms, 1e-6) / 1e6 / 770, 3)}
+                               # H100 SXM data sheet: NVLink 4, 450 GB/s per direction
+                               "nvlink_frac_of_450": round(info.send_bytes / max(tm.exchange_ms, 1e-6) / 1e6 / 450, 3)}
         chain(ts)
 
     # ---- CPU baseline beside it (rank 0, N == 1 only) -------------------------------
@@ -903,7 +920,7 @@ def run_b200(args):
             "dtype": ("c128" if isz == 16 else "f32") + " (bytes; pure data movement)", "data": "synthetic",
             "config": {"workload": workload_name(n, args.workload), "method": repr(method), "overlap": overlap,
                        "transport": comm.transport,
-                       "l2": "inputs (2 GiB per GPU) far larger than the 126 MB L2; no flush needed",
+                       "l2": "inputs (2 GiB per GPU) far larger than the 50 MB L2; no flush needed",
                        "round_trip_bit_exact": ok, "placement_exact_full_size": placed,
                        "leg_ms": dict(zip(LEGS, [round(x, 4) for x in leg_ms]))},
             "gpu_launches": int(launches),
@@ -922,8 +939,7 @@ def run_b200(args):
                             "last download, max over ranks"},
             "roofline": None if dom is None else {
                 "bound": "hbm", "kernel": dom[0], "achieved": dom[1]["GBps"], "peak": peak,
-                "unit": "GB/s", "frac": round(dom[1]["GBps"] / peak, 4), "traffic": traffic_of(dom[0])[0],
-                "traffic_source": traffic_of(dom[0])[1], "peak_source": peak_src,
+                "unit": "GB/s", "frac": round(dom[1]["GBps"] / peak, 4), "peak_source": peak_src,
                 "alg_bytes_per_launch": dom[1]["alg_bytes"] // max(1, dom[1].get("launches", 1)),
                 "selection": "slowest of the BASELINE-shape kernels in `kernels` (K1 pack, K2 unpack, "
                              "K3 fused; configs[1], [3], [4])",
@@ -971,7 +987,11 @@ def main():
     ap.add_argument("--host-chunk-mib", type=int, default=None, help="e2e: tunable host_chunk_bytes")
     ap.add_argument("--quick", action="store_true", help="skip the side measurements (kernels, configs[1])")
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write a seeded sample of the last timed step's arrays as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        raise SystemExit("--steps must be at least 1")
     if args.gpus not in (1, 2, 4, 8):
         raise SystemExit("--gpus must be 1, 2, 4 or 8")
     if args.warmup < 3:

@@ -1,5 +1,5 @@
 /*
- * pa_b200.h -- C ABI of the B200-native global-transposition hot path.
+ * pa_b200.h -- C ABI of the H100-native global-transposition hot path.
  *
  * This is the drop-in boundary for the `transpose!` path of PencilArrays.jl
  * (reference: src/Transpositions/Transpositions.jl).  The reference has no
@@ -52,7 +52,7 @@ typedef enum pa_status {
 typedef enum pa_method {
   PA_POINT_TO_POINT = 0, /* Transpositions.PointToPoint  (Transpositions.jl:18) */
   PA_ALLTOALLV = 1,      /* Transpositions.Alltoallv     (Transpositions.jl:19) */
-  PA_PEER_PUT = 2,       /* B200 extension (no reference counterpart): one-sided puts.
+  PA_PEER_PUT = 2,       /* GPU extension (no reference counterpart): one-sided puts.
                             The pack kernel of each remote block stores straight into
                             the destination rank's `dest` array over NVLink (peer-mapped
                             memory): no send_buf, no recv_buf, no unpack pass.  Needs

@@ -26,7 +26,7 @@ import numpy as np
 
 
 # --------------------------------------------------------------------------- permutations
-# StaticPermutations.jl v0.3 (third-party, not under /root/reference); the
+# StaticPermutations.jl v0.3 (third-party, not part of the reference); the
 # semantics used are pinned by src/arrays.jl:19-31 and Transpositions.jl:503,524,599.
 def perm_apply(p, t):
     """`p * t`: (p * t)[i] = t[p[i]]; p = None is NoPermutation."""

@@ -1,9 +1,9 @@
-"""B200-native implementation of the PencilArrays.jl global-transposition path.
+"""H100-native implementation of the PencilArrays.jl global-transposition path.
 
 Host-side mirror (Python; Julia is not available in this image -- the Julia
 veneer over the same C ABI is in ``julia/B200PencilArrays.jl``) of the
 reference's ``Pencil`` / ``PencilArray`` / ``Transpositions`` interface.  All
-data movement runs in hand-written sm_100a CUDA kernels inside
+data movement runs in hand-written sm_90a CUDA kernels inside
 ``libpa_b200.so``; importing this package without that library fails.
 
 The directory name contains a dot, so import it through the repo-root shim:

@@ -21,7 +21,7 @@ using namespace pa;
 
 extern "C" {
 
-const char* pa_version(void) { return "pa_b200 0.2.0 (sm_100a)"; }
+const char* pa_version(void) { return "pa_b200 0.2.0 (sm_90a)"; }
 
 const char* pa_strerror(pa_status s) {
   switch (s) {

@@ -2,7 +2,7 @@
 //
 // In a PencilFFTs-style transform every transposition is followed by a 1-d FFT
 // along the dimension that has just become local and -- thanks to the pencil's
-// permutation -- contiguous (/root/reference/docs/src/Pencils.md:210-214;
+// permutation -- contiguous (reference docs/src/Pencils.md:210-214;
 // docs/src/Transpositions.md:7-9).  Unfused that is two HBM round trips: the
 // unpack (copy_permuted!, Transpositions.jl:585-664) writes the permuted array,
 // the FFT reads and rewrites it.  This kernel does both in one:
@@ -147,9 +147,8 @@ __global__ void __launch_bounds__(FFT_THREADS) k_unpack_fft(const __grid_constan
   constexpr int RS = FFT_THREADS / C;  // rows per sweep
   constexpr int LOGRS = (C == 8) ? 5 : 6;
   static_assert((1 << LOGRS) == RS, "rows per sweep");
-  // (measured on B200, profiles/r2_fused_fft.txt: a win for 1024-point lines -- one CTA
-  //  per SM less bound by shared memory --, a loss for 512-point lines, where the radix-16
-  //  butterfly's 126 registers cost the third resident CTA: 1.17 -> 1.45 ms at 512^3)
+  // (only for 1024-point lines, where shared memory bounds the CTAs per SM; for 512-point
+  //  lines the radix-16 butterfly's registers would cost the third resident CTA)
   constexpr int LOGR1 = (C == 4 && LOGL > LOGRS) ? (LOGL - LOGRS) : 0;
   static_assert(LOGR1 == 0 || LOGL - LOGR1 == LOGRS, "first-pass stride must equal the sweep");
   const cplx* twp = p.tw;

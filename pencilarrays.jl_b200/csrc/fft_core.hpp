@@ -1,7 +1,7 @@
 // Radix passes of the in-shared-memory 1-d complex FFT that the fused
 // unpack+FFT kernel (fft.cu) runs on every line it has just transposed.
 // SURVEY.md §8(f2): the permutation of a pencil exists to make the FFT axis
-// contiguous (/root/reference/docs/src/Pencils.md:210-214,
+// contiguous (reference docs/src/Pencils.md:210-214,
 // docs/src/Transpositions.md:7-9) -- here the transform is applied before the
 // line ever leaves the SM.
 //

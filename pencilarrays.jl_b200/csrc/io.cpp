@@ -1,5 +1,5 @@
 // PencilIO binary layout (SURVEY.md §8 f4): device arrays <-> the raw binary files of
-// the reference's MPIIODriver (/root/reference/src/PencilIO/mpi_io.jl).
+// the reference's MPIIODriver (reference src/PencilIO/mpi_io.jl).
 //
 // Layout written by the reference and reproduced here byte for byte:
 //  * discontiguous (chunks = false, the default; :372-380 `create_discontiguous_datatype`

@@ -1,4 +1,4 @@
-// sm_100a kernels of the transpose! hot path.
+// sm_90a kernels of the transpose! hot path.
 //
 // Every data movement of the path -- K1 pack (copy_range!,
 // Transpositions.jl:552-583), K2 unpack+permute (copy_permuted! ->
@@ -589,10 +589,10 @@ static long long cdiv(long long a, long long b) { return (a + b - 1) / b; }
 
 static int sm_count() {
   static int n = [] {
-    int dev = 0, v = 148;
+    int dev = 0, v = 132;
     if (cudaGetDevice(&dev) == cudaSuccess)
       cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
-    return v > 0 ? v : 148;
+    return v > 0 ? v : 132;
   }();
   return n;
 }
@@ -708,9 +708,8 @@ static pa_status prepare(const BlockCopy& b, const void* src, void* dst, KParams
     sel.w = W;
     if (vec_used) *vec_used = W;
   } else if (b.klass == KC_TRANSPOSE && (S == 4 || S == 8 || S == 16)) {
-    // destination-run length of a tile = TBQ*16 B.  256 B (TBQ = 16) wins or ties on every
-    // shape measured on B200, from 128 MiB to 2 GiB blocks (profiles/r2_shapes_sweep.txt:
-    // more, smaller tiles -> shorter tail, fewer DRAM pages open per tile); tunable
+    // destination-run length of a tile = TBQ*16 B.  256 B (TBQ = 16) by default: more,
+    // smaller tiles -> shorter tail, fewer DRAM pages open per tile; tunable
     // "transpose_tbq" = 32 selects 512-B runs
     int tbq = g_tun.transpose_tbq == 32 && S != 4 ? 32 : 16;
     const int V = 16 / (int)S;
@@ -723,8 +722,7 @@ static pa_status prepare(const BlockCopy& b, const void* src, void* dst, KParams
     // destination rows are much shorter than the source rows (few tiles along Y, many
     // along X -- typically a 2-d transpose left after merging dims) walking along Y
     // first fills whole destination rows (full DRAM pages) instead of 256-byte pieces
-    // of thousands of them; measured 0.45-0.74 -> 0.95-0.99 of the HBM roofline on the
-    // r2c-shaped grids, neutral elsewhere (profiles/r2_shapes_sweep.txt).  Tunable
+    // of thousands of them (the r2c-shaped grids of bench.py).  Tunable
     // "transpose_y_fastest": -1 = this rule (default), 0 / 1 = forced.
     p.y_fastest = g_tun.transpose_y_fastest >= 0 ? g_tun.transpose_y_fastest
                                                  : (2ull * p.tiles_y <= (unsigned long long)p.tiles_x);

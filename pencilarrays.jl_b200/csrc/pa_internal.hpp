@@ -151,7 +151,7 @@ pa_status launch_multi(int nb, const BlockCopy* const* blocks, const void* const
 // run-time tunables (pa_set_tunable)
 struct Tunables {
   int remote_ctas = -4;   // grid cap of put/get kernels: n > 0 CTAs, n < 0 = |n| per SM, 0 = uncapped
-                          // (4 per SM: full NVLink rate in profiles/r1_nvlink_microbench.txt)
+                          // (a few CTAs per SM drive the links; the rest stay free for local work)
   int box_copy_ctas = 0;  // grid cap applied to pa_box_copy (benchmarks)
   int transpose_y_fastest = -1;  // transpose tile order: 1 = consecutive CTAs along the destination rows,
                                  // 0 = along the source rows, -1 = along the side with fewer tiles (kernels.cu)

@@ -5,7 +5,7 @@
 // block is packed (:406-412) or one Alltoallv after all packs (:418-427); then
 // unpack blocks as they arrive (transpose_recv!, :486-533), self block first.
 //
-// B200 restatement: three CUDA streams (pack / comm / unpack) joined by
+// GPU restatement: three CUDA streams (pack / comm / unpack) joined by
 // events.  PointToPoint = one {send, recv} pair per exchange step, enqueued the
 // moment that step's pack finishes, unpack gated on that step's receive -- so
 // pack(k+1), exchange(k) and unpack(k-1) overlap; every peer block can be cut

@@ -165,7 +165,7 @@ end
 method_code(::PointToPoint) = Cint(0)
 method_code(::Alltoallv) = Cint(1)
 
-# B200 extensions (no reference counterpart): one-sided transposition methods.
+# GPU extensions (no reference counterpart): one-sided transposition methods.
 # `PeerPut`: every remote block is stored by ONE kernel straight into the
 # destination rank's `dest` over NVLink; `PeerGet`: pull flavour.  Usage:
 #     t = Transposition(dest, src; method = B200PencilArrays.PeerPut())
@@ -227,7 +227,7 @@ const DeviceTransposition{T,N} = Transposition{T,N,<:Pencil,<:Pencil,
     <:PencilArray{T,N,<:CuArray},<:PencilArray{T,N,<:CuArray}}
 
 # transpose!(t; waitall) (Transpositions.jl:170-179).
-# `fft = :forward | :backward` (B200 extension, PA_FFT_FORWARD / PA_FFT_BACKWARD): the unpack
+# `fft = :forward | :backward` (GPU extension, PA_FFT_FORWARD / PA_FFT_BACKWARD): the unpack
 # and the 1-d FFT along dest's contiguous dimension -- the next step of a PencilFFTs plan --
 # run as ONE kernel (ComplexF64, power-of-two lines of 8..1024 points, staged methods).
 function Transpositions.transpose!(t::DeviceTransposition; waitall = true, fft = nothing)

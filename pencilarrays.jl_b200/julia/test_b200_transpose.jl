@@ -1,12 +1,12 @@
 # test_b200_transpose.jl -- pins libpa_b200 against the REAL reference.
 #
 # NOT EXECUTED IN THIS REPOSITORY (no Julia / MPI in the build image).  For a
-# maintainer with Julia, MPI, CUDA.jl and >= 1 B200:
+# maintainer with Julia, MPI, CUDA.jl and >= 1 H100:
 #
 #     mpiexec -n 8 julia --project test_b200_transpose.jl
 #
 # Every rank runs the reference's own CPU `transpose!` (Array storage, MPI
-# transport) and the B200 path (CuArray storage, this library) on identical
+# transport) and the GPU path (CuArray storage, this library) on identical
 # inputs and compares the parent arrays byte for byte -- the check this
 # repository can only make against its CPU oracle (oracle/pencil_oracle.py).
 using MPI

@@ -195,7 +195,7 @@ class Pencil:
 
     def __repr__(self):
         return ("Decomposition of {}D data\n    Data dimensions: {}\n    Decomposed dimensions: {}\n"
-                "    Data permutation: {}\n    Array type: CUDA device memory (B200)").format(
+                "    Data permutation: {}\n    Array type: CUDA device memory (H100)").format(
                     self.ndims, self.size_global, self.decomp_dims, self.perm)
 
 

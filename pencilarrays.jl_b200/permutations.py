@@ -1,7 +1,7 @@
 """Index-permutation algebra of the path (host side, tiny).
 
 Restates the subset of StaticPermutations.jl (v0.3, a dependency of the
-reference that is not vendored under /root/reference) that `transpose!` uses;
+reference that is not vendored in the reference) that `transpose!` uses;
 semantics pinned by the reference's own uses and examples:
 
 * ``(p * t)[i] == t[p[i]]``  -- logical -> memory order

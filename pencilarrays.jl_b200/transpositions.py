@@ -46,7 +46,7 @@ class Alltoallv(AbstractTransposeMethod):  # Transpositions.jl:19
 
 
 class PeerPut(AbstractTransposeMethod):
-    """B200 extension (no reference counterpart): one-sided puts over NVLink.
+    """GPU extension (no reference counterpart): one-sided puts over NVLink.
 
     Each remote block is packed by a kernel that stores straight into the
     destination rank's ``dest`` array through a peer mapping -- no ``send_buf``,
@@ -289,7 +289,7 @@ def Waitall(t: Transposition):
 def transpose_(*args, method=None, waitall=True, overlap=True, stage_self=False, fft=None):
     """``transpose!(dest, src; method)`` or ``transpose!(t; waitall)`` (:160-179).
 
-    ``fft="forward"`` / ``"backward"`` (B200 extension, SURVEY 8 f2): the unpack and the
+    ``fft="forward"`` / ``"backward"`` (GPU extension, SURVEY 8 f2): the unpack and the
     1-d complex FFT along ``dest``'s contiguous dimension -- the step a PencilFFTs-style
     plan runs next -- execute as one kernel; ``dest`` receives the transformed array."""
     if len(args) == 1 and isinstance(args[0], Transposition):

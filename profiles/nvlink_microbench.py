@@ -4,7 +4,7 @@
 One process, two GPUs (peer access enabled by torch): the same `pa_box_copy`
 kernels the PeerPut / PeerGet paths launch, with src or dst on the other GPU,
 timed with CUDA events -- against `cudaMemcpyPeerAsync` (torch `copy_`) as the
-yardstick.  Needs >= 2 GPUs:  gpurun --gpus 2 -- python profiles/nvlink_microbench.py
+yardstick.  Needs >= 2 GPUs:  python profiles/nvlink_microbench.py
 """
 import ctypes as C
 import os
@@ -106,7 +106,7 @@ def main():
     def cap(n):
         check(lib.pa_set_tunable(b"box_copy_ctas", n))
 
-    for c in (37, 74, 148, 296, 592, 1184, 0):
+    for c in (33, 66, 132, 264, 528, 1056, 0):  # multiples of the 132 SMs
         cap(c)
         rec(f"k_transpose_vec<16> PUT grid cap {c}", timeit([lambda: launch(e, s_, d_, 16, a0, b1, 0)], [0]))
         rec(f"k_transpose_vec<16> GET grid cap {c}", timeit([lambda: launch(e, s_, d_, 16, a1, b0, 0)], [0]))
@@ -117,7 +117,7 @@ def main():
     hi = torch.cuda.Stream(device=0, priority=-1)
     lo = torch.cuda.Stream(device=0, priority=0)
     c0 = torch.empty(N, dtype=torch.uint8, device="cuda:0")
-    for c in (0, 148, 296, 592):
+    for c in (0, 132, 264, 528):
         def both():
             with torch.cuda.stream(lo):
                 cap(0)
@@ -137,7 +137,7 @@ def main():
     # ---- TMA bulk-copy pipeline (k_rows_bulk, tunable bulk_rows) ----
     check(lib.pa_set_tunable(b"bulk_rows", 1))
     e4, s4, d4 = [256, 256 * 1024], [1, 1024], [1, 256]
-    for c in (148, 296, 444, 592, 888):
+    for c in (132, 264, 396, 528, 792):
         cap(c)
         rec(f"k_rows_bulk local contiguous, {c} CTAs", timeit([lambda: launch([nel], [1], [1], 16, a0, b0, 0)], [0]))
         rec(f"k_rows_bulk PUT contiguous, {c} CTAs", timeit([lambda: launch([nel], [1], [1], 16, a0, b1, 0)], [0]))

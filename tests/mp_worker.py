@@ -269,7 +269,7 @@ def main():
             u = pa.PencilArray.undef(tdt, pen, *extra)
             u.data.view(torch.uint8).reshape(-1).copy_(torch.from_numpy(
                 np.ascontiguousarray(mine.data.reshape(-1, order="F")).view(np.uint8).copy()))
-            fname = f"/tmp/pa_io_{os.environ.get('MASTER_PORT', '0')}_{case['name']}.bin"
+            fname = os.path.join(os.environ["PA_TEST_TMPDIR"], f"pa_io_{case['name']}.bin")
             with pa.open_(pa.MPIIODriver(), fname, comm, write=True, create=True) as ff:
                 ff.write("u", u, chunks=False)
                 ff.write("u_chunks", u, chunks=True)

@@ -1,6 +1,6 @@
 """bench.py contract pieces that can run without a GPU: the reference arm
 (CPU port of the reference path) prints one JSON line with the agreed keys,
-and the B200 arm refuses to run (no CPU fallback) on a GPU-less box."""
+and the GPU arm refuses to run (no CPU fallback) on a GPU-less box."""
 import json
 import os
 import subprocess
