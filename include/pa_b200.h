@@ -338,6 +338,24 @@ pa_status pa_wait(pa_plan* plan, void* stream);
 pa_status pa_transpose_host(pa_plan* plan, pa_comm* comm, const void* host_src,
                             void* host_dst, unsigned flags);
 
+/* ---- real-to-complex line transforms ----------------------------------------
+ * Step 1 of a PencilFFTs real-input plan (rfft along the first, local dimension; the
+ * two complex steps are the fused transposes above), and its inverse.  `real` has global
+ * size (..., N, ...), `cplx` the same with N/2+1 along the transform axis = the first
+ * MEMORY-order dimension (perm[1]) of both, which must not be decomposed; same topology
+ * object, decomposition and permutation (Pencil(p; size_global) builds such a pencil).
+ *   PA_FFT_FORWARD:  src = real Float64 array, dst = ComplexF64 array, dst = rfft(src)
+ *   PA_FFT_BACKWARD: src = ComplexF64, dst = Float64, dst = N * irfft(src, N) -- unnormalised
+ *                    like FFTW's brfft; the imaginary parts of bins 0 and N/2 are ignored and
+ *                    `src` is left unmodified.
+ * N: power of two in 16..2048.  One kernel per call, local to the rank (no communication);
+ * extra dims are batched.  Arrays dense (parent layout), 16-byte aligned, not overlapping;
+ * NULL allowed where the local array is empty.  Ordered on `stream` like pa_transpose.
+ * PA_EINCOMPAT: pencils not related as above; PA_EINVAL: other bad arguments.          */
+pa_status pa_rfft(const pa_pencil* real, const pa_pencil* cplx, int n_extra,
+                  const int64_t* extra_dims, unsigned flags, const void* src, void* dst,
+                  void* stream);
+
 /* ---- host chains -----------------------------------------------------------
  * A sequence of transpositions applied to HOST arrays (plan i+1 consumes what
  * plan i produces): one submit = upload of `host_src`, every transpose! on the

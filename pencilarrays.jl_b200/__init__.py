@@ -23,7 +23,8 @@ from .arrays import (PencilArray, ManyPencilArray, parent, pencil, extra_dims, n
                      size_local, similar)
 from . import transpositions as Transpositions
 from .transpositions import (Transposition, transpose_, transpose_bang, Waitall, PointToPoint,
-                             Alltoallv, PeerPut, PeerGet, HostChain, transpose_host_, set_tunable, fft_)
+                             Alltoallv, PeerPut, PeerGet, HostChain, transpose_host_, set_tunable, fft_,
+                             rfft_, brfft_)
 
 
 from . import pencilio as PencilIO

@@ -652,6 +652,111 @@ pa_status pa_transpose_host(pa_plan* plan, pa_comm* comm, const void* host_src, 
   })
 }
 
+// ---- real-to-complex line transforms ------------------------------------------------
+// Every check runs on the host before any device call.
+static pa_status rfft_checks(const pa_pencil* real, const pa_pencil* cplx, int n_extra,
+                             const int64_t* extra_dims, unsigned flags, const void* src,
+                             const void* dst, int* N_out, i64* nlines_out) {
+  if (!real || !cplx) {
+    set_error("pa_rfft: null pencil");
+    return PA_EINVAL;
+  }
+  const Pencil& R = *real->p;
+  const Pencil& Cp = *cplx->p;
+  if (R.topo != Cp.topo || R.N != Cp.N) {
+    set_error("pa_rfft: the pencils must share their topology and number of dimensions");
+    return PA_EINCOMPAT;
+  }
+  const int M = R.topo->M;
+  for (int i = 0; i < M; ++i)
+    if (R.decomp[i] != Cp.decomp[i]) {
+      set_error("pa_rfft: the pencils have different decompositions");
+      return PA_EINCOMPAT;
+    }
+  for (int d = 0; d < R.N; ++d)
+    if (R.perm[d] != Cp.perm[d]) {
+      set_error("pa_rfft: the pencils have different permutations");
+      return PA_EINCOMPAT;
+    }
+  const int ax = R.perm[0];  // logical dim of the first memory dim: the transform axis
+  for (int i = 0; i < M; ++i)
+    if (R.decomp[i] == ax) {
+      set_error("pa_rfft: the transform axis (logical dim %d) is decomposed", ax + 1);
+      return PA_EINCOMPAT;
+    }
+  for (int d = 0; d < R.N; ++d)
+    if (d != ax && R.size_global[d] != Cp.size_global[d]) {
+      set_error("pa_rfft: global sizes differ along dim %d", d + 1);
+      return PA_EINCOMPAT;
+    }
+  const i64 N = R.size_global[ax];
+  if (Cp.size_global[ax] != N / 2 + 1) {
+    set_error("pa_rfft: the complex pencil has %lld points along the transform axis, expected "
+              "N/2+1 = %lld", (long long)Cp.size_global[ax], (long long)(N / 2 + 1));
+    return PA_EINCOMPAT;
+  }
+  if (flags != PA_FFT_FORWARD && flags != PA_FFT_BACKWARD) {
+    set_error("pa_rfft: flags must be exactly PA_FFT_FORWARD or PA_FFT_BACKWARD");
+    return PA_EINVAL;
+  }
+  if (N < 16 || N > 2048 || (N & (N - 1))) {
+    set_error("pa_rfft: N = %lld is not a power of two in 16..2048", (long long)N);
+    return PA_EINVAL;
+  }
+  if (n_extra < 0 || (n_extra > 0 && !extra_dims) || R.N + n_extra > PA_MAX_DIMS) {
+    set_error("pa_rfft: %d extra dims on a %d-d pencil (at most %d dims in all)", n_extra, R.N,
+              PA_MAX_DIMS);
+    return PA_EINVAL;
+  }
+  i64 lo[PA_MAX_DIMS], hi[PA_MAX_DIMS];
+  R.range_local(lo, hi);
+  i64 nlines = 1;
+  for (int d = 0; d < R.N; ++d)
+    if (d != ax) nlines *= hi[d] - lo[d];
+  for (int i = 0; i < n_extra; ++i) {
+    if (extra_dims[i] < 0) {
+      set_error("pa_rfft: negative extra dim");
+      return PA_EINVAL;
+    }
+    nlines *= extra_dims[i];
+  }
+  const bool fwd = flags == PA_FFT_FORWARD;
+  const i64 real_bytes = nlines * N * 8, cplx_bytes = nlines * (N / 2 + 1) * 16;
+  const i64 src_bytes = fwd ? real_bytes : cplx_bytes, dst_bytes = fwd ? cplx_bytes : real_bytes;
+  if (nlines > 0) {
+    if (!src || !dst) {
+      set_error("pa_rfft: null array pointer for a non-empty local array");
+      return PA_EINVAL;
+    }
+    const uintptr_t s = (uintptr_t)src, d = (uintptr_t)dst;
+    if (s < d + (uintptr_t)dst_bytes && d < s + (uintptr_t)src_bytes) {
+      set_error("pa_rfft: src and dst overlap");
+      return PA_EINVAL;
+    }
+    if ((s | d) & 15) {
+      set_error("pa_rfft: src and dst must be 16-byte aligned");
+      return PA_EINVAL;
+    }
+  }
+  *N_out = (int)N;
+  *nlines_out = nlines;
+  return PA_OK;
+}
+
+pa_status pa_rfft(const pa_pencil* real, const pa_pencil* cplx, int n_extra,
+                  const int64_t* extra_dims, unsigned flags, const void* src, void* dst,
+                  void* stream) {
+  GUARD({
+    int N = 0;
+    i64 nlines = 0;
+    pa_status s = rfft_checks(real, cplx, n_extra, extra_dims, flags, src, dst, &N, &nlines);
+    if (s != PA_OK) return s;
+    s = need_gpu();
+    if (s != PA_OK) return s;
+    return rfft_lines(N, flags == PA_FFT_FORWARD, nlines, src, dst, stream);
+  })
+}
+
 pa_status pa_host_chain_create(int n, pa_plan* const* plans, pa_comm* comm, pa_host_chain** out) {
   GUARD({
     if (n < 1 || n > 64 || !plans || !out) {

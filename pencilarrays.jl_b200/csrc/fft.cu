@@ -233,6 +233,107 @@ __global__ void __launch_bounds__(FFT_THREADS) k_unpack_fft(const __grid_constan
   }
 }
 
+// ---- real lines (rfft_ / brfft_, DESIGN §3c): N = 2L reals <-> N/2 + 1 complex bins ----
+// The lines are dense and consecutive on both sides (the transform axis is the first memory dim
+// of both arrays, the other dims are the same), so a launch is a flat batch of `nlines` lines.
+struct RfftParams {
+  const char* src;
+  char* dst;
+  long long nlines;
+  long long src_line, dst_line;  // byte strides of consecutive lines
+  int pitch;
+  const cplx* tw;  // W_N^k, k < N: the post- / pre-pass reads entry k, the L-point passes entry 2i
+};
+
+template <int LOGL, int C, bool FWD>
+__global__ void __launch_bounds__(FFT_THREADS) k_rfft(const __grid_constant__ RfftParams p) {
+  constexpr int L = 1 << LOGL;
+  constexpr int RS = FFT_THREADS / C;  // threads per line
+  constexpr int P = L / 2 + 1;         // pairs (k, L - k) per line
+  extern __shared__ __align__(16) unsigned char fft_smem[];
+  cplx* sm = reinterpret_cast<cplx*>(fft_smem);
+  const int t = threadIdx.x;
+  const long long l0 = (long long)blockIdx.x * C;
+  const int ncol = (int)((p.nlines - l0) < C ? (p.nlines - l0) : C);
+  const int pitch = p.pitch;
+  const cplx* twp = p.tw;
+  auto twN = [twp](int k) {
+    const double2 w = __ldg(reinterpret_cast<const double2*>(twp) + k);
+    return cplx{w.x, w.y};
+  };
+  auto twL = [twp](int i) {  // W_L^i = W_N^(2i)
+    const double2 w = __ldg(reinterpret_cast<const double2*>(twp) + 2 * i);
+    return cplx{w.x, w.y};
+  };
+
+  // ---- load (linear gather): consecutive threads walk along a line with 128-bit loads.
+  //      Forward: the N reals ARE the complex line z[n] = x[2n] + i x[2n+1]; backward: N/2+1 bins ----
+  {
+    constexpr int NIN = FWD ? L : L + 1;
+    constexpr int U = (NIN + RS - 1) / RS;
+    const int c = t / RS, r = t % RS;
+    if (c < ncol) {
+      const double2* s = reinterpret_cast<const double2*>(p.src + (l0 + c) * p.src_line);
+      cplx* line = sm + c * pitch;
+      double2 v[U];
+#pragma unroll
+      for (int q = 0; q < U; ++q)
+        if (r + q * RS < NIN) v[q] = __ldcs(s + r + q * RS);
+#pragma unroll
+      for (int q = 0; q < U; ++q)
+        if (r + q * RS < NIN) line[pa_fft::pad_index(r + q * RS)] = cplx{v[q].x, v[q].y};
+    }
+  }
+  __syncthreads();
+
+  if constexpr (!FWD) {
+    // ---- pre-pass in place: a thread owns the slots k and L - k of its pair ----
+#pragma unroll
+    for (int w0 = 0; w0 < C * P; w0 += FFT_THREADS) {
+      const int w = w0 + t, c = w / P, k = w % P;
+      if (w < C * P && c < ncol) {
+        cplx* line = sm + c * pitch;
+        cplx zk, zl;
+        pa_fft::brfft_pre_pair(k, line[pa_fft::pad_index(k)], line[pa_fft::pad_index(L - k)], twN(k),
+                               &zk, &zl);
+        line[pa_fft::pad_index(k)] = zk;
+        if (k > 0) line[pa_fft::pad_index(L - k)] = zl;
+      }
+    }
+    __syncthreads();
+  }
+
+  fft_passes<LOGL, LOGL, C>(sm, pitch, ncol, FWD ? -1 : 1, twL);
+
+  if constexpr (FWD) {
+    // ---- post-pass + store: N/2 + 1 bins per line, one contiguous run ----
+#pragma unroll
+    for (int w0 = 0; w0 < C * P; w0 += FFT_THREADS) {
+      const int w = w0 + t, c = w / P, k = w % P;
+      if (w < C * P && c < ncol) {
+        const cplx* line = sm + c * pitch;
+        cplx xk, xl;
+        pa_fft::rfft_post_pair(line[pa_fft::pad_index(fft_pos<LOGL, LOGL>(k & (L - 1)))],
+                               line[pa_fft::pad_index(fft_pos<LOGL, LOGL>((L - k) & (L - 1)))], twN(k),
+                               &xk, &xl);
+        double2* out = reinterpret_cast<double2*>(p.dst + (l0 + c) * p.dst_line);
+        __stcs(out + k, make_double2(xk.x, xk.y));
+        if (k != L - k) __stcs(out + (L - k), make_double2(xl.x, xl.y));
+      }
+    }
+  } else {
+    // ---- store: z[n] = x[2n] + i x[2n+1], the N reals of a line as L 128-bit stores ----
+#pragma unroll
+    for (int w0 = 0; w0 < C * L; w0 += FFT_THREADS) {
+      const int w = w0 + t, c = w >> LOGL, n = w & (L - 1);
+      if (c < ncol) {
+        const cplx v = sm[c * pitch + pa_fft::pad_index(fft_pos<LOGL, LOGL>(n))];
+        __stcs(reinterpret_cast<double2*>(p.dst + (l0 + c) * p.dst_line) + n, make_double2(v.x, v.y));
+      }
+    }
+  }
+}
+
 // forward twiddle table W_L^k per (device, L), computed once in extended precision
 static const cplx* twiddles(int L) {
   static std::mutex mu;
@@ -416,6 +517,63 @@ pa_status unpack_fft(int nb, const BlockCopy* const* blocks, const void* const* 
   }
   if (e != cudaSuccess) {
     set_error("fused FFT kernel launch failed: %s", cudaGetErrorString(e));
+    return PA_ECUDA;
+  }
+  count_launch();
+  return PA_OK;
+}
+
+pa_status rfft_lines(int N, bool forward, i64 nlines, const void* src, void* dst, void* stream) {
+  const int L = N / 2;
+  int logL = 0;
+  while ((1 << logL) < L) ++logL;
+  if ((1 << logL) != L || logL < 3 || logL > 10) {
+    set_error("rfft: line length %d is not a power of two in 16..2048", N);
+    return PA_EINVAL;
+  }
+  if (nlines == 0) return PA_OK;
+  RfftParams p;
+  p.src = (const char*)src;
+  p.dst = (char*)dst;
+  p.nlines = nlines;
+  p.src_line = forward ? 8LL * N : 16LL * (L + 1);
+  p.dst_line = forward ? 16LL * (L + 1) : 8LL * N;
+  p.pitch = pa_fft::padded_pitch(forward ? L : L + 1);  // backward stages all N/2 + 1 bins
+  p.tw = twiddles(N);
+  if (!p.tw) {
+    set_error("rfft: twiddle table allocation failed");
+    cudaGetLastError();
+    return PA_ENOMEM;
+  }
+  const int C = fft_lines(logL);
+  const long long grid = (nlines + C - 1) / C;
+  if (grid > 0x7fffffffLL) {
+    set_error("rfft: too many lines for one launch");
+    return PA_EINVAL;
+  }
+  const size_t smem = sizeof(cplx) * (size_t)C * p.pitch;
+  cudaError_t e = cudaSuccess;
+  auto launch = [&](auto kern) {
+    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout,
+                         cudaSharedmemCarveoutMaxShared);
+    cudaGetLastError();
+    kern<<<(unsigned)grid, FFT_THREADS, smem, (cudaStream_t)stream>>>(p);
+    e = cudaGetLastError();
+  };
+  auto launch_dir = [&](auto fwd_kern, auto bwd_kern) { forward ? launch(fwd_kern) : launch(bwd_kern); };
+  switch (logL) {
+    case 3: launch_dir(k_rfft<3, 8, true>, k_rfft<3, 8, false>); break;
+    case 4: launch_dir(k_rfft<4, 8, true>, k_rfft<4, 8, false>); break;
+    case 5: launch_dir(k_rfft<5, 8, true>, k_rfft<5, 8, false>); break;
+    case 6: launch_dir(k_rfft<6, 8, true>, k_rfft<6, 8, false>); break;
+    case 7: launch_dir(k_rfft<7, 8, true>, k_rfft<7, 8, false>); break;
+    case 8: launch_dir(k_rfft<8, 8, true>, k_rfft<8, 8, false>); break;
+    case 9: launch_dir(k_rfft<9, 8, true>, k_rfft<9, 8, false>); break;
+    default: launch_dir(k_rfft<10, 4, true>, k_rfft<10, 4, false>); break;
+  }
+  if (e != cudaSuccess) {
+    set_error("rfft kernel launch failed: %s", cudaGetErrorString(e));
     return PA_ECUDA;
   }
   count_launch();

@@ -243,4 +243,36 @@ PA_HD void butterfly(Line& x, int u, int L, int M, int sign, const Tw& tw) {
   for (int s = 0; s < R; ++s) x.put(base + s * Q, a[s]);
 }
 
+// ---- real lines through the complex core (rfft_ / brfft_, fft.cu) ----
+// A real line x of N = 2L points is read as the complex line z[n] = x[2n] + i x[2n+1] of L
+// points (its bytes, unchanged).  With Z = FFT_L(z) and w = W_N^k = exp(-2 pi i k / N):
+//   X[k]     = E + w O,   E = (Z[k] + conj Z[L-k]) / 2,   O = -i (Z[k] - conj Z[L-k]) / 2
+//   X[L - k] = conj(E - w O)
+// (indices of Z mod L).  One call per pair k = 0 ... L/2 yields all N/2 + 1 bins: k = 0 gives X[0]
+// and X[L] (both real), k = L/2 gives X[L/2] twice.
+PA_HD void rfft_post_pair(cplx zk, cplx zl, cplx w, cplx* xk, cplx* xl) {
+  const cplx e = cplx{0.5 * (zk.x + zl.x), 0.5 * (zk.y - zl.y)};
+  const cplx o = cplx{0.5 * (zk.y + zl.y), -0.5 * (zk.x - zl.x)};
+  const cplx wo = cmul(w, o);
+  *xk = cadd(e, wo);
+  *xl = cplx{e.x - wo.x, wo.y - e.y};
+}
+
+// Inverse of the above, unnormalised (FFTW's c2r): from the bins X[k], X[L-k] the pair of the
+// complex spectrum whose inverse L-point transform is z[n] = x[2n] + i x[2n+1], N x = brfft(X):
+//   F = X[k] + conj X[L-k],   G = (X[k] - conj X[L-k]) conj(w)
+//   Z[k] = F + i G,   Z[L-k] = conj F + i conj G
+// At k = 0 the partner is X[L]; the imaginary parts of X[0] and X[L] are dropped, as numpy and
+// FFTW drop them (a real signal cannot have them); Z[L] is Z[0] and is not produced.
+PA_HD void brfft_pre_pair(int k, cplx xk, cplx xl, cplx w, cplx* zk, cplx* zl) {
+  if (k == 0) {
+    xk.y = 0.0;
+    xl.y = 0.0;
+  }
+  const cplx f = cplx{xk.x + xl.x, xk.y - xl.y};
+  const cplx g = cmul(cplx{xk.x - xl.x, xk.y + xl.y}, cplx{w.x, -w.y});
+  *zk = cplx{f.x - g.y, f.y + g.x};
+  *zl = cplx{f.x + g.y, g.x - f.y};
+}
+
 }  // namespace pa_fft

@@ -265,6 +265,9 @@ pa_status host_chain_time_end(HostChain* c, float* ms);
 // together tile the destination box; srcs[i] = base pointer blocks[i] reads from
 pa_status unpack_fft(int nb, const BlockCopy* const* blocks, const void* const* srcs, void* dst,
                      int sign, void* stream);
+// real-line transforms (fft.cu): `nlines` dense, consecutive lines of N reals (src when forward,
+// dst when backward) <-> N/2 + 1 complex bins; N a power of two in 16..2048
+pa_status rfft_lines(int N, bool forward, i64 nlines, const void* src, void* dst, void* stream);
 
 // standalone flag step on `stream`: signal the n remote words (monotonic max,
 // release at system scope) and/or wait for the n local words to reach seq

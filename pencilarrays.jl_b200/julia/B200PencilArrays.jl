@@ -247,6 +247,29 @@ end
 fft_lines!(u::PencilArray{T,N,<:CuArray}; direction = :forward) where {T,N} =
     (Transpositions.transpose!(Transposition(u, u); fft = direction); u)
 
+# Real-to-complex 1-d FFT along the first memory dimension (not decomposed), step 1 of a
+# PencilFFTs real-input plan: `dest = rfft(src)` there.  `src` lives on a pencil of global size
+# (..., N, ...), `dest` on `Pencil(pencil(src); size_global = (..., N÷2+1, ...))`; N a power of
+# two in 16..2048.  `brfft!` is the unnormalised inverse (AbstractFFTs' `brfft`); it ignores the
+# imaginary parts of bins 1 and N÷2+1 and leaves `src` unmodified.  One kernel, no communication.
+function _rfft!(real::PencilArray{Float64,N,<:CuArray}, cplx::PencilArray{ComplexF64,N,<:CuArray},
+                flags::Cuint, src, dst) where {N}
+    H = handles(pencil(real).topology)
+    extra_dims(real) == extra_dims(cplx) ||
+        throw(ArgumentError("incompatible extra dimensions: $(extra_dims(real)) != $(extra_dims(cplx))"))
+    ex = Int64[extra_dims(real)...]
+    ptr_or_null(A) = isempty(A) ? C_NULL : devptr(A)
+    check(ccall((:pa_rfft, libpa), Cint,
+        (Ptr{Cvoid}, Ptr{Cvoid}, Cint, Ptr{Int64}, Cuint, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}),
+        pencil_handle(H, pencil(real)), pencil_handle(H, pencil(cplx)), length(ex), ex, flags,
+        ptr_or_null(parent(src)), ptr_or_null(parent(dst)), stream_ptr()))
+end
+
+rfft!(dest::PencilArray{ComplexF64,N,<:CuArray}, src::PencilArray{Float64,N,<:CuArray}) where {N} =
+    (_rfft!(src, dest, Cuint(8), src, dest); dest)       # PA_FFT_FORWARD
+brfft!(dest::PencilArray{Float64,N,<:CuArray}, src::PencilArray{ComplexF64,N,<:CuArray}) where {N} =
+    (_rfft!(dest, src, Cuint(16), src, dest); dest)      # PA_FFT_BACKWARD
+
 # ---- host arrays: a chain of transpositions on `Array`-backed data ------------------
 # pa_host_chain_*: one submit = upload, every transpose! on the device, download;
 # asynchronous, double-buffered (download of one submit || upload of the next).

@@ -329,6 +329,37 @@ def fft_(u: PencilArray, direction="forward"):
     return transpose_(t, fft=direction).Ao
 
 
+def _rfft(dest: PencilArray, src: PencilArray, forward: bool):
+    real, cplx = (src, dest) if forward else (dest, src)
+    if real.dtype != torch.float64 or cplx.dtype != torch.complex128:
+        raise ArgumentError(_lib.PA_EINVAL, "real array must be float64 and complex array "
+                            f"complex128: got {real.dtype} and {cplx.dtype}")
+    if src.extra_dims != dest.extra_dims:
+        raise ArgumentError(_lib.PA_EINVAL, "incompatible extra dimensions of PencilArrays: "
+                            f"{src.extra_dims} != {dest.extra_dims}")
+    ex = dest.extra_dims
+    flags = _lib.PA_FFT_FORWARD if forward else _lib.PA_FFT_BACKWARD
+    check(lib.pa_rfft(real.pencil._h, cplx.pencil._h, len(ex), i64arr(ex), flags,
+                      C.c_void_p(src.data_ptr() or None), C.c_void_p(dest.data_ptr() or None),
+                      _stream_ptr()))
+    return dest
+
+
+def rfft_(dest: PencilArray, src: PencilArray):
+    """Real-to-complex 1-d FFT along the first memory dimension (not decomposed): ``dest =
+    numpy.fft.rfft(src)`` there.  ``src``: float64 on a pencil of global size (..., N, ...);
+    ``dest``: complex128 on ``Pencil(src.pencil, size_global=(..., N//2+1, ...))``.  Step 1 of a
+    PencilFFTs real-input plan; the two complex steps are ``transpose_(t, fft=...)``."""
+    return _rfft(dest, src, True)
+
+
+def brfft_(dest: PencilArray, src: PencilArray):
+    """Inverse of :func:`rfft_`, unnormalised like FFTW's ``brfft``: ``dest = N *
+    numpy.fft.irfft(src, n=N)``.  The imaginary parts of bins 0 and N/2 are ignored and
+    ``src`` is left unmodified."""
+    return _rfft(dest, src, False)
+
+
 def transpose_host_(t: Transposition, host_src: torch.Tensor, host_dst: torch.Tensor):
     """``transpose!`` on HOST arrays through ``pa_transpose_host``: upload, kernels and
     download pipelined inside the library; returns when ``host_dst`` is valid.  Pin the
