@@ -329,6 +329,13 @@ pa_status pa_plan_set_recv_window(pa_plan* plan, int n, void* peer_recv_buf);
 pa_status pa_transpose(pa_plan* plan, pa_comm* comm, const void* src, void* dst,
                        unsigned flags, void* stream);
 pa_status pa_wait(pa_plan* plan, void* stream);
+/* Can pa_transpose fuse PA_FFT_FORWARD / PA_FFT_BACKWARD into this plan?  PA_OK, or
+ * PA_EINVAL with the reason in pa_last_error.  The answer depends on the global geometry
+ * only (element size, line length, the blocks every rank of the grid line gathers), so it
+ * is the same on every rank of the line: a caller may pick the fused or the separate
+ * transpose + transform up front.  pa_transpose asks the same question before it enqueues
+ * anything, and a refused fused transpose launches nothing.  Host-only; no device needed. */
+pa_status pa_plan_fft_check(const pa_plan* plan);
 /* same, with HOST arrays: H2D of `src`, transpose!, D2H of `dst`; blocks until
  * `host_dst` is valid.  Device staging is owned by the plan.  A purely local
  * transposition (nproc == 1 or dim == nothing) is cut along the source's outermost

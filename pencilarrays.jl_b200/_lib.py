@@ -120,6 +120,7 @@ SIGNATURES = {
     "pa_plan_set_recv_window": (C.c_int, [_P, C.c_int, _P]),
     "pa_transpose": (C.c_int, [_P, _P, _P, _P, C.c_uint, _P]),
     "pa_wait": (C.c_int, [_P, _P]),
+    "pa_plan_fft_check": (C.c_int, [_P]),
     "pa_transpose_host": (C.c_int, [_P, _P, _P, _P, C.c_uint]),
     "pa_rfft": (C.c_int, [_P, _P, C.c_int, _I64P, C.c_uint, _P, _P, _P]),
     "pa_host_chain_create": (C.c_int, [C.c_int, C.POINTER(_P), _P, C.POINTER(_P)]),

@@ -639,6 +639,16 @@ pa_status pa_transpose(pa_plan* plan, pa_comm* comm, const void* src, void* dst,
   })
 }
 
+pa_status pa_plan_fft_check(const pa_plan* plan) {
+  GUARD({
+    if (!plan) {
+      set_error("pa_plan_fft_check: null plan");
+      return PA_EINVAL;
+    }
+    return plan_fft_check(plan->p);
+  })
+}
+
 pa_status pa_wait(pa_plan* plan, void* stream) {
   if (!plan) return PA_EINVAL;
   return wait_sends(plan->p, stream);

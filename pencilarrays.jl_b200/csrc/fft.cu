@@ -356,12 +356,15 @@ static const cplx* twiddles(int L) {
   return d;
 }
 
-// `blocks[i]` moves block i from `srcs[i]` (recv_buf, or the src parent for the fused
-// self block) into `dst`; together they must tile the destination box.
-pa_status unpack_fft(int nb, const BlockCopy* const* blocks, const void* const* srcs, void* dst,
-                     int sign, void* stream) {
-  FftParams p;
+// Launch geometry of the fused kernel from the blocks of one rank (`blocks[i]` moves block i
+// from `srcs[i]` -- recv_buf, or the src parent for the fused self block -- into `dst`;
+// together they must tile the destination box), and every check of it.  srcs / dst may be
+// NULL: plan_fft_check runs this on the blocks a peer would see, without arrays.  *grid = 0:
+// nothing to do on this rank.
+static pa_status fft_geometry(int nb, const BlockCopy* const* blocks, const void* const* srcs,
+                              void* dst, FftParams& p, int* C_out, unsigned long long* grid_out) {
   memset(&p, 0, sizeof p);
+  *grid_out = 0;
   // the line dim: destination stride 1 (and extent > 1) in some block
   int jy = -1;
   for (int b = 0; b < nb && jy < 0; ++b)
@@ -370,6 +373,18 @@ pa_status unpack_fft(int nb, const BlockCopy* const* blocks, const void* const* 
         jy = i;
         break;
       }
+  // (every block one row long -- as many ranks as points: the dim of destination stride 1
+  //  along which the blocks lie side by side)
+  for (int i = 0; jy < 0 && nb > 0 && i < blocks[0]->nd_raw; ++i) {
+    i64 rows = 0;
+    bool unit = true;
+    for (int b = 0; b < nb; ++b)
+      if (blocks[b]->count > 0) {
+        unit = unit && blocks[b]->nd_raw == blocks[0]->nd_raw && blocks[b]->raw[i].ds == 1;
+        rows += blocks[b]->raw[i].e;
+      }
+    if (unit && rows > 1) jy = i;
+  }
   if (jy < 0) {
     set_error("fused FFT: the destination has no contiguous dimension longer than 1");
     return PA_EINVAL;
@@ -408,9 +423,15 @@ pa_status unpack_fft(int nb, const BlockCopy* const* blocks, const void* const* 
       set_error("fused FFT: unexpected source layout");
       return PA_EINVAL;
     }
-    if (linear && B.raw[0].ds != 1) return PA_EINVAL;
+    if (linear && B.raw[0].ds != 1) {
+      set_error("fused FFT: unexpected destination layout");
+      return PA_EINVAL;
+    }
     if (!ref) ref = &B;
-    if (B.nd_raw != ref->nd_raw) return PA_EINVAL;
+    if (B.nd_raw != ref->nd_raw) {
+      set_error("fused FFT: the blocks do not share their line set");
+      return PA_EINVAL;
+    }
     for (int i = 0; i < B.nd_raw; ++i)
       if (i != jy && (B.raw[i].e != ref->raw[i].e || B.raw[i].ds != ref->raw[i].ds)) {
         set_error("fused FFT: the blocks do not share their line set");
@@ -418,7 +439,7 @@ pa_status unpack_fft(int nb, const BlockCopy* const* blocks, const void* const* 
       }
     if (min_doff < 0 || B.dst_off < min_doff) min_doff = B.dst_off;
   }
-  if (!ref) return PA_OK;  // nothing to do on this rank
+  if (!ref) return PA_OK;  // nothing to do on this rank (*grid = 0)
   i64 L = 0;
   for (int b = 0; b < nb; ++b) {
     const BlockCopy& B = *blocks[b];
@@ -428,7 +449,7 @@ pa_status unpack_fft(int nb, const BlockCopy* const* blocks, const void* const* 
       return PA_EINVAL;
     }
     FftBlock& F = p.blk[p.nb++];
-    F.src = (const char*)srcs[b] + B.src_off * 16;
+    F.src = srcs ? (const char*)srcs[b] + B.src_off * 16 : nullptr;
     F.y0 = (int)(B.dst_off - min_doff);
     F.ey = (int)B.raw[jy].e;
     F.ssy = B.raw[jy].ss * 16;
@@ -458,38 +479,55 @@ pa_status unpack_fft(int nb, const BlockCopy* const* blocks, const void* const* 
       pos += s.second;
     }
   }
-  p.dst = (char*)dst + min_doff * 16;
+  p.dst = dst ? (char*)dst + min_doff * 16 : nullptr;
   p.linear = linear ? 1 : 0;
   p.ex = jx >= 0 ? ref->raw[jx].e : 1;
   p.dsx = jx >= 0 ? ref->raw[jx].ds * 16 : 16;
   p.no = 0;
   for (int i = 1; i < ref->nd_raw; ++i)
     if (i != jy && i != jx && ref->raw[i].e > 1) {
-      if (p.no >= FFT_MAXO) return PA_EINVAL;
+      if (p.no >= FFT_MAXO) {
+        set_error("fused FFT: more than %d outer dims", FFT_MAXO);
+        return PA_EINVAL;
+      }
       p.oe[p.no] = ref->raw[i].e;
       p.dso[p.no] = ref->raw[i].ds * 16;
       ++p.no;
     }
   p.L = (int)L;
   p.logL = logL;
-  p.sign = sign < 0 ? -1 : 1;
   p.pitch = pa_fft::padded_pitch((int)L);
-  p.tw = twiddles((int)L);
-  if (!p.tw) {
-    set_error("fused FFT: twiddle table allocation failed");
-    cudaGetLastError();
-    return PA_ENOMEM;
-  }
   // tunable "fft_lines" = 4: 4 lines per CTA also for 256- / 512-point lines (64-byte gathers,
   // first pass of radix 4 / 8 in registers, half the shared memory per CTA)
   const int C = (g_tun.fft_lines == 4 && logL >= 8) ? 4 : fft_lines(logL);
   p.tiles_x = (unsigned)((p.ex + C - 1) / C);
   unsigned long long grid = p.tiles_x;
   for (int i = 0; i < p.no; ++i) grid *= (unsigned long long)p.oe[i];
-  if (grid == 0) return PA_OK;
   if (grid > 0x7fffffffULL) {
     set_error("fused FFT: too many lines for one launch");
     return PA_EINVAL;
+  }
+  *C_out = C;
+  *grid_out = grid;
+  return PA_OK;
+}
+
+pa_status unpack_fft(int nb, const BlockCopy* const* blocks, const void* const* srcs, void* dst,
+                     int sign, void* stream) {
+  // (pa_transpose has already asked plan_fft_check, for every rank of the line, before it
+  //  enqueued anything: these checks only guard direct callers)
+  FftParams p;
+  int C = 0;
+  unsigned long long grid = 0;
+  pa_status s = fft_geometry(nb, blocks, srcs, dst, p, &C, &grid);
+  if (s != PA_OK || grid == 0) return s;
+  const int logL = p.logL;
+  p.sign = sign < 0 ? -1 : 1;
+  p.tw = twiddles(p.L);
+  if (!p.tw) {
+    set_error("fused FFT: twiddle table allocation failed");
+    cudaGetLastError();
+    return PA_ENOMEM;
   }
   const size_t smem = sizeof(cplx) * (size_t)C * p.pitch;
   cudaError_t e = cudaSuccess;
@@ -521,6 +559,68 @@ pa_status unpack_fft(int nb, const BlockCopy* const* blocks, const void* const* 
   }
   count_launch();
   return PA_OK;
+}
+
+// Can pa_transpose fuse the FFT into this plan's unpack?  Every rank of a grid line must
+// get the same answer: a rank that refused before the exchange while its peers went ahead
+// would leave them waiting on flags it never sets.  So the answer depends on the global
+// geometry only: the blocks that EVERY rank of the line would gather -- each rank's plan
+// rebuilt from the pencils with that rank's coordinates -- with the self block read from src
+// and staged through recv_buf alike.  Cached per plan (and per value of tunable fft_lines).
+pa_status plan_fft_check(Plan* P) {
+  if (P->fft_check_lines == g_tun.fft_lines) {
+    if (P->fft_check != PA_OK) set_error("%s", P->fft_check_err.c_str());
+    return P->fft_check;
+  }
+  auto verdict = [&](pa_status s) {
+    P->fft_check = s;
+    P->fft_check_err = s == PA_OK ? std::string() : std::string(last_error());
+    P->fft_check_lines = g_tun.fft_lines;
+    return s;
+  };
+  if (P->elsize != 16) {
+    set_error("fused FFT: ComplexF64 (16-byte) elements only");
+    return verdict(PA_EINVAL);
+  }
+  FftParams p;
+  int C = 0;
+  unsigned long long grid = 0;
+  if (P->dim < 0 || P->nproc == 1) {
+    const BlockCopy* b = &P->self_fused;
+    return verdict(fft_geometry(1, &b, nullptr, nullptr, p, &C, &grid));
+  }
+  for (int n = 0; n < P->nproc; ++n) {
+    std::unique_ptr<Plan> hold;
+    const Plan* Q = P;
+    if (n != P->self_index) {
+      auto topo = std::make_shared<Topology>(*P->pin->topo);
+      topo->coords[P->dim] = n;
+      topo->rank = topo->rank_of(topo->coords);
+      auto pin = std::make_shared<Pencil>(*P->pin);
+      auto pout = std::make_shared<Pencil>(*P->pout);
+      pin->topo = topo;
+      pout->topo = topo;
+      Plan* q = nullptr;
+      pa_status s = build_plan(pin, pout, P->n_extra, P->extra, P->elsize, P->method, &q);
+      if (s != PA_OK) return verdict(s);
+      hold.reset(q);
+      Q = q;
+    }
+    for (int staged_self = 0; staged_self < 2; ++staged_self) {
+      std::vector<const BlockCopy*> bl;
+      for (int k = 0; k < Q->nproc; ++k)
+        bl.push_back(k == Q->self_index && !staged_self ? &Q->self_fused : &Q->peers[k].unpack);
+      pa_status s = fft_geometry(Q->nproc, bl.data(), nullptr, nullptr, p, &C, &grid);
+      if (s != PA_OK) {
+        if (n != P->self_index) {
+          const std::string why = last_error();
+          set_error("%s (on rank %d of the grid line)", why.c_str(), n + 1);
+        }
+        return verdict(s);
+      }
+    }
+  }
+  return verdict(PA_OK);
 }
 
 pa_status rfft_lines(int N, bool forward, i64 nlines, const void* src, void* dst, void* stream) {

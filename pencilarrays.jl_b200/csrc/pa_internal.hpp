@@ -220,6 +220,10 @@ struct Plan {
   void* h_src_dev = nullptr;
   void* h_dst_dev = nullptr;
   i64 h_src_cap = 0, h_dst_cap = 0;
+  // cached answer of plan_fft_check (valid while tunable fft_lines == fft_check_lines)
+  int fft_check_lines = -1;
+  pa_status fft_check = PA_OK;
+  std::string fft_check_err;
   ~Plan();
 };
 
@@ -265,6 +269,9 @@ pa_status host_chain_time_end(HostChain* c, float* ms);
 // together tile the destination box; srcs[i] = base pointer blocks[i] reads from
 pa_status unpack_fft(int nb, const BlockCopy* const* blocks, const void* const* srcs, void* dst,
                      int sign, void* stream);
+// can pa_transpose fuse a FFT into this plan's unpack?  The same answer on every rank of the
+// grid line (global geometry only); PA_EINVAL + last_error otherwise.  No device call.
+pa_status plan_fft_check(Plan* plan);
 // real-line transforms (fft.cu): `nlines` dense, consecutive lines of N reals (src when forward,
 // dst when backward) <-> N/2 + 1 complex bins; N a power of two in 16..2048
 pa_status rfft_lines(int N, bool forward, i64 nlines, const void* src, void* dst, void* stream);

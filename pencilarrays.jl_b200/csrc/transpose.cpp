@@ -1072,20 +1072,23 @@ static pa_status staged(Plan* P, Comm* comm, const void* src, void* dst, unsigne
 
 pa_status transpose(Plan* P, Comm* comm, const void* src, void* dst, unsigned flags,
                     void* stream) {
-  RC(ensure_state(P));
-  TransposeState& S = *P->st;
-  cudaStream_t user = (cudaStream_t)stream;
-  const i64 ES = P->elsize;
-  const bool timing = S.timing;
   // a rank may own nothing (more processes than points, Pencils.jl:193-218): its
   // empty arrays have no storage, yet it takes part in the exchange
   if ((!src && P->length_in > 0) || (!dst && P->length_out > 0)) {
     set_error("pa_transpose: null array pointer");
     return PA_EINVAL;
   }
+  const int fft_sign = (flags & PA_FFT_FORWARD) ? -1 : ((flags & PA_FFT_BACKWARD) ? 1 : 0);
+  // a fused FFT this plan cannot run is refused before anything is enqueued -- and on every
+  // rank of the line alike (the peers of a refusing rank must not start the exchange)
+  if (fft_sign) RC(plan_fft_check(P));
+  RC(ensure_state(P));
+  TransposeState& S = *P->st;
+  cudaStream_t user = (cudaStream_t)stream;
+  const i64 ES = P->elsize;
+  const bool timing = S.timing;
   if (timing) CU(cudaEventRecord(S.t[0], user));
 
-  const int fft_sign = (flags & PA_FFT_FORWARD) ? -1 : ((flags & PA_FFT_BACKWARD) ? 1 : 0);
   // src and dst may not alias -- except for the plain in-place transform along the contiguous
   // dim (same pencil on both sides, src == dst): a CTA reads its lines completely before it
   // writes them back

@@ -242,6 +242,12 @@ function Transpositions.transpose!(t::DeviceTransposition; waitall = true, fft =
     t
 end
 
+# Whether `transpose!(t; fft)` can fuse the unpack and the FFT (pa_plan_fft_check).  The same
+# answer on every rank of the grid line (global geometry only): choose the fused or the separate
+# transpose + transform up front.
+fft_fusable(t::DeviceTransposition) =
+    ccall((:pa_plan_fft_check, libpa), Cint, (Ptr{Cvoid},), first(plan_handle(t))) == 0
+
 # In-place 1-d FFT of `u` along its contiguous dimension (same kernel, no transposition): with
 # the two fused transposes this is a whole PencilFFTs-style 3-d transform in three kernels.
 fft_lines!(u::PencilArray{T,N,<:CuArray}; direction = :forward) where {T,N} =

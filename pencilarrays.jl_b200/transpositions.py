@@ -279,6 +279,13 @@ class Transposition:
     def enable_timing(self, on=True):
         check(lib.pa_plan_enable_timing(self._plan.h, 1 if on else 0))
 
+    def fft_fusable(self) -> bool:
+        """Whether ``transpose_(self, fft=...)`` can run the unpack and the 1-d FFT as one
+        kernel (``pa_plan_fft_check``).  The answer depends on the global geometry only, so it
+        is the same on every rank of the grid line; when it is False, transpose and transform
+        separately."""
+        return lib.pa_plan_fft_check(self._plan.h) == _lib.PA_OK
+
 
 def Waitall(t: Transposition):
     """``MPI.Waitall(t::Transposition)`` (:127-130): sends done => send_buf reusable."""

@@ -197,11 +197,28 @@ def main():
                             out = pa.PencilArray.undef(tdt, pens[k], *extra)
                             t = pa.Transposition(out, src, method=method)
                             if not ok_shape:
+                                # refused on every rank before anything is enqueued: no launch,
+                                # dst untouched, and the plan still transposes bit-exactly
+                                assert not t.fft_fusable(), (case["name"], k, rank)
+                                out.data.view(torch.uint8).fill_(0x3C)
+                                torch.cuda.synchronize()
+                                before = out.data.clone()
+                                n0 = pa.launch_count()
                                 try:
                                     pa.transpose_(t, fft=direction)
                                     raise AssertionError("fused FFT accepted an unsupported shape")
                                 except pa.ArgumentError:
-                                    continue
+                                    pass
+                                torch.cuda.synchronize()
+                                assert pa.launch_count() == n0, (case["name"], k, rank, method)
+                                assert torch.equal(out.data.view(torch.uint8), before.view(torch.uint8))
+                                pa.transpose_(t)
+                                torch.cuda.synchronize()
+                                got = np.ascontiguousarray(out.data.cpu().numpy()).reshape(-1)
+                                assert got.tobytes() == np.ascontiguousarray(
+                                    a_out.data.reshape(-1, order="F")).tobytes(), \
+                                    ("plain after refusal", case["name"], k, rank, method)
+                                continue
                             pa.transpose_(t, fft=direction)
                             torch.cuda.synchronize()
                             ref = np.fft.fft(a_out.data, axis=0) if direction == "forward" else \
