@@ -400,9 +400,11 @@ pa_status pa_host_chain_time_end(pa_host_chain* c, float* ms);
  * `offset` = byte offset of the dataset in the file (MPIFile position, :159-164).
  * Every rank calls these for its own part (no collective: ranks pwrite / pread
  * disjoint byte ranges of the same file); the device array moves through a double-
- * buffered pinned staging area on a stream of the library's own: the calls block until
- * the transfer is complete and are NOT ordered against work queued on the caller's
- * streams -- synchronise those first.  The JSON sidecar (:194-211) is written by the host
+ * buffered pinned staging area on a stream of the library's own.  Each call first waits
+ * for ALL device work queued so far in the process, on any stream (cudaDeviceSynchronize:
+ * a kernel may still be writing the array that is about to be written, or reading the one
+ * about to be read), and returns once the transfer is complete, so work queued afterwards
+ * on any stream sees the read data.  The JSON sidecar (:194-211) is written by the host
  * veneer (Julia: the reference's own add_metadata; Python mirror: pencilio.py).     */
 pa_status pa_io_sizes(const pa_pencil* p, int n_extra, const int64_t* extra_dims, int elsize,
                       int chunks, int64_t* global_bytes, int64_t* local_bytes, int64_t* nruns,

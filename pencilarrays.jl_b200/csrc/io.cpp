@@ -208,6 +208,16 @@ pa_status io_transfer(const Pencil& P, int n_extra, const i64* extra, int elsize
     close(fd);
     return PA_OK;
   }
+  // Work queued on any stream of the process may still write the array (before a write) or
+  // read it (before a read), and the copies below run on a stream of their own: wait for all
+  // of it.  Both calls block until the transfer is done anyway.
+  const cudaError_t prior = cudaDeviceSynchronize();
+  if (prior != cudaSuccess) {
+    close(fd);
+    cudaGetLastError();
+    set_error("pa_io: prior device work failed: %s", cudaGetErrorString(prior));
+    return PA_ECUDA;
+  }
   // pieces of whole runs, about 32 MiB each, through two pinned buffers
   const i64 target = 32ll << 20;
   const i64 runs_per_piece = std::max<i64>(1, std::min<i64>(L.nruns, target / std::max<i64>(1, L.run_bytes)));

@@ -479,6 +479,25 @@ static pa_status buffer_events(Buffers& B, cudaEvent_t* comm_ev, cudaEvent_t* un
   return PA_OK;
 }
 
+// A one-rank use of the recv arena on the caller's stream (the nproc == 1 staged self block,
+// the aliased local permutation's scratch): it starts after the last exchange into the arena
+// and the last unpack out of it, whatever stream those ran on ...
+static pa_status arena_acquire(Buffers& B, cudaStream_t user) {
+  cudaEvent_t comm_ev, unpack_ev;
+  RC(buffer_events(B, &comm_ev, &unpack_ev));
+  CU(cudaStreamWaitEvent(user, comm_ev, 0));
+  CU(cudaStreamWaitEvent(user, unpack_ev, 0));
+  return PA_OK;
+}
+
+// ... and the next user of the arena waits for it: both events move past its last read (the
+// caller's stream already waited for their previous records, so the chain stays transitive)
+static pa_status arena_release(Buffers& B, cudaStream_t user) {
+  CU(cudaEventRecord((cudaEvent_t)B.comm_done_event, user));
+  CU(cudaEventRecord((cudaEvent_t)B.unpack_done_event, user));
+  return PA_OK;
+}
+
 // ---- per-plan stream/event state --------------------------------------------
 struct TransposeState {
   cudaStream_t pack_s = nullptr, comm_s = nullptr, unpack_s = nullptr;
@@ -1114,11 +1133,15 @@ pa_status transpose(Plan* P, Comm* comm, const void* src, void* dst, unsigned fl
     void* scratch = nullptr;
     const i64 bytes = P->length_out * ES;
     if (bytes == 0) return PA_OK;
-    if (!P->same_perm && ranges_overlap(src, bytes, dst, bytes)) {
-      RC(P->pin->bufs->reserve(0, std::max<i64>(1, bytes)));  // reuses Pi.recv_buf (:255)
-      scratch = P->pin->bufs->recv;
+    const bool staged_local = !P->same_perm && ranges_overlap(src, bytes, dst, bytes);
+    if (staged_local) {
+      Buffers& Bi = *P->pin->bufs;
+      RC(Bi.reserve(0, std::max<i64>(1, bytes)));  // reuses Pi.recv_buf (:255)
+      scratch = Bi.recv;
+      RC(arena_acquire(Bi, user));
     }
     RC(local_transpose(P, src, dst, scratch, user));
+    if (staged_local) RC(arena_release(*P->pin->bufs, user));
     if (timing) {
       CU(cudaEventRecord(S.t[6], user));
       S.timed_once = true;
@@ -1157,8 +1180,10 @@ pa_status transpose(Plan* P, Comm* comm, const void* src, void* dst, unsigned fl
     // only the self block: no exchange, everything on the caller's stream
     if (stage_self) {
       char* rbuf = (char*)B.recv;
+      RC(arena_acquire(B, user));
       RC(launch_block(self.pack, src, rbuf, user, nullptr, 0, true));
       RC(launch_block(self.unpack, rbuf, dst, user, nullptr, 0, true));
+      RC(arena_release(B, user));
     } else {
       RC(launch_block(P->self_fused, src, dst, user, nullptr, 0, true));
     }

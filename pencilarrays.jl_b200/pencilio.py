@@ -101,7 +101,6 @@ class MPIFile:
             raise ArgumentError(_lib.PA_EINVAL, "file was not opened for writing")
         offset = self.position
         for u in _collection(x):
-            torch.cuda.current_stream().synchronize()  # the array must be final before it is read
             check(lib.pa_io_write(u.pencil._h, len(u.extra_dims), i64arr(u.extra_dims), u.elsize,
                                   1 if chunks else 0, C.c_void_p(u.data_ptr() or None),
                                   self.filename.encode(), offset))
@@ -176,7 +175,6 @@ def read_(ff: MPIFile, x, name=None, *, offset=0, collective=True):
         if sizeof_global(x) > os.path.getsize(ff.filename):
             raise RuntimeError("attempt to read file without JSON metadata failed: the file size is "
                                "inferior to the expected dataset size")
-    torch.cuda.current_stream().synchronize()  # queued work on the arrays (fills, kernels) comes first
     for u in _collection(x):
         check(lib.pa_io_read(u.pencil._h, len(u.extra_dims), i64arr(u.extra_dims), u.elsize,
                              1 if chunks else 0, C.c_void_p(u.data_ptr() or None),

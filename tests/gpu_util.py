@@ -32,6 +32,45 @@ def ptr(t: torch.Tensor, byte_offset: int = 0):
     return C.c_void_p(t.data_ptr() + byte_offset)
 
 
+# ---- ordering checks: hold a stream, then produce the input behind the hold --------------
+HOLD_MS = 50.0
+_hold_cycles = None
+
+
+def hold_cycles() -> int:
+    """Cycles of `torch.cuda._sleep` that spin for about HOLD_MS, calibrated once with CUDA
+    events (the SM clock is not assumed); never more than 1e8 (0.1 s at 1 GHz)."""
+    global _hold_cycles
+    if _hold_cycles is None:
+        torch.cuda._sleep(1000)  # (the first launch loads the kernel)
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        n = 1 << 22
+        a.record()
+        torch.cuda._sleep(n)
+        b.record()
+        b.synchronize()
+        ms = max(a.elapsed_time(b), 1e-3)
+        _hold_cycles = min(int(n * HOLD_MS / ms), 100_000_000)
+    return _hold_cycles
+
+
+def timing_event() -> torch.cuda.Event:
+    """A timing event recorded on the current stream."""
+    ev = torch.cuda.Event(enable_timing=True)
+    ev.record()
+    return ev
+
+
+def hold() -> torch.cuda.Event:
+    """One bounded spin (about HOLD_MS) on the current stream; returns the event `held`,
+    recorded right after it.  Work enqueued on this stream afterwards runs only once the spin
+    is over, so a library call that is not ordered behind the caller's stream reads whatever
+    the input held before, and `held.query()` is still False when a call that does not
+    synchronise the host returns."""
+    torch.cuda._sleep(hold_cycles())
+    return timing_event()
+
+
 def box_copy(extent, sstr, dstr, elsize, src: torch.Tensor, dst: torch.Tensor, src_off=0,
              dst_off=0):
     d = BlockDesc()
