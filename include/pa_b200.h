@@ -73,14 +73,21 @@ typedef enum pa_method {
  * along the destination's contiguous dimension (the one that has just become local:
  * the reason the pencil is permuted, docs/src/Pencils.md:210-214) run as ONE kernel --
  * `dst` receives fft(transposed array) (forward: exp(-2*pi*i*jk/n); backward: the
- * unnormalised inverse, as FFTW / PencilFFTs).  ComplexF64, power-of-two lines of
- * 8..1024 points, staged methods or local transposes, src and dst not aliased;
+ * unnormalised inverse, as FFTW / PencilFFTs).  ComplexF64 (or ComplexF32 with
+ * PA_FFT_F32), power-of-two lines of 8..1024 points, staged methods or local
+ * transposes, src and dst not aliased;
  * PA_EINVAL otherwise (transpose, then transform, separately).  A plan between
  * IDENTICAL pencils with src == dst is the plain in-place transform along the
  * contiguous dim -- the first step of a PencilFFTs-style 3-d transform, whose other
  * two steps are the fused transposes.                                               */
 #define PA_FFT_FORWARD  8u
 #define PA_FFT_BACKWARD 16u
+/* Single precision, with PA_FFT_FORWARD / PA_FFT_BACKWARD only: on pa_transpose the
+ * elements are ComplexF32 (the plan's elsize must be 8; elsize 16 is PA_EINVAL), on
+ * pa_rfft the pair is Float32 <-> ComplexF32.  Storage and arithmetic are fp32.  The
+ * element size alone never selects it: without this flag an elsize-8 plan is refused
+ * for a fused FFT as before.                                                         */
+#define PA_FFT_F32      32u
 
 typedef struct pa_topology pa_topology; /* MPITopology   (MPITopologies.jl:72-119) */
 typedef struct pa_pencil pa_pencil;     /* Pencil        (Pencils.jl:151-272)      */
@@ -336,6 +343,10 @@ pa_status pa_wait(pa_plan* plan, void* stream);
  * transpose + transform up front.  pa_transpose asks the same question before it enqueues
  * anything, and a refused fused transpose launches nothing.  Host-only; no device needed. */
 pa_status pa_plan_fft_check(const pa_plan* plan);
+/* same question for the precision in `flags` (the pa_transpose flags of the fused call;
+ * only PA_FFT_F32 matters): PA_FFT_F32 set asks about ComplexF32, unset about
+ * ComplexF64 like pa_plan_fft_check.  Each precision's verdict is cached on its own. */
+pa_status pa_plan_fft_check_ex(const pa_plan* plan, unsigned flags);
 /* same, with HOST arrays: H2D of `src`, transpose!, D2H of `dst`; blocks until
  * `host_dst` is valid.  Device staging is owned by the plan.  A purely local
  * transposition (nproc == 1 or dim == nothing) is cut along the source's outermost
@@ -355,6 +366,7 @@ pa_status pa_transpose_host(pa_plan* plan, pa_comm* comm, const void* host_src,
  *   PA_FFT_BACKWARD: src = ComplexF64, dst = Float64, dst = N * irfft(src, N) -- unnormalised
  *                    like FFTW's brfft; the imaginary parts of bins 0 and N/2 are ignored and
  *                    `src` is left unmodified.
+ *   either | PA_FFT_F32: the same with Float32 / ComplexF32 arrays and fp32 arithmetic.
  * N: power of two in 16..2048.  One kernel per call, local to the rank (no communication);
  * extra dims are batched.  Arrays dense (parent layout), 16-byte aligned, not overlapping;
  * NULL allowed where the local array is empty.  Ordered on `stream` like pa_transpose.

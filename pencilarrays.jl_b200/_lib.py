@@ -27,6 +27,7 @@ PA_NO_OVERLAP = 2
 PA_STAGE_SELF = 4
 PA_FFT_FORWARD = 8
 PA_FFT_BACKWARD = 16
+PA_FFT_F32 = 32
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libpa_b200.so")
@@ -121,6 +122,7 @@ SIGNATURES = {
     "pa_transpose": (C.c_int, [_P, _P, _P, _P, C.c_uint, _P]),
     "pa_wait": (C.c_int, [_P, _P]),
     "pa_plan_fft_check": (C.c_int, [_P]),
+    "pa_plan_fft_check_ex": (C.c_int, [_P, C.c_uint]),
     "pa_transpose_host": (C.c_int, [_P, _P, _P, _P, C.c_uint]),
     "pa_rfft": (C.c_int, [_P, _P, C.c_int, _I64P, C.c_uint, _P, _P, _P]),
     "pa_host_chain_create": (C.c_int, [C.c_int, C.POINTER(_P), _P, C.POINTER(_P)]),

@@ -645,7 +645,17 @@ pa_status pa_plan_fft_check(const pa_plan* plan) {
       set_error("pa_plan_fft_check: null plan");
       return PA_EINVAL;
     }
-    return plan_fft_check(plan->p);
+    return plan_fft_check(plan->p, false);
+  })
+}
+
+pa_status pa_plan_fft_check_ex(const pa_plan* plan, unsigned flags) {
+  GUARD({
+    if (!plan) {
+      set_error("pa_plan_fft_check_ex: null plan");
+      return PA_EINVAL;
+    }
+    return plan_fft_check(plan->p, (flags & PA_FFT_F32) != 0);
   })
 }
 
@@ -705,8 +715,10 @@ static pa_status rfft_checks(const pa_pencil* real, const pa_pencil* cplx, int n
               "N/2+1 = %lld", (long long)Cp.size_global[ax], (long long)(N / 2 + 1));
     return PA_EINCOMPAT;
   }
-  if (flags != PA_FFT_FORWARD && flags != PA_FFT_BACKWARD) {
-    set_error("pa_rfft: flags must be exactly PA_FFT_FORWARD or PA_FFT_BACKWARD");
+  const unsigned dir = flags & ~PA_FFT_F32;
+  if (dir != PA_FFT_FORWARD && dir != PA_FFT_BACKWARD) {
+    set_error("pa_rfft: flags must be exactly PA_FFT_FORWARD or PA_FFT_BACKWARD, optionally "
+              "with PA_FFT_F32");
     return PA_EINVAL;
   }
   if (N < 16 || N > 2048 || (N & (N - 1))) {
@@ -730,8 +742,9 @@ static pa_status rfft_checks(const pa_pencil* real, const pa_pencil* cplx, int n
     }
     nlines *= extra_dims[i];
   }
-  const bool fwd = flags == PA_FFT_FORWARD;
-  const i64 real_bytes = nlines * N * 8, cplx_bytes = nlines * (N / 2 + 1) * 16;
+  const bool fwd = dir == PA_FFT_FORWARD;
+  const i64 rs = (flags & PA_FFT_F32) ? 4 : 8;  // bytes of a real element; a complex one is 2 rs
+  const i64 real_bytes = nlines * N * rs, cplx_bytes = nlines * (N / 2 + 1) * 2 * rs;
   const i64 src_bytes = fwd ? real_bytes : cplx_bytes, dst_bytes = fwd ? cplx_bytes : real_bytes;
   if (nlines > 0) {
     if (!src || !dst) {
@@ -763,7 +776,8 @@ pa_status pa_rfft(const pa_pencil* real, const pa_pencil* cplx, int n_extra,
     if (s != PA_OK) return s;
     s = need_gpu();
     if (s != PA_OK) return s;
-    return rfft_lines(N, flags == PA_FFT_FORWARD, nlines, src, dst, stream);
+    return rfft_lines(N, (flags & ~PA_FFT_F32) == PA_FFT_FORWARD, (flags & PA_FFT_F32) != 0, nlines,
+                      src, dst, stream);
   })
 }
 

@@ -22,12 +22,17 @@
 // HBM traffic: 2 * s * n bytes for n elements, the same as the plain unpack.
 // ComplexF64 lines of 8 ... 1024 points (power of two); anything else is refused
 // (PA_EINVAL) and the caller transposes and transforms separately.
+//
+// Single precision (PA_FFT_F32, DESIGN §3d): the same kernels instantiated for float --
+// ComplexF32 elements, fp32 arithmetic, an fp32 twiddle table rounded from the same
+// long-double values -- with 16 lines per CTA (128-byte gathers again), 8 for 1024 points.
 #include <cuda_runtime.h>
 
 #include <algorithm>
 #include <cmath>
 #include <map>
 #include <mutex>
+#include <tuple>
 #include <vector>
 
 // twiddles: one table lookup per butterfly, the other powers by squaring / products (the
@@ -41,6 +46,21 @@
 namespace pa {
 
 using pa_fft::cplx;
+using pa_fft::cplx_t;
+
+// the 64-bit (float2) or 128-bit (double2) vector of one complex element
+template <class T>
+struct Vec2;
+template <>
+struct Vec2<double> {
+  using type = double2;
+};
+template <>
+struct Vec2<float> {
+  using type = float2;
+};
+__device__ __forceinline__ double2 vec2(double x, double y) { return make_double2(x, y); }
+__device__ __forceinline__ float2 vec2(float x, float y) { return make_float2(x, y); }
 
 constexpr int FFT_MAXB = 8;   // blocks gathered by one launch (ranks of a grid line on one box)
 constexpr int FFT_MAXO = PA_MAX_DIMS - 2;
@@ -48,6 +68,9 @@ constexpr int FFT_THREADS = 256;
 // lines per CTA: 8 (128-byte gathers); 4 for 1024-point lines so that three CTAs still
 // share an SM's shared memory (75 KB each)
 constexpr int fft_lines(int logL) { return logL >= 10 ? 4 : 8; }
+// single precision: twice as many lines in the same shared memory -- 16 (128-byte gathers of
+// 8-byte elements) up to 512 points, 8 for 1024 points
+constexpr int fft_lines_f32(int logL) { return logL >= 10 ? 8 : 16; }
 
 struct FftBlock {
   const char* src;  // block origin
@@ -67,14 +90,15 @@ struct FftParams {
   int L, logL, sign, pitch;
   int linear;  // the lines are contiguous in the source too (no transposition): consecutive
                // threads then walk along a line instead of across the columns
-  const cplx* tw;
+  const void* tw;  // twiddle table of the kernel's precision (cplx or cplxf)
   unsigned tiles_x;
 };
 
+template <class T>
 struct SmLine {
-  cplx* p;
-  __device__ __forceinline__ cplx get(int i) const { return p[pa_fft::pad_index(i)]; }
-  __device__ __forceinline__ void put(int i, cplx v) { p[pa_fft::pad_index(i)] = v; }
+  cplx_t<T>* p;
+  __device__ __forceinline__ cplx_t<T> get(int i) const { return p[pa_fft::pad_index(i)]; }
+  __device__ __forceinline__ void put(int i, cplx_t<T> v) { p[pa_fft::pad_index(i)] = v; }
 };
 
 // radix of the pass that starts at sub-length 2^LOGM (the odd bits go first: radices_of)
@@ -83,8 +107,8 @@ struct PassRadix {
   static constexpr int LOGR = (LOGM % 3 == 0) ? 3 : (LOGM % 3);
 };
 
-template <int LOGL, int LOGM, int C, class Tw>
-__device__ __forceinline__ void fft_passes(cplx* sm, int pitch, int ncol, int sign, const Tw& tw) {
+template <int LOGL, int LOGM, int C, class T, class Tw>
+__device__ __forceinline__ void fft_passes(cplx_t<T>* sm, int pitch, int ncol, int sign, const Tw& tw) {
   if constexpr (LOGM > 0) {
     constexpr int LOGR = PassRadix<LOGM>::LOGR;
     constexpr int R = 1 << LOGR, L = 1 << LOGL, M = 1 << LOGM;
@@ -95,7 +119,7 @@ __device__ __forceinline__ void fft_passes(cplx* sm, int pitch, int ncol, int si
       const int w = w0 + (int)threadIdx.x;
       const int c = w / PER_LINE, u = w % PER_LINE;
       if (w < TOTAL && c < ncol) {
-        SmLine x{sm + c * pitch};
+        SmLine<T> x{sm + c * pitch};
         pa_fft::butterfly<R>(x, u, L, M, sign, tw);
       }
     }
@@ -115,11 +139,13 @@ __device__ __forceinline__ int fft_pos(int k) {
   }
 }
 
-template <int LOGL, int C>
+template <int LOGL, int C, class T>
 __global__ void __launch_bounds__(FFT_THREADS) k_unpack_fft(const __grid_constant__ FftParams p) {
+  using cx = cplx_t<T>;
+  using V = typename Vec2<T>::type;
   constexpr int L = 1 << LOGL;
   extern __shared__ __align__(16) unsigned char fft_smem[];
-  cplx* sm = reinterpret_cast<cplx*>(fft_smem);
+  cx* sm = reinterpret_cast<cx*>(fft_smem);
   const int t = threadIdx.x;
   unsigned long long bid = blockIdx.x;
   const long long x0 = (long long)(bid % p.tiles_x) * C;
@@ -140,31 +166,34 @@ __global__ void __launch_bounds__(FFT_THREADS) k_unpack_fft(const __grid_constan
   const int ncol = (int)((p.ex - x0) < C ? (p.ex - x0) : C);
   const int pitch = p.pitch;
 
-  // ---- gather (+ first pass): C threads read C consecutive columns (C x 16 B) of one
+  // ---- gather (+ first pass): C threads read C consecutive columns (C x sizeof(cx)) of one
   //      source row.  A thread owns the rows r, r + RS, r + 2 RS, ... of its column: exactly
   //      the inputs of one butterfly of a first pass of radix R1 = L / RS -- so that pass runs
   //      on the values as they arrive from HBM, before they ever touch shared memory ----
   constexpr int RS = FFT_THREADS / C;  // rows per sweep
-  constexpr int LOGRS = (C == 8) ? 5 : 6;
+  constexpr int LOGRS = (C == 16) ? 4 : (C == 8) ? 5 : 6;
   static_assert((1 << LOGRS) == RS, "rows per sweep");
   // (only for 1024-point lines, where shared memory bounds the CTAs per SM; for 512-point
-  //  lines the radix-16 butterfly's registers would cost the third resident CTA)
-  constexpr int LOGR1 = (C == 4 && LOGL > LOGRS) ? (LOGL - LOGRS) : 0;
+  //  lines the radix-16 butterfly's registers would cost the third resident CTA.  Single
+  //  precision holds 8 1024-point lines: a sweep of 32 rows would need a radix-32 pass, which
+  //  does not exist, so every pass runs in shared memory there)
+  constexpr int LOGR1 = (sizeof(T) == 8 && C == 4 && LOGL > LOGRS) ? (LOGL - LOGRS) : 0;
   static_assert(LOGR1 == 0 || LOGL - LOGR1 == LOGRS, "first-pass stride must equal the sweep");
-  const cplx* twp = p.tw;
+  static_assert(LOGR1 <= 4, "the register first pass is at most radix 16");
+  const V* twp = reinterpret_cast<const V*>(p.tw);
   auto tw = [twp](int i) {
-    const double2 w = __ldg(reinterpret_cast<const double2*>(twp) + i);
-    return cplx{w.x, w.y};
+    const V w = __ldg(twp + i);
+    return cx{w.x, w.y};
   };
   {
     // transposing gather: C consecutive threads read C consecutive columns of one source row;
     // linear gather (lines contiguous in the source): consecutive threads read along a line
     const int c = p.linear ? t / RS : t % C, r = p.linear ? t % RS : t / C;
-    cplx* line = sm + c * pitch;
+    cx* line = sm + c * pitch;
     if constexpr (LOGR1 > 0) {
       constexpr int R1 = 1 << LOGR1;
       if (c < ncol) {
-        double2 v[R1];
+        V v[R1];
 #pragma unroll
         for (int q = 0; q < R1; ++q) {
           const int y = r + q * RS;
@@ -174,11 +203,11 @@ __global__ void __launch_bounds__(FFT_THREADS) k_unpack_fft(const __grid_constan
             if (b < p.nb && y >= p.blk[b].y0 && y < p.blk[b].y0 + p.blk[b].ey)
               s = p.blk[b].src + so_off[b] + (long long)(y - p.blk[b].y0) * p.blk[b].ssy +
                   (x0 + c) * p.blk[b].ssx;
-          v[q] = __ldcs(reinterpret_cast<const double2*>(s));
+          v[q] = __ldcs(reinterpret_cast<const V*>(s));
         }
-        cplx a[R1];
+        cx a[R1];
 #pragma unroll
-        for (int q = 0; q < R1; ++q) a[q] = cplx{v[q].x, v[q].y};
+        for (int q = 0; q < R1; ++q) a[q] = cx{v[q].x, v[q].y};
         pa_fft::butterfly_regs<R1>(a, r, L, L, p.sign, tw);
 #pragma unroll
         for (int q = 0; q < R1; ++q) line[pa_fft::pad_index(r + q * RS)] = a[q];
@@ -193,16 +222,16 @@ __global__ void __launch_bounds__(FFT_THREADS) k_unpack_fft(const __grid_constan
           const int ey = B.ey, y0 = B.y0;
           const long long ssy = B.ssy;
           for (int y = r; y < ey; y += U * RS) {
-            double2 v[U];
+            V v[U];
 #pragma unroll
             for (int k = 0; k < U; ++k) {
               const int yy = y + k * RS;
-              if (c < ncol && yy < ey) v[k] = __ldcs(reinterpret_cast<const double2*>(s + (long long)yy * ssy));
+              if (c < ncol && yy < ey) v[k] = __ldcs(reinterpret_cast<const V*>(s + (long long)yy * ssy));
             }
 #pragma unroll
             for (int k = 0; k < U; ++k) {
               const int yy = y + k * RS;
-              if (c < ncol && yy < ey) line[pa_fft::pad_index(y0 + yy)] = cplx{v[k].x, v[k].y};
+              if (c < ncol && yy < ey) line[pa_fft::pad_index(y0 + yy)] = cx{v[k].x, v[k].y};
             }
           }
         }
@@ -217,8 +246,8 @@ __global__ void __launch_bounds__(FFT_THREADS) k_unpack_fft(const __grid_constan
   // ---- store: natural order, every line one contiguous run ----
   char* d = p.dst + x0 * p.dsx + d_off;
   for (int c = 0; c < ncol; ++c) {
-    const cplx* line = sm + c * pitch;
-    double2* out = reinterpret_cast<double2*>(d + c * p.dsx);
+    const cx* line = sm + c * pitch;
+    V* out = reinterpret_cast<V*>(d + c * p.dsx);
 #pragma unroll
     for (int k0 = 0; k0 < L; k0 += FFT_THREADS) {
       const int k = k0 + t;
@@ -226,8 +255,8 @@ __global__ void __launch_bounds__(FFT_THREADS) k_unpack_fft(const __grid_constan
         // position of frequency k: first-pass digit, then the digits of the later passes
         const int pos = ((k & ((1 << LOGR1) - 1)) << (LOGL - LOGR1)) +
                         fft_pos<LOGL, LOGL - LOGR1>(k >> LOGR1);
-        const cplx v = line[pa_fft::pad_index(pos)];
-        __stcs(out + k, make_double2(v.x, v.y));
+        const cx v = line[pa_fft::pad_index(pos)];
+        __stcs(out + k, vec2(v.x, v.y));
       }
     }
   }
@@ -242,46 +271,50 @@ struct RfftParams {
   long long nlines;
   long long src_line, dst_line;  // byte strides of consecutive lines
   int pitch;
-  const cplx* tw;  // W_N^k, k < N: the post- / pre-pass reads entry k, the L-point passes entry 2i
+  const void* tw;  // W_N^k, k < N: the post- / pre-pass reads entry k, the L-point passes entry 2i
 };
 
-template <int LOGL, int C, bool FWD>
+// Single precision: complex lines are 8 (N/2 + 1) bytes, an odd multiple of 8, so every other
+// line starts only 8-byte aligned; every access is one 8-byte element (float2) on both sides.
+template <int LOGL, int C, bool FWD, class T>
 __global__ void __launch_bounds__(FFT_THREADS) k_rfft(const __grid_constant__ RfftParams p) {
+  using cx = cplx_t<T>;
+  using V = typename Vec2<T>::type;
   constexpr int L = 1 << LOGL;
   constexpr int RS = FFT_THREADS / C;  // threads per line
   constexpr int P = L / 2 + 1;         // pairs (k, L - k) per line
   extern __shared__ __align__(16) unsigned char fft_smem[];
-  cplx* sm = reinterpret_cast<cplx*>(fft_smem);
+  cx* sm = reinterpret_cast<cx*>(fft_smem);
   const int t = threadIdx.x;
   const long long l0 = (long long)blockIdx.x * C;
   const int ncol = (int)((p.nlines - l0) < C ? (p.nlines - l0) : C);
   const int pitch = p.pitch;
-  const cplx* twp = p.tw;
+  const V* twp = reinterpret_cast<const V*>(p.tw);
   auto twN = [twp](int k) {
-    const double2 w = __ldg(reinterpret_cast<const double2*>(twp) + k);
-    return cplx{w.x, w.y};
+    const V w = __ldg(twp + k);
+    return cx{w.x, w.y};
   };
   auto twL = [twp](int i) {  // W_L^i = W_N^(2i)
-    const double2 w = __ldg(reinterpret_cast<const double2*>(twp) + 2 * i);
-    return cplx{w.x, w.y};
+    const V w = __ldg(twp + 2 * i);
+    return cx{w.x, w.y};
   };
 
-  // ---- load (linear gather): consecutive threads walk along a line with 128-bit loads.
+  // ---- load (linear gather): consecutive threads walk along a line, one element per load.
   //      Forward: the N reals ARE the complex line z[n] = x[2n] + i x[2n+1]; backward: N/2+1 bins ----
   {
     constexpr int NIN = FWD ? L : L + 1;
     constexpr int U = (NIN + RS - 1) / RS;
     const int c = t / RS, r = t % RS;
     if (c < ncol) {
-      const double2* s = reinterpret_cast<const double2*>(p.src + (l0 + c) * p.src_line);
-      cplx* line = sm + c * pitch;
-      double2 v[U];
+      const V* s = reinterpret_cast<const V*>(p.src + (l0 + c) * p.src_line);
+      cx* line = sm + c * pitch;
+      V v[U];
 #pragma unroll
       for (int q = 0; q < U; ++q)
         if (r + q * RS < NIN) v[q] = __ldcs(s + r + q * RS);
 #pragma unroll
       for (int q = 0; q < U; ++q)
-        if (r + q * RS < NIN) line[pa_fft::pad_index(r + q * RS)] = cplx{v[q].x, v[q].y};
+        if (r + q * RS < NIN) line[pa_fft::pad_index(r + q * RS)] = cx{v[q].x, v[q].y};
     }
   }
   __syncthreads();
@@ -292,8 +325,8 @@ __global__ void __launch_bounds__(FFT_THREADS) k_rfft(const __grid_constant__ Rf
     for (int w0 = 0; w0 < C * P; w0 += FFT_THREADS) {
       const int w = w0 + t, c = w / P, k = w % P;
       if (w < C * P && c < ncol) {
-        cplx* line = sm + c * pitch;
-        cplx zk, zl;
+        cx* line = sm + c * pitch;
+        cx zk, zl;
         pa_fft::brfft_pre_pair(k, line[pa_fft::pad_index(k)], line[pa_fft::pad_index(L - k)], twN(k),
                                &zk, &zl);
         line[pa_fft::pad_index(k)] = zk;
@@ -311,48 +344,65 @@ __global__ void __launch_bounds__(FFT_THREADS) k_rfft(const __grid_constant__ Rf
     for (int w0 = 0; w0 < C * P; w0 += FFT_THREADS) {
       const int w = w0 + t, c = w / P, k = w % P;
       if (w < C * P && c < ncol) {
-        const cplx* line = sm + c * pitch;
-        cplx xk, xl;
+        const cx* line = sm + c * pitch;
+        cx xk, xl;
         pa_fft::rfft_post_pair(line[pa_fft::pad_index(fft_pos<LOGL, LOGL>(k & (L - 1)))],
                                line[pa_fft::pad_index(fft_pos<LOGL, LOGL>((L - k) & (L - 1)))], twN(k),
                                &xk, &xl);
-        double2* out = reinterpret_cast<double2*>(p.dst + (l0 + c) * p.dst_line);
-        __stcs(out + k, make_double2(xk.x, xk.y));
-        if (k != L - k) __stcs(out + (L - k), make_double2(xl.x, xl.y));
+        V* out = reinterpret_cast<V*>(p.dst + (l0 + c) * p.dst_line);
+        __stcs(out + k, vec2(xk.x, xk.y));
+        if (k != L - k) __stcs(out + (L - k), vec2(xl.x, xl.y));
       }
     }
   } else {
-    // ---- store: z[n] = x[2n] + i x[2n+1], the N reals of a line as L 128-bit stores ----
+    // ---- store: z[n] = x[2n] + i x[2n+1], the N reals of a line as L pair stores ----
 #pragma unroll
     for (int w0 = 0; w0 < C * L; w0 += FFT_THREADS) {
       const int w = w0 + t, c = w >> LOGL, n = w & (L - 1);
       if (c < ncol) {
-        const cplx v = sm[c * pitch + pa_fft::pad_index(fft_pos<LOGL, LOGL>(n))];
-        __stcs(reinterpret_cast<double2*>(p.dst + (l0 + c) * p.dst_line) + n, make_double2(v.x, v.y));
+        const cx v = sm[c * pitch + pa_fft::pad_index(fft_pos<LOGL, LOGL>(n))];
+        __stcs(reinterpret_cast<V*>(p.dst + (l0 + c) * p.dst_line) + n, vec2(v.x, v.y));
       }
     }
   }
 }
 
-// forward twiddle table W_L^k per (device, L), computed once in extended precision
-static const cplx* twiddles(int L) {
+// forward twiddle table W_L^k per (device, L, precision), computed once in extended precision
+// and rounded once to double (cplx) or float (cplxf)
+template <class T>
+static std::vector<cplx_t<T>> twiddle_values(int L) {
+  std::vector<cplx_t<T>> h(L);
+  for (int k = 0; k < L; ++k) {
+    const long double a = -2.0L * 3.141592653589793238462643383279502884L * k / L;
+    h[k] = cplx_t<T>{(T)cosl(a), (T)sinl(a)};
+  }
+  return h;
+}
+
+static const void* twiddles(int L, bool f32) {
   static std::mutex mu;
-  static std::map<std::pair<int, int>, cplx*> cache;
+  static std::map<std::tuple<int, int, bool>, void*> cache;
   std::lock_guard<std::mutex> lock(mu);
   int dev = 0;
   cudaGetDevice(&dev);
-  auto key = std::make_pair(dev, L);
+  auto key = std::make_tuple(dev, L, f32);
   auto it = cache.find(key);
   if (it != cache.end()) return it->second;
-  std::vector<cplx> h(L);
-  for (int k = 0; k < L; ++k) {
-    const long double a = -2.0L * 3.141592653589793238462643383279502884L * k / L;
-    h[k] = cplx{(double)cosl(a), (double)sinl(a)};
+  auto upload = [&](const void* h, size_t bytes) -> void* {
+    void* d = nullptr;
+    if (cudaMalloc(&d, bytes) != cudaSuccess) return nullptr;
+    if (cudaMemcpy(d, h, bytes, cudaMemcpyHostToDevice) != cudaSuccess) return nullptr;
+    return d;
+  };
+  void* d = nullptr;
+  if (f32) {
+    const auto h = twiddle_values<float>(L);
+    d = upload(h.data(), sizeof(h[0]) * L);
+  } else {
+    const auto h = twiddle_values<double>(L);
+    d = upload(h.data(), sizeof(h[0]) * L);
   }
-  cplx* d = nullptr;
-  if (cudaMalloc((void**)&d, sizeof(cplx) * L) != cudaSuccess) return nullptr;
-  if (cudaMemcpy(d, h.data(), sizeof(cplx) * L, cudaMemcpyHostToDevice) != cudaSuccess) return nullptr;
-  cache[key] = d;
+  if (d) cache[key] = d;
   return d;
 }
 
@@ -360,9 +410,11 @@ static const cplx* twiddles(int L) {
 // from `srcs[i]` -- recv_buf, or the src parent for the fused self block -- into `dst`;
 // together they must tile the destination box), and every check of it.  srcs / dst may be
 // NULL: plan_fft_check runs this on the blocks a peer would see, without arrays.  *grid = 0:
-// nothing to do on this rank.
+// nothing to do on this rank.  f32: ComplexF32 elements (PA_FFT_F32), else ComplexF64.
 static pa_status fft_geometry(int nb, const BlockCopy* const* blocks, const void* const* srcs,
-                              void* dst, FftParams& p, int* C_out, unsigned long long* grid_out) {
+                              void* dst, bool f32, FftParams& p, int* C_out,
+                              unsigned long long* grid_out) {
+  const i64 es = f32 ? 8 : 16;  // element bytes
   memset(&p, 0, sizeof p);
   *grid_out = 0;
   // the line dim: destination stride 1 (and extent > 1) in some block
@@ -415,8 +467,9 @@ static pa_status fft_geometry(int nb, const BlockCopy* const* blocks, const void
   for (int b = 0; b < nb; ++b) {
     const BlockCopy& B = *blocks[b];
     if (B.count == 0) continue;
-    if (B.elsize != 16) {
-      set_error("fused FFT: ComplexF64 (16-byte) elements only");
+    if (B.elsize != es) {
+      set_error(f32 ? "fused FFT: PA_FFT_F32 takes ComplexF32 (8-byte) elements only"
+                    : "fused FFT: ComplexF64 (16-byte) elements only");
       return PA_EINVAL;
     }
     if (B.raw[0].ss != 1) {
@@ -449,14 +502,14 @@ static pa_status fft_geometry(int nb, const BlockCopy* const* blocks, const void
       return PA_EINVAL;
     }
     FftBlock& F = p.blk[p.nb++];
-    F.src = srcs ? (const char*)srcs[b] + B.src_off * 16 : nullptr;
+    F.src = srcs ? (const char*)srcs[b] + B.src_off * es : nullptr;
     F.y0 = (int)(B.dst_off - min_doff);
     F.ey = (int)B.raw[jy].e;
-    F.ssy = B.raw[jy].ss * 16;
-    F.ssx = jx >= 0 ? B.raw[jx].ss * 16 : 16;
+    F.ssy = B.raw[jy].ss * es;
+    F.ssx = jx >= 0 ? B.raw[jx].ss * es : es;
     int o = 0;
     for (int i = 1; i < B.nd_raw; ++i)
-      if (i != jy && i != jx && B.raw[i].e > 1) F.so[o++] = B.raw[i].ss * 16;
+      if (i != jy && i != jx && B.raw[i].e > 1) F.so[o++] = B.raw[i].ss * es;
     L += B.raw[jy].e;
   }
   int logL = 0;
@@ -479,10 +532,10 @@ static pa_status fft_geometry(int nb, const BlockCopy* const* blocks, const void
       pos += s.second;
     }
   }
-  p.dst = dst ? (char*)dst + min_doff * 16 : nullptr;
+  p.dst = dst ? (char*)dst + min_doff * es : nullptr;
   p.linear = linear ? 1 : 0;
   p.ex = jx >= 0 ? ref->raw[jx].e : 1;
-  p.dsx = jx >= 0 ? ref->raw[jx].ds * 16 : 16;
+  p.dsx = jx >= 0 ? ref->raw[jx].ds * es : es;
   p.no = 0;
   for (int i = 1; i < ref->nd_raw; ++i)
     if (i != jy && i != jx && ref->raw[i].e > 1) {
@@ -491,15 +544,17 @@ static pa_status fft_geometry(int nb, const BlockCopy* const* blocks, const void
         return PA_EINVAL;
       }
       p.oe[p.no] = ref->raw[i].e;
-      p.dso[p.no] = ref->raw[i].ds * 16;
+      p.dso[p.no] = ref->raw[i].ds * es;
       ++p.no;
     }
   p.L = (int)L;
   p.logL = logL;
   p.pitch = pa_fft::padded_pitch((int)L);
   // tunable "fft_lines" = 4: 4 lines per CTA also for 256- / 512-point lines (64-byte gathers,
-  // first pass of radix 4 / 8 in registers, half the shared memory per CTA)
-  const int C = (g_tun.fft_lines == 4 && logL >= 8) ? 4 : fft_lines(logL);
+  // first pass of radix 4 / 8 in registers, half the shared memory per CTA); double precision
+  // only -- single precision always takes fft_lines_f32
+  const int C = f32 ? fft_lines_f32(logL)
+                    : ((g_tun.fft_lines == 4 && logL >= 8) ? 4 : fft_lines(logL));
   p.tiles_x = (unsigned)((p.ex + C - 1) / C);
   unsigned long long grid = p.tiles_x;
   for (int i = 0; i < p.no; ++i) grid *= (unsigned long long)p.oe[i];
@@ -513,23 +568,23 @@ static pa_status fft_geometry(int nb, const BlockCopy* const* blocks, const void
 }
 
 pa_status unpack_fft(int nb, const BlockCopy* const* blocks, const void* const* srcs, void* dst,
-                     int sign, void* stream) {
+                     int sign, bool f32, void* stream) {
   // (pa_transpose has already asked plan_fft_check, for every rank of the line, before it
   //  enqueued anything: these checks only guard direct callers)
   FftParams p;
   int C = 0;
   unsigned long long grid = 0;
-  pa_status s = fft_geometry(nb, blocks, srcs, dst, p, &C, &grid);
+  pa_status s = fft_geometry(nb, blocks, srcs, dst, f32, p, &C, &grid);
   if (s != PA_OK || grid == 0) return s;
   const int logL = p.logL;
   p.sign = sign < 0 ? -1 : 1;
-  p.tw = twiddles(p.L);
+  p.tw = twiddles(p.L, f32);
   if (!p.tw) {
     set_error("fused FFT: twiddle table allocation failed");
     cudaGetLastError();
     return PA_ENOMEM;
   }
-  const size_t smem = sizeof(cplx) * (size_t)C * p.pitch;
+  const size_t smem = (f32 ? sizeof(pa_fft::cplxf) : sizeof(cplx)) * (size_t)C * p.pitch;
   cudaError_t e = cudaSuccess;
   auto launch = [&](auto kern) {
     // shared memory is the scarce resource: ask for the largest carve-out so that
@@ -543,15 +598,28 @@ pa_status unpack_fft(int nb, const BlockCopy* const* blocks, const void* const* 
     kern<<<(unsigned)grid, FFT_THREADS, smem, (cudaStream_t)stream>>>(p);
     e = cudaGetLastError();
   };
-  switch (logL) {
-    case 3: launch(k_unpack_fft<3, 8>); break;
-    case 4: launch(k_unpack_fft<4, 8>); break;
-    case 5: launch(k_unpack_fft<5, 8>); break;
-    case 6: launch(k_unpack_fft<6, 8>); break;
-    case 7: launch(k_unpack_fft<7, 8>); break;
-    case 8: if (C == 4) launch(k_unpack_fft<8, 4>); else launch(k_unpack_fft<8, 8>); break;
-    case 9: if (C == 4) launch(k_unpack_fft<9, 4>); else launch(k_unpack_fft<9, 8>); break;
-    default: launch(k_unpack_fft<10, 4>); break;
+  if (f32) {
+    switch (logL) {
+      case 3: launch(k_unpack_fft<3, 16, float>); break;
+      case 4: launch(k_unpack_fft<4, 16, float>); break;
+      case 5: launch(k_unpack_fft<5, 16, float>); break;
+      case 6: launch(k_unpack_fft<6, 16, float>); break;
+      case 7: launch(k_unpack_fft<7, 16, float>); break;
+      case 8: launch(k_unpack_fft<8, 16, float>); break;
+      case 9: launch(k_unpack_fft<9, 16, float>); break;
+      default: launch(k_unpack_fft<10, 8, float>); break;
+    }
+  } else {
+    switch (logL) {
+      case 3: launch(k_unpack_fft<3, 8, double>); break;
+      case 4: launch(k_unpack_fft<4, 8, double>); break;
+      case 5: launch(k_unpack_fft<5, 8, double>); break;
+      case 6: launch(k_unpack_fft<6, 8, double>); break;
+      case 7: launch(k_unpack_fft<7, 8, double>); break;
+      case 8: if (C == 4) launch(k_unpack_fft<8, 4, double>); else launch(k_unpack_fft<8, 8, double>); break;
+      case 9: if (C == 4) launch(k_unpack_fft<9, 4, double>); else launch(k_unpack_fft<9, 8, double>); break;
+      default: launch(k_unpack_fft<10, 4, double>); break;
+    }
   }
   if (e != cudaSuccess) {
     set_error("fused FFT kernel launch failed: %s", cudaGetErrorString(e));
@@ -566,20 +634,26 @@ pa_status unpack_fft(int nb, const BlockCopy* const* blocks, const void* const* 
 // would leave them waiting on flags it never sets.  So the answer depends on the global
 // geometry only: the blocks that EVERY rank of the line would gather -- each rank's plan
 // rebuilt from the pencils with that rank's coordinates -- with the self block read from src
-// and staged through recv_buf alike.  Cached per plan (and per value of tunable fft_lines).
-pa_status plan_fft_check(Plan* P) {
-  if (P->fft_check_lines == g_tun.fft_lines) {
-    if (P->fft_check != PA_OK) set_error("%s", P->fft_check_err.c_str());
-    return P->fft_check;
+// and staged through recv_buf alike.  Cached per plan, per precision (f32: ComplexF32) and per
+// value of tunable fft_lines.
+pa_status plan_fft_check(Plan* P, bool f32) {
+  const int q = f32 ? 1 : 0;
+  if (P->fft_check_lines[q] == g_tun.fft_lines) {
+    if (P->fft_check[q] != PA_OK) set_error("%s", P->fft_check_err[q].c_str());
+    return P->fft_check[q];
   }
   auto verdict = [&](pa_status s) {
-    P->fft_check = s;
-    P->fft_check_err = s == PA_OK ? std::string() : std::string(last_error());
-    P->fft_check_lines = g_tun.fft_lines;
+    P->fft_check[q] = s;
+    P->fft_check_err[q] = s == PA_OK ? std::string() : std::string(last_error());
+    P->fft_check_lines[q] = g_tun.fft_lines;
     return s;
   };
-  if (P->elsize != 16) {
+  if (!f32 && P->elsize != 16) {
     set_error("fused FFT: ComplexF64 (16-byte) elements only");
+    return verdict(PA_EINVAL);
+  }
+  if (f32 && P->elsize != 8) {
+    set_error("fused FFT: PA_FFT_F32 takes ComplexF32 (8-byte) elements only");
     return verdict(PA_EINVAL);
   }
   FftParams p;
@@ -587,7 +661,7 @@ pa_status plan_fft_check(Plan* P) {
   unsigned long long grid = 0;
   if (P->dim < 0 || P->nproc == 1) {
     const BlockCopy* b = &P->self_fused;
-    return verdict(fft_geometry(1, &b, nullptr, nullptr, p, &C, &grid));
+    return verdict(fft_geometry(1, &b, nullptr, nullptr, f32, p, &C, &grid));
   }
   for (int n = 0; n < P->nproc; ++n) {
     std::unique_ptr<Plan> hold;
@@ -610,7 +684,7 @@ pa_status plan_fft_check(Plan* P) {
       std::vector<const BlockCopy*> bl;
       for (int k = 0; k < Q->nproc; ++k)
         bl.push_back(k == Q->self_index && !staged_self ? &Q->self_fused : &Q->peers[k].unpack);
-      pa_status s = fft_geometry(Q->nproc, bl.data(), nullptr, nullptr, p, &C, &grid);
+      pa_status s = fft_geometry(Q->nproc, bl.data(), nullptr, nullptr, f32, p, &C, &grid);
       if (s != PA_OK) {
         if (n != P->self_index) {
           const std::string why = last_error();
@@ -623,7 +697,8 @@ pa_status plan_fft_check(Plan* P) {
   return verdict(PA_OK);
 }
 
-pa_status rfft_lines(int N, bool forward, i64 nlines, const void* src, void* dst, void* stream) {
+pa_status rfft_lines(int N, bool forward, bool f32, i64 nlines, const void* src, void* dst,
+                     void* stream) {
   const int L = N / 2;
   int logL = 0;
   while ((1 << logL) < L) ++logL;
@@ -636,22 +711,23 @@ pa_status rfft_lines(int N, bool forward, i64 nlines, const void* src, void* dst
   p.src = (const char*)src;
   p.dst = (char*)dst;
   p.nlines = nlines;
-  p.src_line = forward ? 8LL * N : 16LL * (L + 1);
-  p.dst_line = forward ? 16LL * (L + 1) : 8LL * N;
+  const long long rs = f32 ? 4 : 8, cs = 2 * rs;  // bytes of a real / a complex element
+  p.src_line = forward ? rs * N : cs * (L + 1);
+  p.dst_line = forward ? cs * (L + 1) : rs * N;
   p.pitch = pa_fft::padded_pitch(forward ? L : L + 1);  // backward stages all N/2 + 1 bins
-  p.tw = twiddles(N);
+  p.tw = twiddles(N, f32);
   if (!p.tw) {
     set_error("rfft: twiddle table allocation failed");
     cudaGetLastError();
     return PA_ENOMEM;
   }
-  const int C = fft_lines(logL);
+  const int C = f32 ? fft_lines_f32(logL) : fft_lines(logL);
   const long long grid = (nlines + C - 1) / C;
   if (grid > 0x7fffffffLL) {
     set_error("rfft: too many lines for one launch");
     return PA_EINVAL;
   }
-  const size_t smem = sizeof(cplx) * (size_t)C * p.pitch;
+  const size_t smem = (size_t)cs * C * p.pitch;
   cudaError_t e = cudaSuccess;
   auto launch = [&](auto kern) {
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -662,15 +738,28 @@ pa_status rfft_lines(int N, bool forward, i64 nlines, const void* src, void* dst
     e = cudaGetLastError();
   };
   auto launch_dir = [&](auto fwd_kern, auto bwd_kern) { forward ? launch(fwd_kern) : launch(bwd_kern); };
-  switch (logL) {
-    case 3: launch_dir(k_rfft<3, 8, true>, k_rfft<3, 8, false>); break;
-    case 4: launch_dir(k_rfft<4, 8, true>, k_rfft<4, 8, false>); break;
-    case 5: launch_dir(k_rfft<5, 8, true>, k_rfft<5, 8, false>); break;
-    case 6: launch_dir(k_rfft<6, 8, true>, k_rfft<6, 8, false>); break;
-    case 7: launch_dir(k_rfft<7, 8, true>, k_rfft<7, 8, false>); break;
-    case 8: launch_dir(k_rfft<8, 8, true>, k_rfft<8, 8, false>); break;
-    case 9: launch_dir(k_rfft<9, 8, true>, k_rfft<9, 8, false>); break;
-    default: launch_dir(k_rfft<10, 4, true>, k_rfft<10, 4, false>); break;
+  if (f32) {
+    switch (logL) {
+      case 3: launch_dir(k_rfft<3, 16, true, float>, k_rfft<3, 16, false, float>); break;
+      case 4: launch_dir(k_rfft<4, 16, true, float>, k_rfft<4, 16, false, float>); break;
+      case 5: launch_dir(k_rfft<5, 16, true, float>, k_rfft<5, 16, false, float>); break;
+      case 6: launch_dir(k_rfft<6, 16, true, float>, k_rfft<6, 16, false, float>); break;
+      case 7: launch_dir(k_rfft<7, 16, true, float>, k_rfft<7, 16, false, float>); break;
+      case 8: launch_dir(k_rfft<8, 16, true, float>, k_rfft<8, 16, false, float>); break;
+      case 9: launch_dir(k_rfft<9, 16, true, float>, k_rfft<9, 16, false, float>); break;
+      default: launch_dir(k_rfft<10, 8, true, float>, k_rfft<10, 8, false, float>); break;
+    }
+  } else {
+    switch (logL) {
+      case 3: launch_dir(k_rfft<3, 8, true, double>, k_rfft<3, 8, false, double>); break;
+      case 4: launch_dir(k_rfft<4, 8, true, double>, k_rfft<4, 8, false, double>); break;
+      case 5: launch_dir(k_rfft<5, 8, true, double>, k_rfft<5, 8, false, double>); break;
+      case 6: launch_dir(k_rfft<6, 8, true, double>, k_rfft<6, 8, false, double>); break;
+      case 7: launch_dir(k_rfft<7, 8, true, double>, k_rfft<7, 8, false, double>); break;
+      case 8: launch_dir(k_rfft<8, 8, true, double>, k_rfft<8, 8, false, double>); break;
+      case 9: launch_dir(k_rfft<9, 8, true, double>, k_rfft<9, 8, false, double>); break;
+      default: launch_dir(k_rfft<10, 4, true, double>, k_rfft<10, 4, false, double>); break;
+    }
   }
   if (e != cudaSuccess) {
     set_error("rfft kernel launch failed: %s", cudaGetErrorString(e));

@@ -27,22 +27,39 @@
 
 namespace pa_fft {
 
-struct cplx {
-  double x, y;
+// complex of real type T: double (ComplexF64) or float (ComplexF32, PA_FFT_F32).  Both the
+// storage and the arithmetic are in T; `cplx` is the double-precision type.
+template <class T>
+struct cplx_t {
+  T x, y;
 };
+using cplx = cplx_t<double>;
+using cplxf = cplx_t<float>;
 
-PA_HD cplx cadd(cplx a, cplx b) { return cplx{a.x + b.x, a.y + b.y}; }
-PA_HD cplx csub(cplx a, cplx b) { return cplx{a.x - b.x, a.y - b.y}; }
-PA_HD cplx cmul(cplx a, cplx b) { return cplx{a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x}; }
+template <class T>
+PA_HD cplx_t<T> cadd(cplx_t<T> a, cplx_t<T> b) { return cplx_t<T>{a.x + b.x, a.y + b.y}; }
+template <class T>
+PA_HD cplx_t<T> csub(cplx_t<T> a, cplx_t<T> b) { return cplx_t<T>{a.x - b.x, a.y - b.y}; }
+template <class T>
+PA_HD cplx_t<T> cmul(cplx_t<T> a, cplx_t<T> b) {
+  return cplx_t<T>{a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x};
+}
 // multiplication by -i (forward) / +i (backward): sign = -1 forward, +1 backward
-PA_HD cplx mul_i(cplx a, int sign) { return sign < 0 ? cplx{a.y, -a.x} : cplx{-a.y, a.x}; }
+template <class T>
+PA_HD cplx_t<T> mul_i(cplx_t<T> a, int sign) {
+  return sign < 0 ? cplx_t<T>{a.y, -a.x} : cplx_t<T>{-a.y, a.x};
+}
 
 // storage index of logical position i: one pad element after every 8, 64 and 512
 // elements, so that accesses at every power-of-8 stride (the strides of the radix-8
-// passes and of the digit-reversed read-out) fall into different 16-byte bank groups
+// passes and of the digit-reversed read-out) fall into different 16-byte bank groups.
+// The same padding serves 8-byte (ComplexF32) elements: strides of 8, 64 and 512 points
+// become 9, 73 and 585 stored elements, each 18 banks mod 32, and 18 i mod 32 is a distinct
+// even bank for each of the 16 threads of a 64-bit shared-memory phase (DESIGN §3d)
 PA_HD int pad_index(int i) { return i + (i >> 3) + (i >> 6) + (i >> 9); }
 // elements per padded line, forced to 1 mod 8 (the C lines of a CTA are written
-// column-wise by 8 consecutive threads)
+// column-wise by 8 consecutive threads; for 8-byte elements by 16, and 2 pitch mod 32 is
+// then 2 or 18: distinct banks for all 16)
 PA_HD int padded_pitch(int L) {
   int n = pad_index(L - 1) + 1;
   while ((n & 7) != 1) ++n;
@@ -88,21 +105,25 @@ PA_HD int fft_position_of(int k, int L, const Radices& R) {
 }
 
 // R-point DFT in registers, a[q] -> A[s] = sum_q a[q] * w^(q*s), w = exp(sign*2*pi*i/R)
-PA_HD void dft2(cplx* a) {
-  cplx t = a[0];
+template <class T>
+PA_HD void dft2(cplx_t<T>* a) {
+  cplx_t<T> t = a[0];
   a[0] = cadd(t, a[1]);
   a[1] = csub(t, a[1]);
 }
-PA_HD void dft4(cplx* a, int sign) {
-  cplx t0 = cadd(a[0], a[2]), t1 = csub(a[0], a[2]);
-  cplx t2 = cadd(a[1], a[3]), t3 = mul_i(csub(a[1], a[3]), sign);
+template <class T>
+PA_HD void dft4(cplx_t<T>* a, int sign) {
+  cplx_t<T> t0 = cadd(a[0], a[2]), t1 = csub(a[0], a[2]);
+  cplx_t<T> t2 = cadd(a[1], a[3]), t3 = mul_i(csub(a[1], a[3]), sign);
   a[0] = cadd(t0, t2);
   a[1] = cadd(t1, t3);
   a[2] = csub(t0, t2);
   a[3] = csub(t1, t3);
 }
-PA_HD void dft8(cplx* a, int sign) {
-  const double h = 0.70710678118654752440;
+template <class T>
+PA_HD void dft8(cplx_t<T>* a, int sign) {
+  using cplx = cplx_t<T>;
+  const T h = T(0.70710678118654752440);
   // even / odd 4-point transforms
   cplx e[4] = {a[0], a[2], a[4], a[6]};
   cplx o[4] = {a[1], a[3], a[5], a[7]};
@@ -123,9 +144,11 @@ PA_HD void dft8(cplx* a, int sign) {
 }
 
 // 16 = 4 x 4: a[4*q1 + q2] -> A[s1 + 4*s2]
-PA_HD void dft16(cplx* a, int sign) {
-  const double c1 = 0.92387953251128675613, s1 = 0.38268343236508977173;  // cos, sin(pi/8)
-  const double h = 0.70710678118654752440;
+template <class T>
+PA_HD void dft16(cplx_t<T>* a, int sign) {
+  using cplx = cplx_t<T>;
+  const T c1 = T(0.92387953251128675613), s1 = T(0.38268343236508977173);  // cos, sin(pi/8)
+  const T h = T(0.70710678118654752440);
   cplx b[4][4];
 #if defined(__CUDACC__)
 #pragma unroll
@@ -165,8 +188,8 @@ PA_HD void dft16(cplx* a, int sign) {
 
 // the R-1 twiddles W^(step*s), s = 1..R-1, of one butterfly from the table entries at
 // step, 2 step, 4 step (and 8 step): the others are one or two complex products away
-template <int R, class Tw>
-PA_HD void butterfly_twiddles(cplx* w, int step, int L, int sign, const Tw& tw) {
+template <int R, class T, class Tw>
+PA_HD void butterfly_twiddles(cplx_t<T>* w, int step, int L, int sign, const Tw& tw) {
 #if defined(PA_FFT_TWIDDLE_LOOKUPS) && PA_FFT_TWIDDLE_LOOKUPS == 1
   // one table lookup per butterfly, the powers by squaring / products (<= 4 roundings
   // more than a direct lookup: still far inside 8 eps log2(L))
@@ -203,15 +226,15 @@ PA_HD void butterfly_twiddles(cplx* w, int step, int L, int sign, const Tw& tw) 
 
 // The R-point transform + twiddles of one butterfly on values already in registers
 // (the fused kernel's first pass works on the rows it has just loaded from HBM).
-template <int R, class Tw>
-PA_HD void butterfly_regs(cplx* a, int j, int L, int M, int sign, const Tw& tw) {
+template <int R, class T, class Tw>
+PA_HD void butterfly_regs(cplx_t<T>* a, int j, int L, int M, int sign, const Tw& tw) {
   if (R == 2) dft2(a);
   if (R == 4) dft4(a, sign);
   if (R == 8) dft8(a, sign);
   if (R == 16) dft16(a, sign);
   const int step = j * (L / M);   // W_M^(j*s) = W_L^(j*s*L/M)
   if (step > 0) {
-    cplx w[R > 1 ? R : 2];
+    cplx_t<T> w[R > 1 ? R : 2];
     butterfly_twiddles<R>(w, step, L, sign, tw);
 #if defined(__CUDACC__)
 #pragma unroll
@@ -231,7 +254,7 @@ PA_HD void butterfly(Line& x, int u, int L, int M, int sign, const Tw& tw) {
   const int Q = M / R;            // stride between the R inputs
   const int g = u / Q, j = u % Q;
   const int base = g * M + j;
-  cplx a[R];
+  decltype(x.get(0)) a[R];   // the line's element type: cplx or cplxf
 #if defined(__CUDACC__)
 #pragma unroll
 #endif
@@ -250,9 +273,12 @@ PA_HD void butterfly(Line& x, int u, int L, int M, int sign, const Tw& tw) {
 //   X[L - k] = conj(E - w O)
 // (indices of Z mod L).  One call per pair k = 0 ... L/2 yields all N/2 + 1 bins: k = 0 gives X[0]
 // and X[L] (both real), k = L/2 gives X[L/2] twice.
-PA_HD void rfft_post_pair(cplx zk, cplx zl, cplx w, cplx* xk, cplx* xl) {
-  const cplx e = cplx{0.5 * (zk.x + zl.x), 0.5 * (zk.y - zl.y)};
-  const cplx o = cplx{0.5 * (zk.y + zl.y), -0.5 * (zk.x - zl.x)};
+template <class T>
+PA_HD void rfft_post_pair(cplx_t<T> zk, cplx_t<T> zl, cplx_t<T> w, cplx_t<T>* xk, cplx_t<T>* xl) {
+  using cplx = cplx_t<T>;
+  const T half = T(0.5);
+  const cplx e = cplx{half * (zk.x + zl.x), half * (zk.y - zl.y)};
+  const cplx o = cplx{half * (zk.y + zl.y), -half * (zk.x - zl.x)};
   const cplx wo = cmul(w, o);
   *xk = cadd(e, wo);
   *xl = cplx{e.x - wo.x, wo.y - e.y};
@@ -264,10 +290,13 @@ PA_HD void rfft_post_pair(cplx zk, cplx zl, cplx w, cplx* xk, cplx* xl) {
 //   Z[k] = F + i G,   Z[L-k] = conj F + i conj G
 // At k = 0 the partner is X[L]; the imaginary parts of X[0] and X[L] are dropped, as numpy and
 // FFTW drop them (a real signal cannot have them); Z[L] is Z[0] and is not produced.
-PA_HD void brfft_pre_pair(int k, cplx xk, cplx xl, cplx w, cplx* zk, cplx* zl) {
+template <class T>
+PA_HD void brfft_pre_pair(int k, cplx_t<T> xk, cplx_t<T> xl, cplx_t<T> w, cplx_t<T>* zk,
+                          cplx_t<T>* zl) {
+  using cplx = cplx_t<T>;
   if (k == 0) {
-    xk.y = 0.0;
-    xl.y = 0.0;
+    xk.y = T(0);
+    xl.y = T(0);
   }
   const cplx f = cplx{xk.x + xl.x, xk.y - xl.y};
   const cplx g = cmul(cplx{xk.x - xl.x, xk.y + xl.y}, cplx{w.x, -w.y});

@@ -220,10 +220,11 @@ struct Plan {
   void* h_src_dev = nullptr;
   void* h_dst_dev = nullptr;
   i64 h_src_cap = 0, h_dst_cap = 0;
-  // cached answer of plan_fft_check (valid while tunable fft_lines == fft_check_lines)
-  int fft_check_lines = -1;
-  pa_status fft_check = PA_OK;
-  std::string fft_check_err;
+  // cached answers of plan_fft_check, [0] ComplexF64 and [1] ComplexF32 (PA_FFT_F32), each
+  // valid while tunable fft_lines == fft_check_lines[i]
+  int fft_check_lines[2] = {-1, -1};
+  pa_status fft_check[2] = {PA_OK, PA_OK};
+  std::string fft_check_err[2];
   ~Plan();
 };
 
@@ -266,15 +267,19 @@ pa_status host_chain_time_begin(HostChain* c);
 pa_status host_chain_time_end(HostChain* c, float* ms);
 
 // fused unpack + 1-d FFT along the destination's contiguous dim (fft.cu): the blocks
-// together tile the destination box; srcs[i] = base pointer blocks[i] reads from
+// together tile the destination box; srcs[i] = base pointer blocks[i] reads from.
+// f32: ComplexF32 elements and fp32 arithmetic (PA_FFT_F32), else ComplexF64
 pa_status unpack_fft(int nb, const BlockCopy* const* blocks, const void* const* srcs, void* dst,
-                     int sign, void* stream);
-// can pa_transpose fuse a FFT into this plan's unpack?  The same answer on every rank of the
-// grid line (global geometry only); PA_EINVAL + last_error otherwise.  No device call.
-pa_status plan_fft_check(Plan* plan);
+                     int sign, bool f32, void* stream);
+// can pa_transpose fuse a FFT of the given precision into this plan's unpack?  The same answer
+// on every rank of the grid line (global geometry only); PA_EINVAL + last_error otherwise.
+// No device call.
+pa_status plan_fft_check(Plan* plan, bool f32);
 // real-line transforms (fft.cu): `nlines` dense, consecutive lines of N reals (src when forward,
-// dst when backward) <-> N/2 + 1 complex bins; N a power of two in 16..2048
-pa_status rfft_lines(int N, bool forward, i64 nlines, const void* src, void* dst, void* stream);
+// dst when backward) <-> N/2 + 1 complex bins; N a power of two in 16..2048.  f32: Float32 <->
+// ComplexF32, else Float64 <-> ComplexF64
+pa_status rfft_lines(int N, bool forward, bool f32, i64 nlines, const void* src, void* dst,
+                     void* stream);
 
 // standalone flag step on `stream`: signal the n remote words (monotonic max,
 // release at system scope) and/or wait for the n local words to reach seq

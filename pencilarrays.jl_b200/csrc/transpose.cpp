@@ -1041,7 +1041,7 @@ static pa_status staged(Plan* P, Comm* comm, const void* src, void* dst, unsigne
       bl.push_back(fused_self ? &P->self_fused : &P->peers[n].unpack);
       sp.push_back(fused_self ? src : (const void*)rbuf);
     }
-    RC(unpack_fft(nproc, bl.data(), sp.data(), dst, fft_sign, S.unpack_s));
+    RC(unpack_fft(nproc, bl.data(), sp.data(), dst, fft_sign, (flags & PA_FFT_F32) != 0, S.unpack_s));
   } else if (stage_self) {
     RC(launch_block(self.unpack, rbuf, dst, S.unpack_s, nullptr));  // local data first (:511)
   }
@@ -1098,9 +1098,14 @@ pa_status transpose(Plan* P, Comm* comm, const void* src, void* dst, unsigned fl
     return PA_EINVAL;
   }
   const int fft_sign = (flags & PA_FFT_FORWARD) ? -1 : ((flags & PA_FFT_BACKWARD) ? 1 : 0);
+  const bool fft_f32 = (flags & PA_FFT_F32) != 0;  // ComplexF32 elements (elsize 8)
+  if (fft_f32 && !fft_sign) {
+    set_error("pa_transpose: PA_FFT_F32 without PA_FFT_FORWARD / PA_FFT_BACKWARD");
+    return PA_EINVAL;
+  }
   // a fused FFT this plan cannot run is refused before anything is enqueued -- and on every
   // rank of the line alike (the peers of a refusing rank must not start the exchange)
-  if (fft_sign) RC(plan_fft_check(P));
+  if (fft_sign) RC(plan_fft_check(P, fft_f32));
   RC(ensure_state(P));
   TransposeState& S = *P->st;
   cudaStream_t user = (cudaStream_t)stream;
@@ -1121,7 +1126,7 @@ pa_status transpose(Plan* P, Comm* comm, const void* src, void* dst, unsigned fl
     // one block: the whole local array, src -> fft(permuted dest)
     if (P->length_out == 0) return PA_OK;
     const BlockCopy* b = &P->self_fused;
-    RC(unpack_fft(1, &b, &src, dst, fft_sign, user));
+    RC(unpack_fft(1, &b, &src, dst, fft_sign, fft_f32, user));
     if (timing) {
       CU(cudaEventRecord(S.t[6], user));
       S.timed_once = true;

@@ -229,12 +229,17 @@ const DeviceTransposition{T,N} = Transposition{T,N,<:Pencil,<:Pencil,
 # transpose!(t; waitall) (Transpositions.jl:170-179).
 # `fft = :forward | :backward` (GPU extension, PA_FFT_FORWARD / PA_FFT_BACKWARD): the unpack
 # and the 1-d FFT along dest's contiguous dimension -- the next step of a PencilFFTs plan --
-# run as ONE kernel (ComplexF64, power-of-two lines of 8..1024 points, staged methods).
-function Transpositions.transpose!(t::DeviceTransposition; waitall = true, fft = nothing)
+# run as ONE kernel (ComplexF64, or ComplexF32 in single precision; power-of-two lines of
+# 8..1024 points, staged methods).
+# PA_FFT_F32 for ComplexF32 elements: the plan only knows sizeof(T), and 8 bytes is Float64 too
+fft_precision_flag(::Type{T}) where {T} = T === ComplexF32 ? Cuint(32) : Cuint(0)
+
+function Transpositions.transpose!(t::DeviceTransposition{T}; waitall = true, fft = nothing) where {T}
     plan, H = plan_handle(t)
     flags = waitall ? Cuint(1) : Cuint(0)        # PA_WAITALL
     fft === :forward && (flags |= Cuint(8))
     fft === :backward && (flags |= Cuint(16))
+    fft === nothing || (flags |= fft_precision_flag(T))   # PA_FFT_F32
     ptr_or_null(A) = isempty(A) ? C_NULL : devptr(A)   # a rank may own nothing (Pencils.jl:193-218)
     check(ccall((:pa_transpose, libpa), Cint,
         (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Cuint, Ptr{Cvoid}),
@@ -242,14 +247,16 @@ function Transpositions.transpose!(t::DeviceTransposition; waitall = true, fft =
     t
 end
 
-# Whether `transpose!(t; fft)` can fuse the unpack and the FFT (pa_plan_fft_check).  The same
-# answer on every rank of the grid line (global geometry only): choose the fused or the separate
-# transpose + transform up front.
-fft_fusable(t::DeviceTransposition) =
-    ccall((:pa_plan_fft_check, libpa), Cint, (Ptr{Cvoid},), first(plan_handle(t))) == 0
+# Whether `transpose!(t; fft)` can fuse the unpack and the FFT (pa_plan_fft_check_ex, in the
+# precision of eltype).  The same answer on every rank of the grid line (global geometry only):
+# choose the fused or the separate transpose + transform up front.
+fft_fusable(t::DeviceTransposition{T}) where {T} =
+    ccall((:pa_plan_fft_check_ex, libpa), Cint, (Ptr{Cvoid}, Cuint), first(plan_handle(t)),
+          fft_precision_flag(T)) == 0
 
 # In-place 1-d FFT of `u` along its contiguous dimension (same kernel, no transposition): with
 # the two fused transposes this is a whole PencilFFTs-style 3-d transform in three kernels.
+# ComplexF64 or ComplexF32 (the flag follows eltype through transpose!).
 fft_lines!(u::PencilArray{T,N,<:CuArray}; direction = :forward) where {T,N} =
     (Transpositions.transpose!(Transposition(u, u); fft = direction); u)
 
@@ -258,8 +265,10 @@ fft_lines!(u::PencilArray{T,N,<:CuArray}; direction = :forward) where {T,N} =
 # (..., N, ...), `dest` on `Pencil(pencil(src); size_global = (..., N÷2+1, ...))`; N a power of
 # two in 16..2048.  `brfft!` is the unnormalised inverse (AbstractFFTs' `brfft`); it ignores the
 # imaginary parts of bins 1 and N÷2+1 and leaves `src` unmodified.  One kernel, no communication.
-function _rfft!(real::PencilArray{Float64,N,<:CuArray}, cplx::PencilArray{ComplexF64,N,<:CuArray},
-                flags::Cuint, src, dst) where {N}
+# Float64 <-> ComplexF64, or Float32 <-> ComplexF32 in single precision (PA_FFT_F32).
+function _rfft!(real::PencilArray{R,N,<:CuArray}, cplx::PencilArray{Complex{R},N,<:CuArray},
+                flags::Cuint, src, dst) where {R<:Union{Float64,Float32},N}
+    R === Float32 && (flags |= Cuint(32))        # PA_FFT_F32
     H = handles(pencil(real).topology)
     extra_dims(real) == extra_dims(cplx) ||
         throw(ArgumentError("incompatible extra dimensions: $(extra_dims(real)) != $(extra_dims(cplx))"))
@@ -275,6 +284,10 @@ rfft!(dest::PencilArray{ComplexF64,N,<:CuArray}, src::PencilArray{Float64,N,<:Cu
     (_rfft!(src, dest, Cuint(8), src, dest); dest)       # PA_FFT_FORWARD
 brfft!(dest::PencilArray{Float64,N,<:CuArray}, src::PencilArray{ComplexF64,N,<:CuArray}) where {N} =
     (_rfft!(dest, src, Cuint(16), src, dest); dest)      # PA_FFT_BACKWARD
+rfft!(dest::PencilArray{ComplexF32,N,<:CuArray}, src::PencilArray{Float32,N,<:CuArray}) where {N} =
+    (_rfft!(src, dest, Cuint(8), src, dest); dest)       # PA_FFT_FORWARD | PA_FFT_F32
+brfft!(dest::PencilArray{Float32,N,<:CuArray}, src::PencilArray{ComplexF32,N,<:CuArray}) where {N} =
+    (_rfft!(dest, src, Cuint(16), src, dest); dest)      # PA_FFT_BACKWARD | PA_FFT_F32
 
 # ---- host arrays: a chain of transpositions on `Array`-backed data ------------------
 # pa_host_chain_*: one submit = upload, every transpose! on the device, download;

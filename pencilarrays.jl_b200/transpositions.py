@@ -283,8 +283,14 @@ class Transposition:
         """Whether ``transpose_(self, fft=...)`` can run the unpack and the 1-d FFT as one
         kernel (``pa_plan_fft_check``).  The answer depends on the global geometry only, so it
         is the same on every rank of the grid line; when it is False, transpose and transform
-        separately."""
-        return lib.pa_plan_fft_check(self._plan.h) == _lib.PA_OK
+        separately.  complex64 arrays are asked about in single precision (``PA_FFT_F32``)."""
+        return lib.pa_plan_fft_check_ex(self._plan.h, _fft_precision_flag(self.Ai)) == _lib.PA_OK
+
+
+def _fft_precision_flag(u: PencilArray) -> int:
+    """PA_FFT_F32 for complex64 arrays: a plan only knows its element size, and 8 bytes is
+    float64 as well as complex64."""
+    return _lib.PA_FFT_F32 if u.dtype == torch.complex64 else 0
 
 
 def Waitall(t: Transposition):
@@ -298,7 +304,8 @@ def transpose_(*args, method=None, waitall=True, overlap=True, stage_self=False,
 
     ``fft="forward"`` / ``"backward"`` (GPU extension, SURVEY 8 f2): the unpack and the
     1-d complex FFT along ``dest``'s contiguous dimension -- the step a PencilFFTs-style
-    plan runs next -- execute as one kernel; ``dest`` receives the transformed array."""
+    plan runs next -- execute as one kernel; ``dest`` receives the transformed array.
+    complex128 arrays are transformed in double precision, complex64 in single."""
     if len(args) == 1 and isinstance(args[0], Transposition):
         t = args[0]
     elif len(args) == 2:
@@ -318,6 +325,7 @@ def transpose_(*args, method=None, waitall=True, overlap=True, stage_self=False,
             flags |= _lib.PA_FFT_BACKWARD
         else:
             raise ArgumentError(_lib.PA_EINVAL, "fft must be 'forward' or 'backward'")
+        flags |= _fft_precision_flag(t.Ai)
     comm = t.Pi.topology.comm.handle
     # (an empty local array may have a null data pointer: the library accepts that)
     check(lib.pa_transpose(t.plan.h, comm, C.c_void_p(t.Ai.data_ptr() or None),
@@ -331,21 +339,23 @@ transpose_bang = transpose_
 def fft_(u: PencilArray, direction="forward"):
     """In-place 1-d complex FFT of ``u`` along its contiguous (first memory) dimension: the
     first step of a PencilFFTs-style 3-d transform (the other two are ``transpose_(t,
-    fft=...)``).  Same kernel as the fused unpack+FFT, without a transposition."""
+    fft=...)``).  Same kernel as the fused unpack+FFT, without a transposition.  complex128 or
+    complex64 (single precision)."""
     t = Transposition(u, u)
     return transpose_(t, fft=direction).Ao
 
 
 def _rfft(dest: PencilArray, src: PencilArray, forward: bool):
     real, cplx = (src, dest) if forward else (dest, src)
-    if real.dtype != torch.float64 or cplx.dtype != torch.complex128:
-        raise ArgumentError(_lib.PA_EINVAL, "real array must be float64 and complex array "
-                            f"complex128: got {real.dtype} and {cplx.dtype}")
+    pairs = {(torch.float64, torch.complex128): 0, (torch.float32, torch.complex64): _lib.PA_FFT_F32}
+    if (real.dtype, cplx.dtype) not in pairs:
+        raise ArgumentError(_lib.PA_EINVAL, "real and complex arrays must be float64 and complex128, "
+                            f"or float32 and complex64: got {real.dtype} and {cplx.dtype}")
     if src.extra_dims != dest.extra_dims:
         raise ArgumentError(_lib.PA_EINVAL, "incompatible extra dimensions of PencilArrays: "
                             f"{src.extra_dims} != {dest.extra_dims}")
     ex = dest.extra_dims
-    flags = _lib.PA_FFT_FORWARD if forward else _lib.PA_FFT_BACKWARD
+    flags = (_lib.PA_FFT_FORWARD if forward else _lib.PA_FFT_BACKWARD) | pairs[(real.dtype, cplx.dtype)]
     check(lib.pa_rfft(real.pencil._h, cplx.pencil._h, len(ex), i64arr(ex), flags,
                       C.c_void_p(src.data_ptr() or None), C.c_void_p(dest.data_ptr() or None),
                       _stream_ptr()))
@@ -354,8 +364,9 @@ def _rfft(dest: PencilArray, src: PencilArray, forward: bool):
 
 def rfft_(dest: PencilArray, src: PencilArray):
     """Real-to-complex 1-d FFT along the first memory dimension (not decomposed): ``dest =
-    numpy.fft.rfft(src)`` there.  ``src``: float64 on a pencil of global size (..., N, ...);
-    ``dest``: complex128 on ``Pencil(src.pencil, size_global=(..., N//2+1, ...))``.  Step 1 of a
+    numpy.fft.rfft(src)`` there.  ``src``: float64 (float32) on a pencil of global size (..., N,
+    ...); ``dest``: complex128 (complex64) on ``Pencil(src.pencil, size_global=(..., N//2+1,
+    ...))``; float32 / complex64 run in single precision.  Step 1 of a
     PencilFFTs real-input plan; the two complex steps are ``transpose_(t, fft=...)``."""
     return _rfft(dest, src, True)
 

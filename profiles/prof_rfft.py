@@ -15,8 +15,10 @@ Two numbers per cuFFT baseline:
                 kernel outside torch's own `at::` kernels, memcpy / memset excluded).
 
 HBM bytes per line: rfft_ / brfft_ 8 N + 16 (N/2+1) (no workspace); fft_ 2 * 16 L.
+--single: Float32 <-> ComplexF32 (PA_FFT_F32) against cuFFT's float32 / complex64 transforms;
+4 N + 8 (N/2+1) and 2 * 8 L bytes per line.
 
-  python profiles/prof_rfft.py [--json out.json]
+  python profiles/prof_rfft.py [--single] [--json out.json]
 """
 import argparse
 import json
@@ -88,23 +90,27 @@ def frac(nbytes, ms):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--json", default=None)
+    ap.add_argument("--single", action="store_true", help="Float32 / ComplexF32 instead of Float64 / ComplexF64")
     args = ap.parse_args()
+    rt, ct, rs = (torch.float32, torch.complex64, 4) if args.single else (torch.float64, torch.complex128, 8)
     name, power = card()
     print(f"card: {name}; power.limit, clocks.max.sm: {power}; HBM peak used for fractions: {PEAK} GB/s",
           flush=True)
     rows = [dict(card=name, power_limit_and_max_sm_clock=power, peak_gbs=PEAK)]
+    if args.single:
+        rows[0]["precision"] = "single"
     topo = pa.MPITopology(pa.COMM_SELF, (1, 1))
     for dims in ((512, 512, 512), (2048, 512, 256)):
         N, L = dims[0], dims[0] // 2
         nlines = math.prod(dims[1:])
         pr = pa.Pencil(topo, dims, (2, 3))
         pc = pa.Pencil(pr, size_global=(L + 1,) + dims[1:])
-        xr = pa.PencilArray.undef(torch.float64, pr)
-        xc = pa.PencilArray.undef(torch.complex128, pc)
-        back = pa.PencilArray.undef(torch.float64, pr)
+        xr = pa.PencilArray.undef(rt, pr)
+        xc = pa.PencilArray.undef(ct, pc)
+        back = pa.PencilArray.undef(rt, pr)
         xr.data.normal_()
         pa.rfft_(xc, xr)
-        nb = nlines * (8 * N + 16 * (L + 1))
+        nb = nlines * (rs * N + 2 * rs * (L + 1))
         ms_r = timed(lambda: pa.rfft_(xc, xr))
         ms_b = timed(lambda: pa.brfft_(back, xc))
         del back
@@ -115,10 +121,10 @@ def main():
         (ms_kr, names_r), (ms_kb, names_b) = library_kernels_ms(cr), library_kernels_ms(cb)
         # the in-repo yardstick: the complex fft_ at the same line length L, same number of lines
         pl = pa.Pencil(topo, (L,) + dims[1:], (2, 3))
-        u = pa.PencilArray.undef(torch.complex128, pl)
-        u.data.view(torch.float64).normal_()
+        u = pa.PencilArray.undef(ct, pl)
+        u.data.view(rt).normal_()
         ms_f = timed(lambda: pa.fft_(u, "forward"))
-        nb_f = nlines * 2 * 16 * L
+        nb_f = nlines * 2 * 2 * rs * L
         del u
         r = dict(dims=dims, N=N, L=L, rfft_ms=round(ms_r, 4), rfft_frac_of_hbm=frac(nb, ms_r),
                  brfft_ms=round(ms_b, 4), brfft_frac_of_hbm=frac(nb, ms_b),
@@ -140,8 +146,8 @@ def main():
     pxc = pa.Pencil(pxr, size_global=(dims[0] // 2 + 1,) + dims[1:])
     pyc = pa.Pencil(pxc, decomp_dims=(1, 3), permute=pa.Permutation(2, 1, 3))
     pzc = pa.Pencil(pyc, decomp_dims=(1, 2), permute=pa.Permutation(3, 2, 1))
-    uxr = pa.PencilArray.undef(torch.float64, pxr)
-    uxc, uyc, uzc = (pa.PencilArray.undef(torch.complex128, p) for p in (pxc, pyc, pzc))
+    uxr = pa.PencilArray.undef(rt, pxr)
+    uxc, uyc, uzc = (pa.PencilArray.undef(ct, p) for p in (pxc, pyc, pzc))
     uxr.data.normal_()
     t_xy, t_yz = pa.Transposition(uyc, uxc), pa.Transposition(uzc, uyc)
     t_zy, t_yx = pa.Transposition(uyc, uzc), pa.Transposition(uxc, uyc)
