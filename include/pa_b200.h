@@ -375,6 +375,33 @@ pa_status pa_rfft(const pa_pencil* real, const pa_pencil* cplx, int n_extra,
                   const int64_t* extra_dims, unsigned flags, const void* src, void* dst,
                   void* stream);
 
+/* ---- fused transpose + complex-to-real line transform ---------------------------
+ * The last step of a PencilFFTs real-input backward transform in one kernel per rank after
+ * the exchange: dst = brfft(transpose(src)), with no complex x-pencil array in between.
+ * `plan` is the ordinary complex plan y-pencil -> x-pencil (ComplexF64, elsize 16; with
+ * PA_FFT_F32 ComplexF32, elsize 8); `real` is the real counterpart of the plan's output pencil,
+ * related to it as `real` and `cplx` of pa_rfft (same topology object, decomposition and
+ * permutation; N along perm[1], N/2+1 in the output pencil; that axis not decomposed).
+ *   src: the y-pencil ComplexF64 (ComplexF32) array of the plan, left unmodified;
+ *   dst: the Float64 (Float32) array on `real`, = N * irfft(transpose(src), N) along perm[1],
+ *        unnormalised like FFTW's brfft; the imaginary parts of bins 0 and N/2 are ignored.
+ * N: power of two in 16..2048.  flags: any of PA_WAITALL, PA_NO_OVERLAP, PA_STAGE_SELF and
+ * PA_FFT_F32 -- the direction is implied, any other bit is PA_EINVAL.  Ordering, waitall,
+ * pa_wait, NULL pointers for empty local arrays and the staged methods behave as for
+ * pa_transpose with a fused FFT; PA_PEER_PUT / PA_PEER_GET are refused.  src and dst must not
+ * overlap, dst 16-byte aligned.  Every refusal (PA_EINCOMPAT: pencils not related as above;
+ * PA_EINVAL: other bad arguments, or a geometry pa_plan_brfft_check refuses) happens before
+ * anything is enqueued, and a refused geometry is refused on every rank of the grid line.   */
+pa_status pa_transpose_brfft(pa_plan* plan, pa_comm* comm, const pa_pencil* real,
+                             const void* src, void* dst, unsigned flags, void* stream);
+/* Can pa_transpose_brfft run on this plan?  pa_plan_fft_check_ex's question for the fused
+ * complex-to-real transform (line length N/2+1, at most 8 blocks per line, the destination
+ * strides, and a staged method: PA_PEER_PUT / PA_PEER_GET are refused when the plan exchanges
+ * data): the same answer on every rank of the grid line.  Only PA_FFT_F32 of `flags`
+ * matters.  Cached per plan and precision, apart from pa_plan_fft_check's verdicts.
+ * Host-only; no device needed.                                                            */
+pa_status pa_plan_brfft_check(const pa_plan* plan, unsigned flags);
+
 /* ---- host chains -----------------------------------------------------------
  * A sequence of transpositions applied to HOST arrays (plan i+1 consumes what
  * plan i produces): one submit = upload of `host_src`, every transpose! on the

@@ -125,6 +125,8 @@ SIGNATURES = {
     "pa_plan_fft_check_ex": (C.c_int, [_P, C.c_uint]),
     "pa_transpose_host": (C.c_int, [_P, _P, _P, _P, C.c_uint]),
     "pa_rfft": (C.c_int, [_P, _P, C.c_int, _I64P, C.c_uint, _P, _P, _P]),
+    "pa_transpose_brfft": (C.c_int, [_P, _P, _P, _P, _P, C.c_uint, _P]),
+    "pa_plan_brfft_check": (C.c_int, [_P, C.c_uint]),
     "pa_host_chain_create": (C.c_int, [C.c_int, C.POINTER(_P), _P, C.POINTER(_P)]),
     "pa_host_chain_destroy": (None, [_P]),
     "pa_host_chain_submit": (C.c_int, [_P, _P, _P, _I64P]),

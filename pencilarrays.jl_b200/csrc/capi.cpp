@@ -673,60 +673,62 @@ pa_status pa_transpose_host(pa_plan* plan, pa_comm* comm, const void* host_src, 
 }
 
 // ---- real-to-complex line transforms ------------------------------------------------
-// Every check runs on the host before any device call.
-static pa_status rfft_checks(const pa_pencil* real, const pa_pencil* cplx, int n_extra,
-                             const int64_t* extra_dims, unsigned flags, const void* src,
-                             const void* dst, int* N_out, i64* nlines_out) {
+// Every check runs on the host before any device call.  `who` prefixes the messages; with
+// check_ptrs false the caller checks src / dst itself (pa_transpose_brfft: src is not on `cplx`).
+static pa_status rfft_checks(const char* who, const pa_pencil* real, const pa_pencil* cplx,
+                             int n_extra, const int64_t* extra_dims, unsigned flags,
+                             const void* src, const void* dst, bool check_ptrs, int* N_out,
+                             i64* nlines_out) {
   if (!real || !cplx) {
-    set_error("pa_rfft: null pencil");
+    set_error("%s: null pencil", who);
     return PA_EINVAL;
   }
   const Pencil& R = *real->p;
   const Pencil& Cp = *cplx->p;
   if (R.topo != Cp.topo || R.N != Cp.N) {
-    set_error("pa_rfft: the pencils must share their topology and number of dimensions");
+    set_error("%s: the pencils must share their topology and number of dimensions", who);
     return PA_EINCOMPAT;
   }
   const int M = R.topo->M;
   for (int i = 0; i < M; ++i)
     if (R.decomp[i] != Cp.decomp[i]) {
-      set_error("pa_rfft: the pencils have different decompositions");
+      set_error("%s: the pencils have different decompositions", who);
       return PA_EINCOMPAT;
     }
   for (int d = 0; d < R.N; ++d)
     if (R.perm[d] != Cp.perm[d]) {
-      set_error("pa_rfft: the pencils have different permutations");
+      set_error("%s: the pencils have different permutations", who);
       return PA_EINCOMPAT;
     }
   const int ax = R.perm[0];  // logical dim of the first memory dim: the transform axis
   for (int i = 0; i < M; ++i)
     if (R.decomp[i] == ax) {
-      set_error("pa_rfft: the transform axis (logical dim %d) is decomposed", ax + 1);
+      set_error("%s: the transform axis (logical dim %d) is decomposed", who, ax + 1);
       return PA_EINCOMPAT;
     }
   for (int d = 0; d < R.N; ++d)
     if (d != ax && R.size_global[d] != Cp.size_global[d]) {
-      set_error("pa_rfft: global sizes differ along dim %d", d + 1);
+      set_error("%s: global sizes differ along dim %d", who, d + 1);
       return PA_EINCOMPAT;
     }
   const i64 N = R.size_global[ax];
   if (Cp.size_global[ax] != N / 2 + 1) {
-    set_error("pa_rfft: the complex pencil has %lld points along the transform axis, expected "
-              "N/2+1 = %lld", (long long)Cp.size_global[ax], (long long)(N / 2 + 1));
+    set_error("%s: the complex pencil has %lld points along the transform axis, expected "
+              "N/2+1 = %lld", who, (long long)Cp.size_global[ax], (long long)(N / 2 + 1));
     return PA_EINCOMPAT;
   }
   const unsigned dir = flags & ~PA_FFT_F32;
   if (dir != PA_FFT_FORWARD && dir != PA_FFT_BACKWARD) {
-    set_error("pa_rfft: flags must be exactly PA_FFT_FORWARD or PA_FFT_BACKWARD, optionally "
-              "with PA_FFT_F32");
+    set_error("%s: flags must be exactly PA_FFT_FORWARD or PA_FFT_BACKWARD, optionally "
+              "with PA_FFT_F32", who);
     return PA_EINVAL;
   }
   if (N < 16 || N > 2048 || (N & (N - 1))) {
-    set_error("pa_rfft: N = %lld is not a power of two in 16..2048", (long long)N);
+    set_error("%s: N = %lld is not a power of two in 16..2048", who, (long long)N);
     return PA_EINVAL;
   }
   if (n_extra < 0 || (n_extra > 0 && !extra_dims) || R.N + n_extra > PA_MAX_DIMS) {
-    set_error("pa_rfft: %d extra dims on a %d-d pencil (at most %d dims in all)", n_extra, R.N,
+    set_error("%s: %d extra dims on a %d-d pencil (at most %d dims in all)", who, n_extra, R.N,
               PA_MAX_DIMS);
     return PA_EINVAL;
   }
@@ -737,7 +739,7 @@ static pa_status rfft_checks(const pa_pencil* real, const pa_pencil* cplx, int n
     if (d != ax) nlines *= hi[d] - lo[d];
   for (int i = 0; i < n_extra; ++i) {
     if (extra_dims[i] < 0) {
-      set_error("pa_rfft: negative extra dim");
+      set_error("%s: negative extra dim", who);
       return PA_EINVAL;
     }
     nlines *= extra_dims[i];
@@ -746,18 +748,18 @@ static pa_status rfft_checks(const pa_pencil* real, const pa_pencil* cplx, int n
   const i64 rs = (flags & PA_FFT_F32) ? 4 : 8;  // bytes of a real element; a complex one is 2 rs
   const i64 real_bytes = nlines * N * rs, cplx_bytes = nlines * (N / 2 + 1) * 2 * rs;
   const i64 src_bytes = fwd ? real_bytes : cplx_bytes, dst_bytes = fwd ? cplx_bytes : real_bytes;
-  if (nlines > 0) {
+  if (check_ptrs && nlines > 0) {
     if (!src || !dst) {
-      set_error("pa_rfft: null array pointer for a non-empty local array");
+      set_error("%s: null array pointer for a non-empty local array", who);
       return PA_EINVAL;
     }
     const uintptr_t s = (uintptr_t)src, d = (uintptr_t)dst;
     if (s < d + (uintptr_t)dst_bytes && d < s + (uintptr_t)src_bytes) {
-      set_error("pa_rfft: src and dst overlap");
+      set_error("%s: src and dst overlap", who);
       return PA_EINVAL;
     }
     if ((s | d) & 15) {
-      set_error("pa_rfft: src and dst must be 16-byte aligned");
+      set_error("%s: src and dst must be 16-byte aligned", who);
       return PA_EINVAL;
     }
   }
@@ -772,12 +774,76 @@ pa_status pa_rfft(const pa_pencil* real, const pa_pencil* cplx, int n_extra,
   GUARD({
     int N = 0;
     i64 nlines = 0;
-    pa_status s = rfft_checks(real, cplx, n_extra, extra_dims, flags, src, dst, &N, &nlines);
+    pa_status s =
+        rfft_checks("pa_rfft", real, cplx, n_extra, extra_dims, flags, src, dst, true, &N, &nlines);
     if (s != PA_OK) return s;
     s = need_gpu();
     if (s != PA_OK) return s;
     return rfft_lines(N, (flags & ~PA_FFT_F32) == PA_FFT_FORWARD, (flags & PA_FFT_F32) != 0, nlines,
                       src, dst, stream);
+  })
+}
+
+static pa_status transpose_brfft(pa_plan* plan, pa_comm* comm, const pa_pencil* real,
+                                 const void* src, void* dst, unsigned flags, void* stream) {
+  if (!plan) {
+    set_error("pa_transpose_brfft: null plan");
+    return PA_EINVAL;
+  }
+  if (flags & ~(PA_WAITALL | PA_NO_OVERLAP | PA_STAGE_SELF | PA_FFT_F32)) {
+    set_error("pa_transpose_brfft: flags may combine PA_WAITALL, PA_NO_OVERLAP, PA_STAGE_SELF "
+              "and PA_FFT_F32 only (the direction is implied)");
+    return PA_EINVAL;
+  }
+  Plan& P = *plan->p;
+  const bool f32 = (flags & PA_FFT_F32) != 0;
+  if (P.elsize != (f32 ? 8 : 16)) {
+    set_error(f32 ? "pa_transpose_brfft: PA_FFT_F32 takes a ComplexF32 (elsize 8) plan"
+                  : "pa_transpose_brfft: a ComplexF64 (elsize 16) plan, or PA_FFT_F32 for ComplexF32");
+    return PA_EINVAL;
+  }
+  // `real` against the plan's output pencil, as pa_rfft relates them; the pointers below
+  const pa_pencil out{P.pout};
+  int N = 0;
+  i64 nlines = 0;
+  pa_status s = rfft_checks("pa_transpose_brfft", real, &out, P.n_extra, P.extra,
+                            PA_FFT_BACKWARD | (flags & PA_FFT_F32), nullptr, nullptr, false, &N,
+                            &nlines);
+  if (s != PA_OK) return s;
+  const i64 src_bytes = P.length_in * P.elsize, dst_bytes = nlines * N * (f32 ? 4 : 8);
+  if ((!src && src_bytes > 0) || (!dst && dst_bytes > 0)) {
+    set_error("pa_transpose_brfft: null array pointer for a non-empty local array");
+    return PA_EINVAL;
+  }
+  const uintptr_t a = (uintptr_t)src, b = (uintptr_t)dst;
+  if (src_bytes > 0 && dst_bytes > 0 && a < b + (uintptr_t)dst_bytes && b < a + (uintptr_t)src_bytes) {
+    set_error("pa_transpose_brfft: src and dst overlap");
+    return PA_EINVAL;
+  }
+  if (dst_bytes > 0 && (b & 15)) {
+    set_error("pa_transpose_brfft: dst must be 16-byte aligned");
+    return PA_EINVAL;
+  }
+  // the same verdict on every rank of the grid line: a refusal launches nothing anywhere
+  s = plan_brfft_check(&P, f32);
+  if (s != PA_OK) return s;
+  s = need_gpu();
+  if (s != PA_OK) return s;
+  return transpose(&P, comm ? comm->p : nullptr, src, dst, flags, stream, true);
+}
+
+pa_status pa_transpose_brfft(pa_plan* plan, pa_comm* comm, const pa_pencil* real, const void* src,
+                             void* dst, unsigned flags, void* stream) {
+  GUARD({ return transpose_brfft(plan, comm, real, src, dst, flags, stream); })
+}
+
+pa_status pa_plan_brfft_check(const pa_plan* plan, unsigned flags) {
+  GUARD({
+    if (!plan) {
+      set_error("pa_plan_brfft_check: null plan");
+      return PA_EINVAL;
+    }
+    return plan_brfft_check(plan->p, (flags & PA_FFT_F32) != 0);
   })
 }
 

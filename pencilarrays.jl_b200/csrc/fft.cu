@@ -139,6 +139,59 @@ __device__ __forceinline__ int fft_pos(int k) {
   }
 }
 
+// The gather of every block's rows of one line into shared memory (thread (c, r) owns column
+// c and the rows r, r + RS, ... of every block).  Any total row count: the blocks tile it.
+template <int C, class T>
+__device__ __forceinline__ void gather_rows(const FftParams& p, const long long* so_off, long long x0,
+                                            int c, int r, int ncol, cplx_t<T>* line) {
+  using V = typename Vec2<T>::type;
+  constexpr int RS = FFT_THREADS / C;
+  constexpr int U = 8;
+#pragma unroll
+  for (int b = 0; b < FFT_MAXB; ++b) {
+    if (b < p.nb) {
+      const FftBlock& B = p.blk[b];
+      const char* s = B.src + so_off[b] + (x0 + c) * B.ssx;
+      const int ey = B.ey, y0 = B.y0;
+      const long long ssy = B.ssy;
+      for (int y = r; y < ey; y += U * RS) {
+        V v[U];
+#pragma unroll
+        for (int k = 0; k < U; ++k) {
+          const int yy = y + k * RS;
+          if (c < ncol && yy < ey) v[k] = __ldcs(reinterpret_cast<const V*>(s + (long long)yy * ssy));
+        }
+#pragma unroll
+        for (int k = 0; k < U; ++k) {
+          const int yy = y + k * RS;
+          if (c < ncol && yy < ey) line[pa_fft::pad_index(y0 + yy)] = cplx_t<T>{v[k].x, v[k].y};
+        }
+      }
+    }
+  }
+}
+
+// CTA -> (first column x0, byte offsets of the outer coordinates in every block and in dst)
+__device__ __forceinline__ long long cta_offsets(const FftParams& p, int C, long long* so_off,
+                                                 long long* d_off) {
+  unsigned long long bid = blockIdx.x;
+  const long long x0 = (long long)(bid % p.tiles_x) * C;
+  bid /= p.tiles_x;
+#pragma unroll
+  for (int b = 0; b < FFT_MAXB; ++b) so_off[b] = 0;
+  *d_off = 0;
+#pragma unroll 1
+  for (int i = 0; i < p.no; ++i) {
+    const long long k = (long long)(bid % (unsigned long long)p.oe[i]);
+    bid /= (unsigned long long)p.oe[i];
+    *d_off += k * p.dso[i];
+#pragma unroll
+    for (int b = 0; b < FFT_MAXB; ++b)
+      if (b < p.nb) so_off[b] += k * p.blk[b].so[i];
+  }
+  return x0;
+}
+
 template <int LOGL, int C, class T>
 __global__ void __launch_bounds__(FFT_THREADS) k_unpack_fft(const __grid_constant__ FftParams p) {
   using cx = cplx_t<T>;
@@ -147,22 +200,8 @@ __global__ void __launch_bounds__(FFT_THREADS) k_unpack_fft(const __grid_constan
   extern __shared__ __align__(16) unsigned char fft_smem[];
   cx* sm = reinterpret_cast<cx*>(fft_smem);
   const int t = threadIdx.x;
-  unsigned long long bid = blockIdx.x;
-  const long long x0 = (long long)(bid % p.tiles_x) * C;
-  bid /= p.tiles_x;
-  long long so_off[FFT_MAXB];
-#pragma unroll
-  for (int b = 0; b < FFT_MAXB; ++b) so_off[b] = 0;
-  long long d_off = 0;
-#pragma unroll 1
-  for (int i = 0; i < p.no; ++i) {
-    const long long k = (long long)(bid % (unsigned long long)p.oe[i]);
-    bid /= (unsigned long long)p.oe[i];
-    d_off += k * p.dso[i];
-#pragma unroll
-    for (int b = 0; b < FFT_MAXB; ++b)
-      if (b < p.nb) so_off[b] += k * p.blk[b].so[i];
-  }
+  long long so_off[FFT_MAXB], d_off;
+  const long long x0 = cta_offsets(p, C, so_off, &d_off);
   const int ncol = (int)((p.ex - x0) < C ? (p.ex - x0) : C);
   const int pitch = p.pitch;
 
@@ -213,29 +252,7 @@ __global__ void __launch_bounds__(FFT_THREADS) k_unpack_fft(const __grid_constan
         for (int q = 0; q < R1; ++q) line[pa_fft::pad_index(r + q * RS)] = a[q];
       }
     } else {
-      constexpr int U = 8;
-#pragma unroll
-      for (int b = 0; b < FFT_MAXB; ++b) {
-        if (b < p.nb) {
-          const FftBlock& B = p.blk[b];
-          const char* s = B.src + so_off[b] + (x0 + c) * B.ssx;
-          const int ey = B.ey, y0 = B.y0;
-          const long long ssy = B.ssy;
-          for (int y = r; y < ey; y += U * RS) {
-            V v[U];
-#pragma unroll
-            for (int k = 0; k < U; ++k) {
-              const int yy = y + k * RS;
-              if (c < ncol && yy < ey) v[k] = __ldcs(reinterpret_cast<const V*>(s + (long long)yy * ssy));
-            }
-#pragma unroll
-            for (int k = 0; k < U; ++k) {
-              const int yy = y + k * RS;
-              if (c < ncol && yy < ey) line[pa_fft::pad_index(y0 + yy)] = cx{v[k].x, v[k].y};
-            }
-          }
-        }
-      }
+      gather_rows<C, T>(p, so_off, x0, c, r, ncol, line);
     }
   }
   __syncthreads();
@@ -367,6 +384,71 @@ __global__ void __launch_bounds__(FFT_THREADS) k_rfft(const __grid_constant__ Rf
   }
 }
 
+// ---- fused unpack + complex-to-real line transform (pa_transpose_brfft, DESIGN §3e) ----
+// The gather of k_unpack_fft (the N/2 + 1 = L + 1 bins of each line from every block), then the
+// backward half of k_rfft on the shared-memory lines: its pre-pass, its L-point passes and its
+// store of the N reals.  p.dst / p.dsx / p.dso address the REAL destination (fft_geometry
+// converts them); p.L = N / 2; p.tw = W_N.  Same lines per CTA as k_rfft for that N.
+template <int LOGL, int C, class T>
+__global__ void __launch_bounds__(FFT_THREADS) k_unpack_brfft(const __grid_constant__ FftParams p) {
+  using cx = cplx_t<T>;
+  using V = typename Vec2<T>::type;
+  constexpr int L = 1 << LOGL;
+  constexpr int RS = FFT_THREADS / C;
+  constexpr int P = L / 2 + 1;  // pairs (k, L - k) per line
+  extern __shared__ __align__(16) unsigned char fft_smem[];
+  cx* sm = reinterpret_cast<cx*>(fft_smem);
+  const int t = threadIdx.x;
+  long long so_off[FFT_MAXB], d_off;
+  const long long x0 = cta_offsets(p, C, so_off, &d_off);
+  const int ncol = (int)((p.ex - x0) < C ? (p.ex - x0) : C);
+  const int pitch = p.pitch;
+  const V* twp = reinterpret_cast<const V*>(p.tw);
+  auto twN = [twp](int k) {
+    const V w = __ldg(twp + k);
+    return cx{w.x, w.y};
+  };
+  auto twL = [twp](int i) {  // W_L^i = W_N^(2i)
+    const V w = __ldg(twp + 2 * i);
+    return cx{w.x, w.y};
+  };
+
+  // ---- gather: transposing, or linear (lines contiguous in the source) ----
+  {
+    const int c = p.linear ? t / RS : t % C, r = p.linear ? t % RS : t / C;
+    gather_rows<C, T>(p, so_off, x0, c, r, ncol, sm + c * pitch);
+  }
+  __syncthreads();
+
+  // ---- pre-pass in place (k_rfft<..., false>): a thread owns the slots k and L - k ----
+#pragma unroll 1
+  for (int w0 = 0; w0 < C * P; w0 += FFT_THREADS) {
+    const int w = w0 + t, c = w / P, k = w % P;
+    if (w < C * P && c < ncol) {
+      cx* line = sm + c * pitch;
+      cx zk, zl;
+      pa_fft::brfft_pre_pair(k, line[pa_fft::pad_index(k)], line[pa_fft::pad_index(L - k)], twN(k), &zk,
+                             &zl);
+      line[pa_fft::pad_index(k)] = zk;
+      if (k > 0) line[pa_fft::pad_index(L - k)] = zl;
+    }
+  }
+  __syncthreads();
+
+  fft_passes<LOGL, LOGL, C>(sm, pitch, ncol, 1, twL);
+
+  // ---- store: z[n] = x[2n] + i x[2n+1], the N reals of a line as L pair stores ----
+  char* d = p.dst + x0 * p.dsx + d_off;
+#pragma unroll
+  for (int w0 = 0; w0 < C * L; w0 += FFT_THREADS) {
+    const int w = w0 + t, c = w >> LOGL, n = w & (L - 1);
+    if (c < ncol) {
+      const cx v = sm[c * pitch + pa_fft::pad_index(fft_pos<LOGL, LOGL>(n))];
+      __stcs(reinterpret_cast<V*>(d + c * p.dsx) + n, vec2(v.x, v.y));
+    }
+  }
+}
+
 // forward twiddle table W_L^k per (device, L, precision), computed once in extended precision
 // and rounded once to double (cplx) or float (cplxf)
 template <class T>
@@ -411,8 +493,10 @@ static const void* twiddles(int L, bool f32) {
 // together they must tile the destination box), and every check of it.  srcs / dst may be
 // NULL: plan_fft_check runs this on the blocks a peer would see, without arrays.  *grid = 0:
 // nothing to do on this rank.  f32: ComplexF32 elements (PA_FFT_F32), else ComplexF64.
+// brfft (k_unpack_brfft): the lines are M = N/2 + 1 bins, and `dst` is the REAL array of N
+// reals per line in place of the complex one the blocks describe (DESIGN §3e).
 static pa_status fft_geometry(int nb, const BlockCopy* const* blocks, const void* const* srcs,
-                              void* dst, bool f32, FftParams& p, int* C_out,
+                              void* dst, bool f32, bool brfft, FftParams& p, int* C_out,
                               unsigned long long* grid_out) {
   const i64 es = f32 ? 8 : 16;  // element bytes
   memset(&p, 0, sizeof p);
@@ -512,10 +596,16 @@ static pa_status fft_geometry(int nb, const BlockCopy* const* blocks, const void
       if (i != jy && i != jx && B.raw[i].e > 1) F.so[o++] = B.raw[i].ss * es;
     L += B.raw[jy].e;
   }
+  const i64 M = L;  // rows per line (brfft: bins)
+  if (brfft) L = M - 1;  // the N/2-point complex FFT of a real line of N = 2 (M - 1)
   int logL = 0;
   while ((1LL << logL) < L) ++logL;
   if ((1LL << logL) != L || L < 8 || L > 1024) {
-    set_error("fused FFT: line length %lld is not a power of two in 8..1024", (long long)L);
+    if (brfft)
+      set_error("fused brfft: %lld bins per line are not N/2+1 with N a power of two in 16..2048",
+                (long long)M);
+    else
+      set_error("fused FFT: line length %lld is not a power of two in 8..1024", (long long)L);
     return PA_EINVAL;
   }
   // the blocks must tile [0, L) without gaps
@@ -549,12 +639,35 @@ static pa_status fft_geometry(int nb, const BlockCopy* const* blocks, const void
     }
   p.L = (int)L;
   p.logL = logL;
-  p.pitch = pa_fft::padded_pitch((int)L);
+  p.pitch = pa_fft::padded_pitch((int)M);
+  if (brfft) {
+    // The line dim is the destination's first memory dim (stride 1) and whole (the blocks tile
+    // [0, M)), so every other destination offset and stride is a multiple of M elements: line k
+    // of the complex array starts at k M complex elements, and at k N reals in the real array
+    // of the same shape otherwise.  Only dims of extent > 1 are addressed.
+    const i64 N = 2 * L, rs = es / 2;
+    auto to_real = [&](long long off, long long* out) {
+      if (off % M != 0) {
+        set_error("fused brfft: a destination stride or offset is not a multiple of the %lld bins "
+                  "of a line", (long long)M);
+        return false;
+      }
+      *out = off / M * N * rs;
+      return true;
+    };
+    long long v = 0;
+    if (!to_real(min_doff, &v)) return PA_EINVAL;
+    p.dst = dst ? (char*)dst + v : nullptr;
+    p.dsx = N * rs;
+    if (jx >= 0 && p.ex > 1 && !to_real(ref->raw[jx].ds, &p.dsx)) return PA_EINVAL;
+    for (int o = 0; o < p.no; ++o)
+      if (!to_real(p.dso[o] / es, &p.dso[o])) return PA_EINVAL;
+  }
   // tunable "fft_lines" = 4: 4 lines per CTA also for 256- / 512-point lines (64-byte gathers,
   // first pass of radix 4 / 8 in registers, half the shared memory per CTA); double precision
-  // only -- single precision always takes fft_lines_f32
+  // only -- single precision always takes fft_lines_f32.  brfft: the lines per CTA of k_rfft
   const int C = f32 ? fft_lines_f32(logL)
-                    : ((g_tun.fft_lines == 4 && logL >= 8) ? 4 : fft_lines(logL));
+                    : ((!brfft && g_tun.fft_lines == 4 && logL >= 8) ? 4 : fft_lines(logL));
   p.tiles_x = (unsigned)((p.ex + C - 1) / C);
   unsigned long long grid = p.tiles_x;
   for (int i = 0; i < p.no; ++i) grid *= (unsigned long long)p.oe[i];
@@ -574,7 +687,7 @@ pa_status unpack_fft(int nb, const BlockCopy* const* blocks, const void* const* 
   FftParams p;
   int C = 0;
   unsigned long long grid = 0;
-  pa_status s = fft_geometry(nb, blocks, srcs, dst, f32, p, &C, &grid);
+  pa_status s = fft_geometry(nb, blocks, srcs, dst, f32, false, p, &C, &grid);
   if (s != PA_OK || grid == 0) return s;
   const int logL = p.logL;
   p.sign = sign < 0 ? -1 : 1;
@@ -629,39 +742,84 @@ pa_status unpack_fft(int nb, const BlockCopy* const* blocks, const void* const* 
   return PA_OK;
 }
 
-// Can pa_transpose fuse the FFT into this plan's unpack?  Every rank of a grid line must
-// get the same answer: a rank that refused before the exchange while its peers went ahead
-// would leave them waiting on flags it never sets.  So the answer depends on the global
-// geometry only: the blocks that EVERY rank of the line would gather -- each rank's plan
-// rebuilt from the pencils with that rank's coordinates -- with the self block read from src
-// and staged through recv_buf alike.  Cached per plan, per precision (f32: ComplexF32) and per
-// value of tunable fft_lines.
-pa_status plan_fft_check(Plan* P, bool f32) {
-  const int q = f32 ? 1 : 0;
-  if (P->fft_check_lines[q] == g_tun.fft_lines) {
-    if (P->fft_check[q] != PA_OK) set_error("%s", P->fft_check_err[q].c_str());
-    return P->fft_check[q];
+pa_status unpack_brfft(int nb, const BlockCopy* const* blocks, const void* const* srcs, void* dst,
+                       bool f32, void* stream) {
+  // (pa_transpose_brfft has already asked plan_brfft_check for every rank of the line)
+  FftParams p;
+  int C = 0;
+  unsigned long long grid = 0;
+  pa_status s = fft_geometry(nb, blocks, srcs, dst, f32, true, p, &C, &grid);
+  if (s != PA_OK || grid == 0) return s;
+  const int logL = p.logL;
+  p.sign = 1;
+  p.tw = twiddles(2 * p.L, f32);
+  if (!p.tw) {
+    set_error("fused brfft: twiddle table allocation failed");
+    cudaGetLastError();
+    return PA_ENOMEM;
   }
-  auto verdict = [&](pa_status s) {
-    P->fft_check[q] = s;
-    P->fft_check_err[q] = s == PA_OK ? std::string() : std::string(last_error());
-    P->fft_check_lines[q] = g_tun.fft_lines;
-    return s;
+  const size_t smem = (f32 ? sizeof(pa_fft::cplxf) : sizeof(cplx)) * (size_t)C * p.pitch;
+  cudaError_t e = cudaSuccess;
+  auto launch = [&](auto kern) {
+    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout,
+                         cudaSharedmemCarveoutMaxShared);
+    cudaGetLastError();
+    kern<<<(unsigned)grid, FFT_THREADS, smem, (cudaStream_t)stream>>>(p);
+    e = cudaGetLastError();
   };
+  if (f32) {
+    switch (logL) {
+      case 3: launch(k_unpack_brfft<3, 16, float>); break;
+      case 4: launch(k_unpack_brfft<4, 16, float>); break;
+      case 5: launch(k_unpack_brfft<5, 16, float>); break;
+      case 6: launch(k_unpack_brfft<6, 16, float>); break;
+      case 7: launch(k_unpack_brfft<7, 16, float>); break;
+      case 8: launch(k_unpack_brfft<8, 16, float>); break;
+      case 9: launch(k_unpack_brfft<9, 16, float>); break;
+      default: launch(k_unpack_brfft<10, 8, float>); break;
+    }
+  } else {
+    switch (logL) {
+      case 3: launch(k_unpack_brfft<3, 8, double>); break;
+      case 4: launch(k_unpack_brfft<4, 8, double>); break;
+      case 5: launch(k_unpack_brfft<5, 8, double>); break;
+      case 6: launch(k_unpack_brfft<6, 8, double>); break;
+      case 7: launch(k_unpack_brfft<7, 8, double>); break;
+      case 8: launch(k_unpack_brfft<8, 8, double>); break;
+      case 9: launch(k_unpack_brfft<9, 8, double>); break;
+      default: launch(k_unpack_brfft<10, 4, double>); break;
+    }
+  }
+  if (e != cudaSuccess) {
+    set_error("fused brfft kernel launch failed: %s", cudaGetErrorString(e));
+    return PA_ECUDA;
+  }
+  count_launch();
+  return PA_OK;
+}
+
+// Can pa_transpose fuse the FFT (brfft: pa_transpose_brfft the complex-to-real transform) into
+// this plan's unpack?  Every rank of a grid line must get the same answer: a rank that refused
+// before the exchange while its peers went ahead would leave them waiting on flags it never
+// sets.  So the answer depends on the global geometry only: the blocks that EVERY rank of the
+// line would gather -- each rank's plan rebuilt from the pencils with that rank's coordinates --
+// with the self block read from src and staged through recv_buf alike.
+static pa_status fused_check(Plan* P, bool f32, bool brfft) {
   if (!f32 && P->elsize != 16) {
     set_error("fused FFT: ComplexF64 (16-byte) elements only");
-    return verdict(PA_EINVAL);
+    return PA_EINVAL;
   }
   if (f32 && P->elsize != 8) {
     set_error("fused FFT: PA_FFT_F32 takes ComplexF32 (8-byte) elements only");
-    return verdict(PA_EINVAL);
+    return PA_EINVAL;
   }
   FftParams p;
   int C = 0;
   unsigned long long grid = 0;
   if (P->dim < 0 || P->nproc == 1) {
     const BlockCopy* b = &P->self_fused;
-    return verdict(fft_geometry(1, &b, nullptr, nullptr, f32, p, &C, &grid));
+    return fft_geometry(1, &b, nullptr, nullptr, f32, brfft, p, &C, &grid);
   }
   for (int n = 0; n < P->nproc; ++n) {
     std::unique_ptr<Plan> hold;
@@ -676,7 +834,7 @@ pa_status plan_fft_check(Plan* P, bool f32) {
       pout->topo = topo;
       Plan* q = nullptr;
       pa_status s = build_plan(pin, pout, P->n_extra, P->extra, P->elsize, P->method, &q);
-      if (s != PA_OK) return verdict(s);
+      if (s != PA_OK) return s;
       hold.reset(q);
       Q = q;
     }
@@ -684,17 +842,51 @@ pa_status plan_fft_check(Plan* P, bool f32) {
       std::vector<const BlockCopy*> bl;
       for (int k = 0; k < Q->nproc; ++k)
         bl.push_back(k == Q->self_index && !staged_self ? &Q->self_fused : &Q->peers[k].unpack);
-      pa_status s = fft_geometry(Q->nproc, bl.data(), nullptr, nullptr, f32, p, &C, &grid);
+      pa_status s = fft_geometry(Q->nproc, bl.data(), nullptr, nullptr, f32, brfft, p, &C, &grid);
       if (s != PA_OK) {
         if (n != P->self_index) {
           const std::string why = last_error();
           set_error("%s (on rank %d of the grid line)", why.c_str(), n + 1);
         }
-        return verdict(s);
+        return s;
       }
     }
   }
-  return verdict(PA_OK);
+  return PA_OK;
+}
+
+// Cached per plan, per precision (f32: ComplexF32) and per value of tunable fft_lines.
+pa_status plan_fft_check(Plan* P, bool f32) {
+  const int q = f32 ? 1 : 0;
+  if (P->fft_check_lines[q] != g_tun.fft_lines) {
+    P->fft_check[q] = fused_check(P, f32, false);
+    P->fft_check_err[q] = P->fft_check[q] == PA_OK ? std::string() : std::string(last_error());
+    P->fft_check_lines[q] = g_tun.fft_lines;
+  } else if (P->fft_check[q] != PA_OK) {
+    set_error("%s", P->fft_check_err[q].c_str());
+  }
+  return P->fft_check[q];
+}
+
+// Cached per plan and per precision, apart from plan_fft_check's verdicts (the lines per CTA of
+// the brfft kernel do not depend on tunable fft_lines).
+pa_status plan_brfft_check(Plan* P, bool f32) {
+  const int q = f32 ? 1 : 0;
+  if (!P->brfft_checked[q]) {
+    if (P->dim >= 0 && P->nproc > 1 && (P->method == PA_PEER_PUT || P->method == PA_PEER_GET)) {
+      // (src and the real dst never alias, so these methods never fall back to a staged schedule)
+      set_error("fused brfft: the one-sided methods have no unpack pass to fuse with; use "
+                "PointToPoint / Alltoallv");
+      P->brfft_check[q] = PA_EINVAL;
+    } else {
+      P->brfft_check[q] = fused_check(P, f32, true);
+    }
+    P->brfft_check_err[q] = P->brfft_check[q] == PA_OK ? std::string() : std::string(last_error());
+    P->brfft_checked[q] = true;
+  } else if (P->brfft_check[q] != PA_OK) {
+    set_error("%s", P->brfft_check_err[q].c_str());
+  }
+  return P->brfft_check[q];
 }
 
 pa_status rfft_lines(int N, bool forward, bool f32, i64 nlines, const void* src, void* dst,

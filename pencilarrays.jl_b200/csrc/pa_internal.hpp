@@ -225,6 +225,10 @@ struct Plan {
   int fft_check_lines[2] = {-1, -1};
   pa_status fft_check[2] = {PA_OK, PA_OK};
   std::string fft_check_err[2];
+  // cached answers of plan_brfft_check, [0] ComplexF64 -> Float64, [1] ComplexF32 -> Float32
+  bool brfft_checked[2] = {false, false};
+  pa_status brfft_check[2] = {PA_OK, PA_OK};
+  std::string brfft_check_err[2];
   ~Plan();
 };
 
@@ -240,8 +244,10 @@ void comm_destroy(Comm* c);
 pa_status comm_flags_export(Comm* c, void* handle64, i64* offset);
 pa_status comm_flags_import(Comm* c, int rank, const void* handle64, i64 offset);
 
+// brfft: dst (the real array) = brfft(transpose(src)) through unpack_brfft (pa_transpose_brfft);
+// flags then hold no FFT direction, PA_FFT_F32 selects the precision
 pa_status transpose(Plan* plan, Comm* comm, const void* src, void* dst, unsigned flags,
-                    void* stream);
+                    void* stream, bool brfft = false);
 pa_status wait_sends(Plan* plan, void* stream);
 pa_status permute_local(Plan* plan, const void* src, void* dst, void* scratch, void* stream);
 pa_status transpose_host(Plan* plan, Comm* comm, const void* hsrc, void* hdst, unsigned flags);
@@ -275,6 +281,13 @@ pa_status unpack_fft(int nb, const BlockCopy* const* blocks, const void* const* 
 // on every rank of the grid line (global geometry only); PA_EINVAL + last_error otherwise.
 // No device call.
 pa_status plan_fft_check(Plan* plan, bool f32);
+// fused unpack + complex-to-real line transform (fft.cu, k_unpack_brfft): the blocks tile lines
+// of N/2 + 1 bins of the complex destination box; `dst` is the real array of N reals per line
+// that replaces it (same layout otherwise).  f32: ComplexF32 -> Float32, else ComplexF64 -> Float64
+pa_status unpack_brfft(int nb, const BlockCopy* const* blocks, const void* const* srcs, void* dst,
+                       bool f32, void* stream);
+// plan_fft_check's question for unpack_brfft; its own cache, the same uniformity over the line
+pa_status plan_brfft_check(Plan* plan, bool f32);
 // real-line transforms (fft.cu): `nlines` dense, consecutive lines of N reals (src when forward,
 // dst when backward) <-> N/2 + 1 complex bins; N a power of two in 16..2048.  f32: Float32 <->
 // ComplexF32, else Float64 <-> ComplexF64

@@ -813,7 +813,7 @@ static pa_status one_sided(Plan* P, Comm* comm, const void* src, void* dst, unsi
 
 // ---- the staged schedules (PointToPoint / Alltoallv) --------------------------------
 static pa_status staged(Plan* P, Comm* comm, const void* src, void* dst, unsigned flags,
-                        bool stage_self, cudaStream_t user, cudaEvent_t buf_ev,
+                        bool brfft, bool stage_self, cudaStream_t user, cudaEvent_t buf_ev,
                         cudaEvent_t buf_unpack_ev) {
   TransposeState& S = *P->st;
   Buffers& B = *P->pout->bufs;
@@ -857,7 +857,8 @@ static pa_status staged(Plan* P, Comm* comm, const void* src, void* dst, unsigne
   // same stream (fused K3: src -> dest in one pass) and fills the HBM time the
   // NVLink-bound exchange leaves idle.  tunable "self_first" = 1 restores the
   // reference's order (self block packed first, :393-403).
-  const int fft_sign = (flags & PA_FFT_FORWARD) ? -1 : ((flags & PA_FFT_BACKWARD) ? 1 : 0);
+  // (brfft: the fused unpack is unpack_brfft, a backward transform)
+  const int fft_sign = brfft ? 1 : (flags & PA_FFT_FORWARD) ? -1 : ((flags & PA_FFT_BACKWARD) ? 1 : 0);
   const bool self_first = stage_self || g_tun.self_first;
   if (stage_self) {
     RC(launch_block(self.pack, src, rbuf, S.pack_s, nullptr));  // tail of recv_buf (:393-403)
@@ -1041,7 +1042,9 @@ static pa_status staged(Plan* P, Comm* comm, const void* src, void* dst, unsigne
       bl.push_back(fused_self ? &P->self_fused : &P->peers[n].unpack);
       sp.push_back(fused_self ? src : (const void*)rbuf);
     }
-    RC(unpack_fft(nproc, bl.data(), sp.data(), dst, fft_sign, (flags & PA_FFT_F32) != 0, S.unpack_s));
+    const bool f32 = (flags & PA_FFT_F32) != 0;
+    RC(brfft ? unpack_brfft(nproc, bl.data(), sp.data(), dst, f32, S.unpack_s)
+             : unpack_fft(nproc, bl.data(), sp.data(), dst, fft_sign, f32, S.unpack_s));
   } else if (stage_self) {
     RC(launch_block(self.unpack, rbuf, dst, S.unpack_s, nullptr));  // local data first (:511)
   }
@@ -1090,14 +1093,14 @@ static pa_status staged(Plan* P, Comm* comm, const void* src, void* dst, unsigne
 }
 
 pa_status transpose(Plan* P, Comm* comm, const void* src, void* dst, unsigned flags,
-                    void* stream) {
+                    void* stream, bool brfft) {
   // a rank may own nothing (more processes than points, Pencils.jl:193-218): its
   // empty arrays have no storage, yet it takes part in the exchange
   if ((!src && P->length_in > 0) || (!dst && P->length_out > 0)) {
     set_error("pa_transpose: null array pointer");
     return PA_EINVAL;
   }
-  const int fft_sign = (flags & PA_FFT_FORWARD) ? -1 : ((flags & PA_FFT_BACKWARD) ? 1 : 0);
+  const int fft_sign = brfft ? 1 : (flags & PA_FFT_FORWARD) ? -1 : ((flags & PA_FFT_BACKWARD) ? 1 : 0);
   const bool fft_f32 = (flags & PA_FFT_F32) != 0;  // ComplexF32 elements (elsize 8)
   if (fft_f32 && !fft_sign) {
     set_error("pa_transpose: PA_FFT_F32 without PA_FFT_FORWARD / PA_FFT_BACKWARD");
@@ -1105,7 +1108,10 @@ pa_status transpose(Plan* P, Comm* comm, const void* src, void* dst, unsigned fl
   }
   // a fused FFT this plan cannot run is refused before anything is enqueued -- and on every
   // rank of the line alike (the peers of a refusing rank must not start the exchange)
-  if (fft_sign) RC(plan_fft_check(P, fft_f32));
+  if (brfft)
+    RC(plan_brfft_check(P, fft_f32));
+  else if (fft_sign)
+    RC(plan_fft_check(P, fft_f32));
   RC(ensure_state(P));
   TransposeState& S = *P->st;
   cudaStream_t user = (cudaStream_t)stream;
@@ -1115,9 +1121,10 @@ pa_status transpose(Plan* P, Comm* comm, const void* src, void* dst, unsigned fl
 
   // src and dst may not alias -- except for the plain in-place transform along the contiguous
   // dim (same pencil on both sides, src == dst): a CTA reads its lines completely before it
-  // writes them back
-  const bool fft_in_place = fft_sign && src && src == dst && P->dim < 0 && P->same_perm;
-  if (fft_sign && !fft_in_place && src && dst &&
+  // writes them back.  (brfft: pa_transpose_brfft has checked src against the REAL dst, whose
+  // length the plan does not know)
+  const bool fft_in_place = fft_sign && !brfft && src && src == dst && P->dim < 0 && P->same_perm;
+  if (fft_sign && !brfft && !fft_in_place && src && dst &&
       (src == dst || ranges_overlap(src, P->length_in * ES, dst, P->length_out * ES))) {
     set_error("fused FFT: src and dst must not alias (in place only between identical pencils)");
     return PA_EINVAL;
@@ -1126,7 +1133,8 @@ pa_status transpose(Plan* P, Comm* comm, const void* src, void* dst, unsigned fl
     // one block: the whole local array, src -> fft(permuted dest)
     if (P->length_out == 0) return PA_OK;
     const BlockCopy* b = &P->self_fused;
-    RC(unpack_fft(1, &b, &src, dst, fft_sign, fft_f32, user));
+    RC(brfft ? unpack_brfft(1, &b, &src, dst, fft_f32, user)
+             : unpack_fft(1, &b, &src, dst, fft_sign, fft_f32, user));
     if (timing) {
       CU(cudaEventRecord(S.t[6], user));
       S.timed_once = true;
@@ -1163,8 +1171,8 @@ pa_status transpose(Plan* P, Comm* comm, const void* src, void* dst, unsigned fl
   Buffers& B = *P->pout->bufs;  // Po.send_buf / Po.recv_buf (:313-317)
   // (same base pointer counts even when one side is empty on this rank: every rank of
   //  an in-place transpose must take the same schedule)
-  const bool aliased =
-      src && dst && (src == dst || ranges_overlap(src, P->length_in * ES, dst, P->length_out * ES));
+  const bool aliased = !brfft && src && dst &&
+      (src == dst || ranges_overlap(src, P->length_in * ES, dst, P->length_out * ES));
   const bool stage_self = aliased || (flags & PA_STAGE_SELF);
   const bool one = (P->method == PA_PEER_PUT || P->method == PA_PEER_GET) && !stage_self && nproc > 1;
   if (fft_sign && one) {
@@ -1211,7 +1219,7 @@ pa_status transpose(Plan* P, Comm* comm, const void* src, void* dst, unsigned fl
     CU(cudaStreamWaitEvent(s, buf_unpack_ev, 0));
   }
   if (one) return one_sided(P, comm, src, dst, flags, user);
-  return staged(P, comm, src, dst, flags, stage_self, user, buf_ev, buf_unpack_ev);
+  return staged(P, comm, src, dst, flags, brfft, stage_self, user, buf_ev, buf_unpack_ev);
 }
 
 // MPI.Waitall(t::Transposition) (Transpositions.jl:127-130)

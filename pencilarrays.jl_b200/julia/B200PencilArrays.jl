@@ -289,6 +289,45 @@ rfft!(dest::PencilArray{ComplexF32,N,<:CuArray}, src::PencilArray{Float32,N,<:Cu
 brfft!(dest::PencilArray{Float32,N,<:CuArray}, src::PencilArray{ComplexF32,N,<:CuArray}) where {N} =
     (_rfft!(dest, src, Cuint(16), src, dest); dest)      # PA_FFT_BACKWARD | PA_FFT_F32
 
+# Fused y->x transpose + complex-to-real transform (pa_transpose_brfft): the last step of a
+# PencilFFTs real-input backward transform in one kernel per GPU after the exchange, `dest =
+# brfft(transpose(src))`, without the complex x-pencil array.  `src`: Complex{R} on the complex
+# y-pencil; `dest`: R on the real x-pencil; `pc`: the complex x-pencil the plan transposes to,
+# `Pencil(pencil(dest); size_global = (..., N÷2+1, ...))` -- passed explicitly because a Julia
+# `Transposition` holds arrays of one element type.  PointToPoint or Alltoallv.
+function brfft_plan(src::PencilArray{Complex{R}}, pc::Pencil, method) where {R}
+    H = handles(pencil(src).topology)
+    ex = Int64[extra_dims(src)...]
+    key = (objectid(pencil(src)), objectid(pc), Tuple(ex), sizeof(Complex{R}), method_code(method))
+    plan = get!(H.plans, key) do
+        h = Ref{Ptr{Cvoid}}()
+        check(ccall((:pa_plan_create, libpa), Cint,
+            (Ptr{Cvoid}, Ptr{Cvoid}, Cint, Ptr{Int64}, Cint, Cint, Ptr{Ptr{Cvoid}}),
+            pencil_handle(H, pencil(src)), pencil_handle(H, pc), length(ex), ex, sizeof(Complex{R}),
+            method_code(method), h))
+        h[]
+    end
+    plan, H
+end
+
+function transpose_brfft!(dest::PencilArray{R,N,<:CuArray}, src::PencilArray{Complex{R},N,<:CuArray},
+                          pc::Pencil; method = PointToPoint(), waitall = true) where {R<:Union{Float64,Float32},N}
+    plan, H = brfft_plan(src, pc, method)
+    flags = (waitall ? Cuint(1) : Cuint(0)) | fft_precision_flag(Complex{R})   # PA_WAITALL, PA_FFT_F32
+    ptr_or_null(A) = isempty(A) ? C_NULL : devptr(A)
+    check(ccall((:pa_transpose_brfft, libpa), Cint,
+        (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Cuint, Ptr{Cvoid}),
+        plan, H.comm, pencil_handle(H, pencil(dest)), ptr_or_null(parent(src)), ptr_or_null(parent(dest)),
+        flags, stream_ptr()))
+    dest
+end
+
+# Whether transpose_brfft! can run on this geometry (pa_plan_brfft_check): the same answer on
+# every rank of the grid line.
+brfft_fusable(src::PencilArray{Complex{R}}, pc::Pencil; method = PointToPoint()) where {R} =
+    ccall((:pa_plan_brfft_check, libpa), Cint, (Ptr{Cvoid}, Cuint), first(brfft_plan(src, pc, method)),
+          fft_precision_flag(Complex{R})) == 0
+
 # ---- host arrays: a chain of transpositions on `Array`-backed data ------------------
 # pa_host_chain_*: one submit = upload, every transpose! on the device, download;
 # asynchronous, double-buffered (download of one submit || upload of the next).

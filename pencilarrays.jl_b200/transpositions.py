@@ -5,6 +5,7 @@
     transpose_(t; waitall=True)                           # transpose!(t; waitall)   :170-179
     Waitall(t)                                            # MPI.Waitall(t)           :127-130
     transpose_(dest, src; method=...)                     # transpose!(dest, src)    :160-168
+    t = Transposition(real_x, cplx_y; brfft=True)         # GPU extension: real = brfft(transpose)
 
 Python has no ``!`` in identifiers: ``transpose_`` (torch's in-place naming)
 stands for ``transpose!``; ``transpose_bang`` is an alias.  Errors follow the
@@ -24,6 +25,7 @@ from . import _lib
 from ._lib import lib, check, i64arr, ArgumentError, PlanInfo, PeerInfo, Timings
 from .arrays import PencilArray
 from .pencils import Pencil
+from .permutations import as_tuple
 
 
 class AbstractTransposeMethod:
@@ -239,17 +241,46 @@ def _register_arenas(plan: _Plan, Po: Pencil, comm):
                           lambda n, mapped, pl=pl: lib.pa_plan_set_recv_window(pl.h, n, mapped))
 
 
-class Transposition:
-    """Holds data for transposition between two pencil configurations (:69-119)."""
+def _brfft_pencil(real: Pencil) -> Pencil:
+    """The complex counterpart of a real pencil -- N//2+1 points along its first memory dim --
+    derived once per real pencil.  It is in the same family (shares the staging arenas), so
+    repeated ``Transposition(..., brfft=True)`` reuse one plan cached on it."""
+    pc = real.__dict__.get("_brfft_cplx")
+    if pc is None:
+        ax = as_tuple(real.perm, real.ndims)[0] - 1
+        pc = Pencil(real, size_global=tuple(n // 2 + 1 if d == ax else n
+                                            for d, n in enumerate(real.size_global)))
+        real._brfft_cplx = pc
+    return pc
 
-    def __init__(self, Ao: PencilArray, Ai: PencilArray, *, method=None):
+
+_BRFFT_PAIRS = {(torch.float64, torch.complex128): 0, (torch.float32, torch.complex64): _lib.PA_FFT_F32}
+
+
+class Transposition:
+    """Holds data for transposition between two pencil configurations (:69-119).
+
+    ``brfft=True`` (GPU extension): ``Ao`` is float64 (float32) on a real x-pencil of N points
+    along its first memory dim and ``Ai`` complex128 (complex64) on the complex y-pencil; the plan
+    is the complex y -> x plan to the real pencil's N//2+1 counterpart, and ``transpose_(t)``
+    writes ``Ao = brfft(transpose(Ai))`` in one kernel after the exchange (``pa_transpose_brfft``):
+    the last step of a PencilFFTs real-input backward transform, without the complex x array."""
+
+    def __init__(self, Ao: PencilArray, Ai: PencilArray, *, method=None, brfft=False):
         method = PointToPoint() if method is None else method
         Pi, Po = Ai.pencil, Ao.pencil
+        self.brfft = bool(brfft)
         if Ai.extra_dims != Ao.extra_dims:  # :99-103
             raise ArgumentError(_lib.PA_EINVAL,
                                 "incompatible number of extra dimensions of PencilArrays: "
                                 f"{Ai.extra_dims} != {Ao.extra_dims}")
-        if Ai.dtype != Ao.dtype:  # PencilArray{T,N} for both arguments
+        if self.brfft:
+            if (Ao.dtype, Ai.dtype) not in _BRFFT_PAIRS:
+                raise ArgumentError(_lib.PA_EINVAL, "brfft: dest and src must be float64 and "
+                                    "complex128, or float32 and complex64: got "
+                                    f"{Ao.dtype} and {Ai.dtype}")
+            Po = _brfft_pencil(Ao.pencil)  # the plan's output: the complex x-pencil
+        elif Ai.dtype != Ao.dtype:  # PencilArray{T,N} for both arguments
             raise ArgumentError(_lib.PA_EINVAL, f"element types differ: {Ai.dtype} != {Ao.dtype}")
         if Pi.topology is not Po.topology:  # assert_compatible uses `!==` (:182-184)
             raise ArgumentError(_lib.PA_EINCOMPAT, "pencil topologies must be the same.")
@@ -258,6 +289,10 @@ class Transposition:
         self._plan = _get_plan(Pi, Po, Ai.extra_dims, Ai.elsize, method)  # remaining checks in C
         d = self._plan.info.dim
         self.dim = None if d == 0 else d  # :110
+        if self.brfft and d != 0 and self._plan.info.nproc > 1 and isinstance(method, (PeerPut, PeerGet)):
+            # (the same on every rank of the line: refused before the collective window setup)
+            raise ArgumentError(_lib.PA_EINVAL, "brfft: the one-sided methods have no unpack pass "
+                                "to fuse with; use PointToPoint / Alltoallv")
         if d != 0 and self._plan.info.nproc > 1 and Pi.topology.comm.handle is not None:
             comm = Pi.topology.comm
             if isinstance(method, PeerPut):
@@ -283,7 +318,11 @@ class Transposition:
         """Whether ``transpose_(self, fft=...)`` can run the unpack and the 1-d FFT as one
         kernel (``pa_plan_fft_check``).  The answer depends on the global geometry only, so it
         is the same on every rank of the grid line; when it is False, transpose and transform
-        separately.  complex64 arrays are asked about in single precision (``PA_FFT_F32``)."""
+        separately.  complex64 arrays are asked about in single precision (``PA_FFT_F32``).
+        For a ``brfft=True`` transposition: whether ``pa_transpose_brfft`` can run
+        (``pa_plan_brfft_check``)."""
+        if self.brfft:
+            return lib.pa_plan_brfft_check(self._plan.h, _fft_precision_flag(self.Ai)) == _lib.PA_OK
         return lib.pa_plan_fft_check_ex(self._plan.h, _fft_precision_flag(self.Ai)) == _lib.PA_OK
 
 
@@ -305,7 +344,10 @@ def transpose_(*args, method=None, waitall=True, overlap=True, stage_self=False,
     ``fft="forward"`` / ``"backward"`` (GPU extension, SURVEY 8 f2): the unpack and the
     1-d complex FFT along ``dest``'s contiguous dimension -- the step a PencilFFTs-style
     plan runs next -- execute as one kernel; ``dest`` receives the transformed array.
-    complex128 arrays are transformed in double precision, complex64 in single."""
+    complex128 arrays are transformed in double precision, complex64 in single.
+
+    A ``Transposition(..., brfft=True)`` runs the fused transpose + complex-to-real transform
+    (``fft=`` does not apply to it)."""
     if len(args) == 1 and isinstance(args[0], Transposition):
         t = args[0]
     elif len(args) == 2:
@@ -318,6 +360,15 @@ def transpose_(*args, method=None, waitall=True, overlap=True, stage_self=False,
         raise TypeError("transpose_(dest, src; method) or transpose_(t; waitall)")
     flags = (_lib.PA_WAITALL if waitall else 0) | (0 if overlap else _lib.PA_NO_OVERLAP) | (
         _lib.PA_STAGE_SELF if stage_self else 0)
+    if t.brfft:
+        if fft is not None:
+            raise ArgumentError(_lib.PA_EINVAL, "a brfft transposition implies its transform: "
+                                "transpose_(t) without fft=")
+        check(lib.pa_transpose_brfft(t.plan.h, t.Pi.topology.comm.handle, t.Ao.pencil._h,
+                                     C.c_void_p(t.Ai.data_ptr() or None),
+                                     C.c_void_p(t.Ao.data_ptr() or None),
+                                     flags | _fft_precision_flag(t.Ai), _stream_ptr()))
+        return t if len(args) == 1 else args[0]
     if fft is not None:
         if fft in ("forward", -1):
             flags |= _lib.PA_FFT_FORWARD
