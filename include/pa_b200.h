@@ -375,6 +375,29 @@ pa_status pa_rfft(const pa_pencil* real, const pa_pencil* cplx, int n_extra,
                   const int64_t* extra_dims, unsigned flags, const void* src, void* dst,
                   void* stream);
 
+/* ---- real-to-real line transforms ------------------------------------------------
+ * The DCT / DST of PencilFFTs' Transforms.R2R (walls: Neumann through DCT-II/III, Dirichlet
+ * through DST-II/III) along the first MEMORY-order dimension (perm[1]) of a real array on
+ * `pencil`, which must not be decomposed.  src and dst have the same shape; N points per line,
+ * n, k = 0 ... N-1, unnormalised as FFTW defines them (scipy.fft.dct / dst types 2 and 3):
+ *   PA_REDFT10  DCT-II    Y[k] = 2 sum_n x[n] cos(pi (2n+1) k / 2N)
+ *   PA_REDFT01  DCT-III   Y[k] = x[0] + 2 sum_{n>=1} x[n] cos(pi n (2k+1) / 2N)
+ *   PA_RODFT10  DST-II    Y[k] = 2 sum_n x[n] sin(pi (2n+1) (k+1) / 2N)
+ *   PA_RODFT01  DST-III   Y[k] = (-1)^k x[N-1] + 2 sum_{n<N-1} x[n] sin(pi (n+1) (2k+1) / 2N)
+ * so that REDFT01(REDFT10(x)) = RODFT01(RODFT10(x)) = 2N x.  The kind values are FFTW's
+ * fftw_r2r_kind values.  flags: 0 (Float64) or PA_FFT_F32 (Float32, fp32 arithmetic).
+ * N: power of two in 16..2048.  One kernel per call, local to the rank; extra dims are batched.
+ * Arrays dense (parent layout), 16-byte aligned; src == dst (in place) is allowed, any other
+ * overlap is not; NULL allowed where the local array is empty.  Ordered on `stream` like
+ * pa_transpose.  Every refusal happens before anything is enqueued.  PA_EINCOMPAT: the
+ * transform axis is decomposed; PA_EINVAL: other bad arguments.                          */
+#define PA_REDFT01 4
+#define PA_REDFT10 5
+#define PA_RODFT01 8
+#define PA_RODFT10 9
+pa_status pa_r2r(const pa_pencil* pencil, int n_extra, const int64_t* extra_dims, int kind,
+                 unsigned flags, const void* src, void* dst, void* stream);
+
 /* ---- fused transpose + complex-to-real line transform ---------------------------
  * The last step of a PencilFFTs real-input backward transform in one kernel per rank after
  * the exchange: dst = brfft(transpose(src)), with no complex x-pencil array in between.

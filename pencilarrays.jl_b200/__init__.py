@@ -24,7 +24,7 @@ from .arrays import (PencilArray, ManyPencilArray, parent, pencil, extra_dims, n
 from . import transpositions as Transpositions
 from .transpositions import (Transposition, transpose_, transpose_bang, Waitall, PointToPoint,
                              Alltoallv, PeerPut, PeerGet, HostChain, transpose_host_, set_tunable, fft_,
-                             rfft_, brfft_)
+                             rfft_, brfft_, r2r_)
 
 
 from . import pencilio as PencilIO

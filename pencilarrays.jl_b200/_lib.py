@@ -29,6 +29,12 @@ PA_FFT_FORWARD = 8
 PA_FFT_BACKWARD = 16
 PA_FFT_F32 = 32
 
+# real-to-real kinds (pa_r2r), FFTW's fftw_r2r_kind values
+PA_REDFT01 = 4
+PA_REDFT10 = 5
+PA_RODFT01 = 8
+PA_RODFT10 = 9
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libpa_b200.so")
 
@@ -125,6 +131,7 @@ SIGNATURES = {
     "pa_plan_fft_check_ex": (C.c_int, [_P, C.c_uint]),
     "pa_transpose_host": (C.c_int, [_P, _P, _P, _P, C.c_uint]),
     "pa_rfft": (C.c_int, [_P, _P, C.c_int, _I64P, C.c_uint, _P, _P, _P]),
+    "pa_r2r": (C.c_int, [_P, C.c_int, _I64P, C.c_int, C.c_uint, _P, _P, _P]),
     "pa_transpose_brfft": (C.c_int, [_P, _P, _P, _P, _P, C.c_uint, _P]),
     "pa_plan_brfft_check": (C.c_int, [_P, C.c_uint]),
     "pa_host_chain_create": (C.c_int, [C.c_int, C.POINTER(_P), _P, C.POINTER(_P)]),

@@ -672,6 +672,64 @@ pa_status pa_transpose_host(pa_plan* plan, pa_comm* comm, const void* host_src, 
   })
 }
 
+// ---- line transforms along the first memory dimension (pa_rfft, pa_r2r) ---------------
+// The checks they share; `who` prefixes the messages.
+// The transform axis is perm[1], the logical dim of the first memory dim; it must be local.
+static pa_status line_axis(const char* who, const Pencil& R, int* ax_out) {
+  const int ax = R.perm[0];
+  for (int i = 0; i < R.topo->M; ++i)
+    if (R.decomp[i] == ax) {
+      set_error("%s: the transform axis (logical dim %d) is decomposed", who, ax + 1);
+      return PA_EINCOMPAT;
+    }
+  *ax_out = ax;
+  return PA_OK;
+}
+
+// lines of the local array: its extents off the axis times the extra dims
+static pa_status line_count(const char* who, const Pencil& R, int ax, int n_extra,
+                            const int64_t* extra_dims, i64* nlines_out) {
+  if (n_extra < 0 || (n_extra > 0 && !extra_dims) || R.N + n_extra > PA_MAX_DIMS) {
+    set_error("%s: %d extra dims on a %d-d pencil (at most %d dims in all)", who, n_extra, R.N,
+              PA_MAX_DIMS);
+    return PA_EINVAL;
+  }
+  i64 lo[PA_MAX_DIMS], hi[PA_MAX_DIMS];
+  R.range_local(lo, hi);
+  i64 nlines = 1;
+  for (int d = 0; d < R.N; ++d)
+    if (d != ax) nlines *= hi[d] - lo[d];
+  for (int i = 0; i < n_extra; ++i) {
+    if (extra_dims[i] < 0) {
+      set_error("%s: negative extra dim", who);
+      return PA_EINVAL;
+    }
+    nlines *= extra_dims[i];
+  }
+  *nlines_out = nlines;
+  return PA_OK;
+}
+
+// src / dst of a non-empty local array: not NULL, not overlapping (in_place: src == dst is
+// allowed, any other overlap is not), 16-byte aligned
+static pa_status line_pointers(const char* who, const void* src, i64 src_bytes, const void* dst,
+                               i64 dst_bytes, bool in_place) {
+  if (!src || !dst) {
+    set_error("%s: null array pointer for a non-empty local array", who);
+    return PA_EINVAL;
+  }
+  const uintptr_t s = (uintptr_t)src, d = (uintptr_t)dst;
+  if (!(in_place && s == d) && s < d + (uintptr_t)dst_bytes && d < s + (uintptr_t)src_bytes) {
+    set_error("%s: src and dst overlap", who);
+    return PA_EINVAL;
+  }
+  if ((s | d) & 15) {
+    set_error("%s: src and dst must be 16-byte aligned", who);
+    return PA_EINVAL;
+  }
+  return PA_OK;
+}
+
 // ---- real-to-complex line transforms ------------------------------------------------
 // Every check runs on the host before any device call.  `who` prefixes the messages; with
 // check_ptrs false the caller checks src / dst itself (pa_transpose_brfft: src is not on `cplx`).
@@ -700,12 +758,9 @@ static pa_status rfft_checks(const char* who, const pa_pencil* real, const pa_pe
       set_error("%s: the pencils have different permutations", who);
       return PA_EINCOMPAT;
     }
-  const int ax = R.perm[0];  // logical dim of the first memory dim: the transform axis
-  for (int i = 0; i < M; ++i)
-    if (R.decomp[i] == ax) {
-      set_error("%s: the transform axis (logical dim %d) is decomposed", who, ax + 1);
-      return PA_EINCOMPAT;
-    }
+  int ax = 0;  // logical dim of the first memory dim: the transform axis
+  pa_status s = line_axis(who, R, &ax);
+  if (s != PA_OK) return s;
   for (int d = 0; d < R.N; ++d)
     if (d != ax && R.size_global[d] != Cp.size_global[d]) {
       set_error("%s: global sizes differ along dim %d", who, d + 1);
@@ -727,41 +782,16 @@ static pa_status rfft_checks(const char* who, const pa_pencil* real, const pa_pe
     set_error("%s: N = %lld is not a power of two in 16..2048", who, (long long)N);
     return PA_EINVAL;
   }
-  if (n_extra < 0 || (n_extra > 0 && !extra_dims) || R.N + n_extra > PA_MAX_DIMS) {
-    set_error("%s: %d extra dims on a %d-d pencil (at most %d dims in all)", who, n_extra, R.N,
-              PA_MAX_DIMS);
-    return PA_EINVAL;
-  }
-  i64 lo[PA_MAX_DIMS], hi[PA_MAX_DIMS];
-  R.range_local(lo, hi);
-  i64 nlines = 1;
-  for (int d = 0; d < R.N; ++d)
-    if (d != ax) nlines *= hi[d] - lo[d];
-  for (int i = 0; i < n_extra; ++i) {
-    if (extra_dims[i] < 0) {
-      set_error("%s: negative extra dim", who);
-      return PA_EINVAL;
-    }
-    nlines *= extra_dims[i];
-  }
+  i64 nlines = 0;
+  s = line_count(who, R, ax, n_extra, extra_dims, &nlines);
+  if (s != PA_OK) return s;
   const bool fwd = dir == PA_FFT_FORWARD;
   const i64 rs = (flags & PA_FFT_F32) ? 4 : 8;  // bytes of a real element; a complex one is 2 rs
   const i64 real_bytes = nlines * N * rs, cplx_bytes = nlines * (N / 2 + 1) * 2 * rs;
   const i64 src_bytes = fwd ? real_bytes : cplx_bytes, dst_bytes = fwd ? cplx_bytes : real_bytes;
   if (check_ptrs && nlines > 0) {
-    if (!src || !dst) {
-      set_error("%s: null array pointer for a non-empty local array", who);
-      return PA_EINVAL;
-    }
-    const uintptr_t s = (uintptr_t)src, d = (uintptr_t)dst;
-    if (s < d + (uintptr_t)dst_bytes && d < s + (uintptr_t)src_bytes) {
-      set_error("%s: src and dst overlap", who);
-      return PA_EINVAL;
-    }
-    if ((s | d) & 15) {
-      set_error("%s: src and dst must be 16-byte aligned", who);
-      return PA_EINVAL;
-    }
+    s = line_pointers(who, src, src_bytes, dst, dst_bytes, false);
+    if (s != PA_OK) return s;
   }
   *N_out = (int)N;
   *nlines_out = nlines;
@@ -782,6 +812,52 @@ pa_status pa_rfft(const pa_pencil* real, const pa_pencil* cplx, int n_extra,
     return rfft_lines(N, (flags & ~PA_FFT_F32) == PA_FFT_FORWARD, (flags & PA_FFT_F32) != 0, nlines,
                       src, dst, stream);
   })
+}
+
+// ---- real-to-real line transforms (DCT-II/III, DST-II/III) ----------------------------
+// The checks in pa_rfft's order, all on the host before any device call.
+static pa_status r2r(const pa_pencil* pencil, int n_extra, const int64_t* extra_dims, int kind,
+                     unsigned flags, const void* src, void* dst, void* stream) {
+  const char* who = "pa_r2r";
+  if (!pencil) {
+    set_error("%s: null pencil", who);
+    return PA_EINVAL;
+  }
+  const Pencil& R = *pencil->p;
+  int ax = 0;
+  pa_status s = line_axis(who, R, &ax);
+  if (s != PA_OK) return s;
+  if (kind != PA_REDFT10 && kind != PA_REDFT01 && kind != PA_RODFT10 && kind != PA_RODFT01) {
+    set_error("%s: kind %d is not PA_REDFT10, PA_REDFT01, PA_RODFT10 or PA_RODFT01", who, kind);
+    return PA_EINVAL;
+  }
+  if (flags & ~PA_FFT_F32) {
+    set_error("%s: flags must be 0 or PA_FFT_F32", who);
+    return PA_EINVAL;
+  }
+  const i64 N = R.size_global[ax];
+  if (N < 16 || N > 2048 || (N & (N - 1))) {
+    set_error("%s: N = %lld is not a power of two in 16..2048", who, (long long)N);
+    return PA_EINVAL;
+  }
+  i64 nlines = 0;
+  s = line_count(who, R, ax, n_extra, extra_dims, &nlines);
+  if (s != PA_OK) return s;
+  const bool f32 = (flags & PA_FFT_F32) != 0;
+  const i64 bytes = nlines * N * (f32 ? 4 : 8);
+  if (nlines > 0) {
+    s = line_pointers(who, src, bytes, dst, bytes, true);
+    if (s != PA_OK) return s;
+  }
+  s = need_gpu();
+  if (s != PA_OK) return s;
+  return r2r_lines((int)N, kind == PA_REDFT10 || kind == PA_RODFT10,
+                   kind == PA_RODFT10 || kind == PA_RODFT01, f32, nlines, src, dst, stream);
+}
+
+pa_status pa_r2r(const pa_pencil* pencil, int n_extra, const int64_t* extra_dims, int kind,
+                 unsigned flags, const void* src, void* dst, void* stream) {
+  GUARD({ return r2r(pencil, n_extra, extra_dims, kind, flags, src, dst, stream); })
 }
 
 static pa_status transpose_brfft(pa_plan* plan, pa_comm* comm, const pa_pencil* real,

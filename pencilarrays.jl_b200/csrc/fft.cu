@@ -449,6 +449,146 @@ __global__ void __launch_bounds__(FFT_THREADS) k_unpack_brfft(const __grid_const
   }
 }
 
+// ---- real-to-real lines (r2r_, DESIGN §3f): DCT-II / DCT-III of N = 2L reals through the
+// real-line path of k_rfft (Makhoul's reordering, fft_core.hpp); DST-II / DST-III are sign and
+// order changes of those in the load and the store.  Source and destination lines are both N
+// dense reals; every line of a CTA is in shared memory before any store, so src == dst is safe.
+struct R2rParams {
+  const char* src;
+  char* dst;
+  long long nlines;
+  long long line;   // byte stride of consecutive lines (N reals), both sides
+  int pitch;
+  int sine;         // DST (RODFT10 / RODFT01) instead of DCT (REDFT10 / REDFT01)
+  const void* tw;   // W_N^k, k < N: the rfft table
+  const void* tw4;  // W_4N^k: w_k = exp(-i pi k / 2N), k <= N/2
+};
+
+template <int LOGL, int C, bool FWD, class T>
+__global__ void __launch_bounds__(FFT_THREADS) k_r2r(const __grid_constant__ R2rParams p) {
+  using cx = cplx_t<T>;
+  using V = typename Vec2<T>::type;
+  constexpr int L = 1 << LOGL, N = 2 * L;
+  constexpr int RS = FFT_THREADS / C;  // threads per line
+  constexpr int P = L / 2 + 1;         // pairs (k, L - k) per line
+  extern __shared__ __align__(16) unsigned char fft_smem[];
+  cx* sm = reinterpret_cast<cx*>(fft_smem);
+  const int t = threadIdx.x;
+  const long long l0 = (long long)blockIdx.x * C;
+  const int ncol = (int)((p.nlines - l0) < C ? (p.nlines - l0) : C);
+  const int pitch = p.pitch;
+  const bool sine = p.sine != 0;
+  const V* twp = reinterpret_cast<const V*>(p.tw);
+  const V* tw4p = reinterpret_cast<const V*>(p.tw4);
+  auto twN = [twp](int k) {
+    const V w = __ldg(twp + k);
+    return cx{w.x, w.y};
+  };
+  auto twL = [twp](int i) {  // W_L^i = W_N^(2i)
+    const V w = __ldg(twp + 2 * i);
+    return cx{w.x, w.y};
+  };
+  auto w4 = [tw4p](int k) {  // w_k = W_4N^k
+    const V w = __ldg(tw4p + k);
+    return cx{w.x, w.y};
+  };
+
+  // ---- load (linear gather, as k_rfft): the reals (x[2m], x[2m+1]) of a line, one element per
+  //      load, reordered on their way into shared memory ----
+  {
+    constexpr int U = (L + RS - 1) / RS;
+    const int c = t / RS, r = t % RS;
+    if (c < ncol) {
+      const V* s = reinterpret_cast<const V*>(p.src + (l0 + c) * p.line);
+      T* line = reinterpret_cast<T*>(sm + c * pitch);
+      V v[U];
+#pragma unroll
+      for (int q = 0; q < U; ++q)
+        if (r + q * RS < L) v[q] = __ldcs(s + r + q * RS);
+#pragma unroll
+      for (int q = 0; q < U; ++q) {
+        const int m = r + q * RS;
+        if (m < L) {
+          if constexpr (FWD) {
+            // DCT-II: v[m] = x[2m], v[N-1-m] = x[2m+1], v[i] the part i & 1 of complex slot i / 2.
+            // DST-II transforms (-1)^n x[n]
+            line[2 * pa_fft::pad_index(m >> 1) + (m & 1)] = v[q].x;
+            line[2 * pa_fft::pad_index((N - 1 - m) >> 1) + ((N - 1 - m) & 1)] = sine ? -v[q].y : v[q].y;
+          } else {
+            // DCT-III: slot j holds (X[j], X[N-j]), j = 0 ... L, as brfft_pre_pair's pairs do.
+            // DST-III transforms X reversed: X[2m] is then entry N-1-2m
+            const int ja = sine ? N - 1 - 2 * m : 2 * m, jb = sine ? N - 2 - 2 * m : 2 * m + 1;
+            if (ja <= L) line[2 * pa_fft::pad_index(ja)] = v[q].x;
+            if (ja >= L) line[2 * pa_fft::pad_index(N - ja) + 1] = v[q].x;
+            if (jb <= L) line[2 * pa_fft::pad_index(jb)] = v[q].y;
+            if (jb >= L) line[2 * pa_fft::pad_index(N - jb) + 1] = v[q].y;
+          }
+        }
+      }
+      if (!FWD && r == 0) line[1] = T(0);  // X[N] := 0 (slot 0)
+    }
+  }
+  __syncthreads();
+
+  if constexpr (!FWD) {
+    // ---- pre-pass in place: a thread owns the slots k and L - k of its pair ----
+#pragma unroll
+    for (int w0 = 0; w0 < C * P; w0 += FFT_THREADS) {
+      const int w = w0 + t, c = w / P, k = w % P;
+      if (w < C * P && c < ncol) {
+        cx* line = sm + c * pitch;
+        const cx vk = pa_fft::dct3_pre_pair(line[pa_fft::pad_index(k)], w4(k));
+        const cx vl = pa_fft::dct3_pre_pair(line[pa_fft::pad_index(L - k)], w4(L - k));
+        cx zk, zl;
+        pa_fft::brfft_pre_pair(k, vk, vl, twN(k), &zk, &zl);
+        line[pa_fft::pad_index(k)] = zk;
+        if (k > 0) line[pa_fft::pad_index(L - k)] = zl;
+      }
+    }
+    __syncthreads();
+  }
+
+  fft_passes<LOGL, LOGL, C>(sm, pitch, ncol, FWD ? -1 : 1, twL);
+
+  if constexpr (FWD) {
+    // ---- post-pass + store: the pair k yields V[k] and V[L-k], hence Y[k], Y[N-k], Y[L-k] and
+    //      Y[L+k]; each of the N outputs is stored once.  DST-II stores Y[j] at N-1-j ----
+#pragma unroll
+    for (int w0 = 0; w0 < C * P; w0 += FFT_THREADS) {
+      const int w = w0 + t, c = w / P, k = w % P;
+      if (w < C * P && c < ncol) {
+        const cx* line = sm + c * pitch;
+        cx vk, vl;
+        pa_fft::rfft_post_pair(line[pa_fft::pad_index(fft_pos<LOGL, LOGL>(k & (L - 1)))],
+                               line[pa_fft::pad_index(fft_pos<LOGL, LOGL>((L - k) & (L - 1)))], twN(k),
+                               &vk, &vl);
+        T yk, ynk, yl, ynl;
+        pa_fft::dct2_post_pair(vk, w4(k), &yk, &ynk);      // Y[k], Y[N-k]
+        pa_fft::dct2_post_pair(vl, w4(L - k), &yl, &ynl);  // Y[L-k], Y[L+k]
+        T* out = reinterpret_cast<T*>(p.dst + (l0 + c) * p.line);
+        auto put = [out, sine](int j, T y) { __stcs(out + (sine ? N - 1 - j : j), y); };
+        put(k, yk);
+        if (k > 0 && k < L / 2) put(N - k, ynk);
+        if (k < L / 2) put(L - k, yl);
+        if (k > 0) put(L + k, ynl);
+      }
+    }
+  } else {
+    // ---- store: x[2m] = v[m], x[2m+1] = v[N-1-m] as L pair stores; DST-III: times (-1)^n ----
+#pragma unroll
+    for (int w0 = 0; w0 < C * L; w0 += FFT_THREADS) {
+      const int w = w0 + t, c = w >> LOGL, m = w & (L - 1);
+      if (c < ncol) {
+        const T* line = reinterpret_cast<const T*>(sm + c * pitch);
+        const int i = N - 1 - m;
+        const T a = line[2 * pa_fft::pad_index(fft_pos<LOGL, LOGL>(m >> 1)) + (m & 1)];
+        const T b = line[2 * pa_fft::pad_index(fft_pos<LOGL, LOGL>(i >> 1)) + (i & 1)];
+        __stcs(reinterpret_cast<V*>(p.dst + (l0 + c) * p.line) + m, vec2(a, sine ? -b : b));
+      }
+    }
+  }
+}
+
 // forward twiddle table W_L^k per (device, L, precision), computed once in extended precision
 // and rounded once to double (cplx) or float (cplxf)
 template <class T>
@@ -955,6 +1095,79 @@ pa_status rfft_lines(int N, bool forward, bool f32, i64 nlines, const void* src,
   }
   if (e != cudaSuccess) {
     set_error("rfft kernel launch failed: %s", cudaGetErrorString(e));
+    return PA_ECUDA;
+  }
+  count_launch();
+  return PA_OK;
+}
+
+pa_status r2r_lines(int N, bool forward, bool sine, bool f32, i64 nlines, const void* src, void* dst,
+                    void* stream) {
+  const int L = N / 2;
+  int logL = 0;
+  while ((1 << logL) < L) ++logL;
+  if ((1 << logL) != L || logL < 3 || logL > 10) {
+    set_error("r2r: line length %d is not a power of two in 16..2048", N);
+    return PA_EINVAL;
+  }
+  if (nlines == 0) return PA_OK;
+  R2rParams p;
+  p.src = (const char*)src;
+  p.dst = (char*)dst;
+  p.nlines = nlines;
+  const long long rs = f32 ? 4 : 8, cs = 2 * rs;  // bytes of a real / a complex element
+  p.line = rs * N;
+  p.pitch = pa_fft::padded_pitch(forward ? L : L + 1);  // backward stages the pairs of slots 0..L
+  p.sine = sine ? 1 : 0;
+  p.tw = twiddles(N, f32);
+  p.tw4 = twiddles(4 * N, f32);
+  if (!p.tw || !p.tw4) {
+    set_error("r2r: twiddle table allocation failed");
+    cudaGetLastError();
+    return PA_ENOMEM;
+  }
+  const int C = f32 ? fft_lines_f32(logL) : fft_lines(logL);
+  const long long grid = (nlines + C - 1) / C;
+  if (grid > 0x7fffffffLL) {
+    set_error("r2r: too many lines for one launch");
+    return PA_EINVAL;
+  }
+  const size_t smem = (size_t)cs * C * p.pitch;
+  cudaError_t e = cudaSuccess;
+  auto launch = [&](auto kern) {
+    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout,
+                         cudaSharedmemCarveoutMaxShared);
+    cudaGetLastError();
+    kern<<<(unsigned)grid, FFT_THREADS, smem, (cudaStream_t)stream>>>(p);
+    e = cudaGetLastError();
+  };
+  auto launch_dir = [&](auto fwd_kern, auto bwd_kern) { forward ? launch(fwd_kern) : launch(bwd_kern); };
+  if (f32) {
+    switch (logL) {
+      case 3: launch_dir(k_r2r<3, 16, true, float>, k_r2r<3, 16, false, float>); break;
+      case 4: launch_dir(k_r2r<4, 16, true, float>, k_r2r<4, 16, false, float>); break;
+      case 5: launch_dir(k_r2r<5, 16, true, float>, k_r2r<5, 16, false, float>); break;
+      case 6: launch_dir(k_r2r<6, 16, true, float>, k_r2r<6, 16, false, float>); break;
+      case 7: launch_dir(k_r2r<7, 16, true, float>, k_r2r<7, 16, false, float>); break;
+      case 8: launch_dir(k_r2r<8, 16, true, float>, k_r2r<8, 16, false, float>); break;
+      case 9: launch_dir(k_r2r<9, 16, true, float>, k_r2r<9, 16, false, float>); break;
+      default: launch_dir(k_r2r<10, 8, true, float>, k_r2r<10, 8, false, float>); break;
+    }
+  } else {
+    switch (logL) {
+      case 3: launch_dir(k_r2r<3, 8, true, double>, k_r2r<3, 8, false, double>); break;
+      case 4: launch_dir(k_r2r<4, 8, true, double>, k_r2r<4, 8, false, double>); break;
+      case 5: launch_dir(k_r2r<5, 8, true, double>, k_r2r<5, 8, false, double>); break;
+      case 6: launch_dir(k_r2r<6, 8, true, double>, k_r2r<6, 8, false, double>); break;
+      case 7: launch_dir(k_r2r<7, 8, true, double>, k_r2r<7, 8, false, double>); break;
+      case 8: launch_dir(k_r2r<8, 8, true, double>, k_r2r<8, 8, false, double>); break;
+      case 9: launch_dir(k_r2r<9, 8, true, double>, k_r2r<9, 8, false, double>); break;
+      default: launch_dir(k_r2r<10, 4, true, double>, k_r2r<10, 4, false, double>); break;
+    }
+  }
+  if (e != cudaSuccess) {
+    set_error("r2r kernel launch failed: %s", cudaGetErrorString(e));
     return PA_ECUDA;
   }
   count_launch();

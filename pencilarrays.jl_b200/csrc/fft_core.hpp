@@ -304,4 +304,28 @@ PA_HD void brfft_pre_pair(int k, cplx_t<T> xk, cplx_t<T> xl, cplx_t<T> w, cplx_t
   *zl = cplx{f.x + g.y, g.x - f.y};
 }
 
+// ---- real-to-real lines through the real-line core (r2r_, fft.cu; Makhoul's reordering) ----
+// DCT-II (FFTW REDFT10) of x, N points: the line v[n] = x[2n], v[N-1-n] = x[2n+1] (n < N/2) goes
+// through the forward real-line path (z[m] = v[2m] + i v[2m+1], the N/2-point passes,
+// rfft_post_pair), which yields the bins V[0..N/2] of its N-point FFT.  With
+// w = w_k = exp(-i pi k / 2N) and a = w V[k]:
+//   Y[k] = 2 Re a,   Y[N-k] = -2 Im a          (k = 1 ... N/2; k = 0: Y[0] = 2 Re V[0])
+// Both give the same value at k = N/2.
+template <class T>
+PA_HD void dct2_post_pair(cplx_t<T> v, cplx_t<T> w, T* yk, T* ynk) {
+  const cplx_t<T> a = cmul(w, v);
+  *yk = T(2) * a.x;
+  *ynk = T(-2) * a.y;
+}
+
+// DCT-III (FFTW REDFT01), the inverse path: from s = (X[k], X[N-k]) (X[N] := 0) and w = w_k the
+// bin V[k] = conj(w) (X[k] - i X[N-k]) = conj(w s), k = 0 ... N/2 (V[0] and V[N/2] are real).
+// brfft_pre_pair and the inverse N/2-point passes then give z[m] = v[2m] + i v[2m+1], and
+// x[2n] = v[n], x[2n+1] = v[N-1-n] undoes the reordering: REDFT01(REDFT10(x)) = 2N x.
+template <class T>
+PA_HD cplx_t<T> dct3_pre_pair(cplx_t<T> s, cplx_t<T> w) {
+  const cplx_t<T> a = cmul(w, s);
+  return cplx_t<T>{a.x, -a.y};
+}
+
 }  // namespace pa_fft

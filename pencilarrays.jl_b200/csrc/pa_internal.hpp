@@ -293,6 +293,12 @@ pa_status plan_brfft_check(Plan* plan, bool f32);
 // ComplexF32, else Float64 <-> ComplexF64
 pa_status rfft_lines(int N, bool forward, bool f32, i64 nlines, const void* src, void* dst,
                      void* stream);
+// real-to-real line transforms (fft.cu, k_r2r): `nlines` dense, consecutive lines of N reals on
+// both sides (src == dst allowed).  forward: DCT-II (sine: DST-II), else DCT-III (sine: DST-III),
+// unnormalised as FFTW's REDFT10 / RODFT10 / REDFT01 / RODFT01; N a power of two in 16..2048.
+// f32: Float32, else Float64
+pa_status r2r_lines(int N, bool forward, bool sine, bool f32, i64 nlines, const void* src, void* dst,
+                    void* stream);
 
 // standalone flag step on `stream`: signal the n remote words (monotonic max,
 // release at system scope) and/or wait for the n local words to reach seq

@@ -289,6 +289,30 @@ rfft!(dest::PencilArray{ComplexF32,N,<:CuArray}, src::PencilArray{Float32,N,<:Cu
 brfft!(dest::PencilArray{Float32,N,<:CuArray}, src::PencilArray{ComplexF32,N,<:CuArray}) where {N} =
     (_rfft!(dest, src, Cuint(16), src, dest); dest)      # PA_FFT_BACKWARD | PA_FFT_F32
 
+# Real-to-real 1-d transform along the first memory dimension (not decomposed), PencilFFTs'
+# Transforms.R2R with FFTW's unnormalised kinds: `kind` is FFTW.REDFT10 (DCT-II), REDFT01
+# (DCT-III), RODFT10 (DST-II) or RODFT01 (DST-III) -- the constants pass straight through (4, 5,
+# 8, 9).  `dest` and `src` share the pencil geometry and extra dims; `dest === src` runs in
+# place.  N a power of two in 16..2048.  One kernel, no communication.
+function r2r!(dest::PencilArray{R,N,<:CuArray}, src::PencilArray{R,N,<:CuArray},
+              kind::Integer) where {R<:Union{Float64,Float32},N}
+    pd, ps = pencil(dest), pencil(src)
+    (pd === ps || (topology(pd) === topology(ps) && size_global(pd) == size_global(ps) &&
+                   decomposition(pd) == decomposition(ps) && permutation(pd) == permutation(ps))) ||
+        throw(ArgumentError("r2r!: the arrays must have the same pencil geometry"))
+    extra_dims(dest) == extra_dims(src) ||
+        throw(ArgumentError("incompatible extra dimensions: $(extra_dims(dest)) != $(extra_dims(src))"))
+    H = handles(topology(pd))
+    ex = Int64[extra_dims(dest)...]
+    flags = R === Float32 ? Cuint(32) : Cuint(0)   # PA_FFT_F32
+    ptr_or_null(A) = isempty(A) ? C_NULL : devptr(A)
+    check(ccall((:pa_r2r, libpa), Cint,
+        (Ptr{Cvoid}, Cint, Ptr{Int64}, Cint, Cuint, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}),
+        pencil_handle(H, pd), length(ex), ex, Cint(kind), flags,
+        ptr_or_null(parent(src)), ptr_or_null(parent(dest)), stream_ptr()))
+    dest
+end
+
 # Fused y->x transpose + complex-to-real transform (pa_transpose_brfft): the last step of a
 # PencilFFTs real-input backward transform in one kernel per GPU after the exchange, `dest =
 # brfft(transpose(src))`, without the complex x-pencil array.  `src`: Complex{R} on the complex

@@ -429,6 +429,40 @@ def brfft_(dest: PencilArray, src: PencilArray):
     return _rfft(dest, src, False)
 
 
+_R2R_KINDS = {"REDFT10": _lib.PA_REDFT10, "REDFT01": _lib.PA_REDFT01,
+              "RODFT10": _lib.PA_RODFT10, "RODFT01": _lib.PA_RODFT01}
+
+
+def _same_geometry(a: Pencil, b: Pencil) -> bool:
+    return (a is b or (a.topology is b.topology and a.size_global == b.size_global
+                       and a.decomp_dims == b.decomp_dims and a.perm == b.perm))
+
+
+def r2r_(dest: PencilArray, src: PencilArray, kind: str):
+    """Real-to-real 1-d transform along the first memory dimension (not decomposed), FFTW's
+    unnormalised definitions: ``kind`` is ``"REDFT10"`` (DCT-II, ``scipy.fft.dct(x, 2)``),
+    ``"REDFT01"`` (DCT-III), ``"RODFT10"`` (DST-II) or ``"RODFT01"`` (DST-III), and
+    ``REDFT01(REDFT10(x)) = RODFT01(RODFT10(x)) = 2N x``.  ``src`` and ``dest``: float64, or
+    float32 (single precision), with the same pencil geometry and extra dims; ``dest is src``
+    transforms in place.  N is a power of two in 16..2048."""
+    if kind not in _R2R_KINDS:
+        raise ArgumentError(_lib.PA_EINVAL, f"kind must be one of {sorted(_R2R_KINDS)}: got {kind!r}")
+    flags = {torch.float64: 0, torch.float32: _lib.PA_FFT_F32}
+    if src.dtype != dest.dtype or src.dtype not in flags:
+        raise ArgumentError(_lib.PA_EINVAL, "r2r_ takes two float64 or two float32 arrays: got "
+                            f"{dest.dtype} and {src.dtype}")
+    if not _same_geometry(src.pencil, dest.pencil):
+        raise ArgumentError(_lib.PA_EINVAL, "r2r_: the arrays must have the same pencil geometry")
+    if src.extra_dims != dest.extra_dims:
+        raise ArgumentError(_lib.PA_EINVAL, "incompatible extra dimensions of PencilArrays: "
+                            f"{src.extra_dims} != {dest.extra_dims}")
+    ex = dest.extra_dims
+    check(lib.pa_r2r(dest.pencil._h, len(ex), i64arr(ex), _R2R_KINDS[kind], flags[src.dtype],
+                     C.c_void_p(src.data_ptr() or None), C.c_void_p(dest.data_ptr() or None),
+                     _stream_ptr()))
+    return dest
+
+
 def transpose_host_(t: Transposition, host_src: torch.Tensor, host_dst: torch.Tensor):
     """``transpose!`` on HOST arrays through ``pa_transpose_host``: upload, kernels and
     download pipelined inside the library; returns when ``host_dst`` is valid.  Pin the
