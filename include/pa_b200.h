@@ -425,6 +425,40 @@ pa_status pa_transpose_brfft(pa_plan* plan, pa_comm* comm, const pa_pencil* real
  * Host-only; no device needed.                                                            */
 pa_status pa_plan_brfft_check(const pa_plan* plan, unsigned flags);
 
+/* ---- fused transpose + real line transforms ----------------------------------------
+ * A transposition of REAL arrays and a line transform along the dimension it makes local, in
+ * one kernel per rank after the exchange: the steps of a wall-bounded PencilFFTs transform
+ * (DCT / DST along some dims, RFFT / FFT along the others) without the array in between.
+ * `plan` is an ordinary real plan (Float64, elsize 8; with PA_FFT_F32 Float32, elsize 4); the
+ * transform runs along the first memory dim of its output pencil (not decomposed: PA_EINCOMPAT),
+ * N points, N a power of two in 16..2048.  src: the input-pencil array of the plan, left unmodified.
+ *
+ * pa_transpose_r2r: dst = r2r(transpose(src), kind), the plan's output-pencil array of the same
+ *   element type; kind PA_REDFT10, PA_REDFT01, PA_RODFT10 or PA_RODFT01, as pa_r2r.
+ * pa_transpose_rfft: dst = rfft(transpose(src)), the ComplexF64 (ComplexF32) array on `cplx`, the
+ *   complex counterpart of the plan's output pencil related to it as `cplx` to `real` in pa_rfft
+ *   (N/2+1 points along perm[1]).
+ *
+ * Both equal the unfused pa_transpose + pa_r2r / pa_rfft bit for bit.  flags: any of
+ * PA_WAITALL, PA_NO_OVERLAP, PA_STAGE_SELF and PA_FFT_F32 -- the direction is implied, any other
+ * bit is PA_EINVAL; a kind other than the four is PA_EINVAL.  Ordering, waitall, pa_wait, NULL
+ * pointers for empty local arrays and the staged methods behave as for pa_transpose_brfft;
+ * PA_PEER_PUT / PA_PEER_GET are refused.  src and dst must not overlap, dst 16-byte aligned.
+ * Every refusal (PA_EINCOMPAT: pencils not related as above; PA_EINVAL: other bad arguments, or
+ * a geometry pa_plan_real_check refuses) happens before anything is enqueued, and a refused
+ * geometry is refused on every rank of the grid line.                                     */
+pa_status pa_transpose_r2r(pa_plan* plan, pa_comm* comm, int kind, const void* src, void* dst,
+                           unsigned flags, void* stream);
+pa_status pa_transpose_rfft(pa_plan* plan, pa_comm* comm, const pa_pencil* cplx, const void* src,
+                            void* dst, unsigned flags, void* stream);
+/* Can pa_transpose_r2r / pa_transpose_rfft run on this plan?  One answer for both (their
+ * exchange is the same, N reals per line): line length N, at most 8 blocks per line, the
+ * destination strides, and a staged method (PA_PEER_PUT / PA_PEER_GET are refused when the plan
+ * exchanges data): the same answer on every rank of the grid line.  Only PA_FFT_F32 of `flags`
+ * matters.  Cached per plan and precision, apart from the pa_plan_fft_check_ex and
+ * pa_plan_brfft_check verdicts.  Host-only; no device needed.                             */
+pa_status pa_plan_real_check(const pa_plan* plan, unsigned flags);
+
 /* ---- host chains -----------------------------------------------------------
  * A sequence of transpositions applied to HOST arrays (plan i+1 consumes what
  * plan i produces): one submit = upload of `host_src`, every transpose! on the

@@ -134,6 +134,9 @@ SIGNATURES = {
     "pa_r2r": (C.c_int, [_P, C.c_int, _I64P, C.c_int, C.c_uint, _P, _P, _P]),
     "pa_transpose_brfft": (C.c_int, [_P, _P, _P, _P, _P, C.c_uint, _P]),
     "pa_plan_brfft_check": (C.c_int, [_P, C.c_uint]),
+    "pa_transpose_r2r": (C.c_int, [_P, _P, C.c_int, _P, _P, C.c_uint, _P]),
+    "pa_transpose_rfft": (C.c_int, [_P, _P, _P, _P, _P, C.c_uint, _P]),
+    "pa_plan_real_check": (C.c_int, [_P, C.c_uint]),
     "pa_host_chain_create": (C.c_int, [C.c_int, C.POINTER(_P), _P, C.POINTER(_P)]),
     "pa_host_chain_destroy": (None, [_P]),
     "pa_host_chain_submit": (C.c_int, [_P, _P, _P, _I64P]),

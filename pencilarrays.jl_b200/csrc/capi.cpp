@@ -860,17 +860,44 @@ pa_status pa_r2r(const pa_pencil* pencil, int n_extra, const int64_t* extra_dims
   GUARD({ return r2r(pencil, n_extra, extra_dims, kind, flags, src, dst, stream); })
 }
 
+// ---- fused transpose + line transform (pa_transpose_brfft, _r2r, _rfft) ------------------
+// flags any of PA_WAITALL, PA_NO_OVERLAP, PA_STAGE_SELF, PA_FFT_F32 (the direction is implied)
+static pa_status fused_flags(const char* who, unsigned flags) {
+  if (flags & ~(PA_WAITALL | PA_NO_OVERLAP | PA_STAGE_SELF | PA_FFT_F32)) {
+    set_error("%s: flags may combine PA_WAITALL, PA_NO_OVERLAP, PA_STAGE_SELF and PA_FFT_F32 only "
+              "(the direction is implied)", who);
+    return PA_EINVAL;
+  }
+  return PA_OK;
+}
+
+// src / dst of the local arrays: NULL only when empty, not overlapping, dst 16-byte aligned
+static pa_status fused_pointers(const char* who, const void* src, i64 src_bytes, const void* dst,
+                                i64 dst_bytes) {
+  if ((!src && src_bytes > 0) || (!dst && dst_bytes > 0)) {
+    set_error("%s: null array pointer for a non-empty local array", who);
+    return PA_EINVAL;
+  }
+  const uintptr_t a = (uintptr_t)src, b = (uintptr_t)dst;
+  if (src_bytes > 0 && dst_bytes > 0 && a < b + (uintptr_t)dst_bytes && b < a + (uintptr_t)src_bytes) {
+    set_error("%s: src and dst overlap", who);
+    return PA_EINVAL;
+  }
+  if (dst_bytes > 0 && (b & 15)) {
+    set_error("%s: dst must be 16-byte aligned", who);
+    return PA_EINVAL;
+  }
+  return PA_OK;
+}
+
 static pa_status transpose_brfft(pa_plan* plan, pa_comm* comm, const pa_pencil* real,
                                  const void* src, void* dst, unsigned flags, void* stream) {
   if (!plan) {
     set_error("pa_transpose_brfft: null plan");
     return PA_EINVAL;
   }
-  if (flags & ~(PA_WAITALL | PA_NO_OVERLAP | PA_STAGE_SELF | PA_FFT_F32)) {
-    set_error("pa_transpose_brfft: flags may combine PA_WAITALL, PA_NO_OVERLAP, PA_STAGE_SELF "
-              "and PA_FFT_F32 only (the direction is implied)");
-    return PA_EINVAL;
-  }
+  pa_status s = fused_flags("pa_transpose_brfft", flags);
+  if (s != PA_OK) return s;
   Plan& P = *plan->p;
   const bool f32 = (flags & PA_FFT_F32) != 0;
   if (P.elsize != (f32 ? 8 : 16)) {
@@ -882,30 +909,18 @@ static pa_status transpose_brfft(pa_plan* plan, pa_comm* comm, const pa_pencil* 
   const pa_pencil out{P.pout};
   int N = 0;
   i64 nlines = 0;
-  pa_status s = rfft_checks("pa_transpose_brfft", real, &out, P.n_extra, P.extra,
-                            PA_FFT_BACKWARD | (flags & PA_FFT_F32), nullptr, nullptr, false, &N,
-                            &nlines);
+  s = rfft_checks("pa_transpose_brfft", real, &out, P.n_extra, P.extra,
+                  PA_FFT_BACKWARD | (flags & PA_FFT_F32), nullptr, nullptr, false, &N, &nlines);
   if (s != PA_OK) return s;
   const i64 src_bytes = P.length_in * P.elsize, dst_bytes = nlines * N * (f32 ? 4 : 8);
-  if ((!src && src_bytes > 0) || (!dst && dst_bytes > 0)) {
-    set_error("pa_transpose_brfft: null array pointer for a non-empty local array");
-    return PA_EINVAL;
-  }
-  const uintptr_t a = (uintptr_t)src, b = (uintptr_t)dst;
-  if (src_bytes > 0 && dst_bytes > 0 && a < b + (uintptr_t)dst_bytes && b < a + (uintptr_t)src_bytes) {
-    set_error("pa_transpose_brfft: src and dst overlap");
-    return PA_EINVAL;
-  }
-  if (dst_bytes > 0 && (b & 15)) {
-    set_error("pa_transpose_brfft: dst must be 16-byte aligned");
-    return PA_EINVAL;
-  }
+  s = fused_pointers("pa_transpose_brfft", src, src_bytes, dst, dst_bytes);
+  if (s != PA_OK) return s;
   // the same verdict on every rank of the grid line: a refusal launches nothing anywhere
   s = plan_brfft_check(&P, f32);
   if (s != PA_OK) return s;
   s = need_gpu();
   if (s != PA_OK) return s;
-  return transpose(&P, comm ? comm->p : nullptr, src, dst, flags, stream, true);
+  return transpose(&P, comm ? comm->p : nullptr, src, dst, flags, stream, FusedMode::brfft);
 }
 
 pa_status pa_transpose_brfft(pa_plan* plan, pa_comm* comm, const pa_pencil* real, const void* src,
@@ -920,6 +935,97 @@ pa_status pa_plan_brfft_check(const pa_plan* plan, unsigned flags) {
       return PA_EINVAL;
     }
     return plan_brfft_check(plan->p, (flags & PA_FFT_F32) != 0);
+  })
+}
+
+// A real plan (Float64, elsize 8; Float32, elsize 4 with PA_FFT_F32) for pa_transpose_r2r /
+// pa_transpose_rfft
+static pa_status real_plan(const char* who, const Plan& P, bool f32) {
+  if (P.elsize != (f32 ? 4 : 8)) {
+    set_error(f32 ? "%s: PA_FFT_F32 takes a Float32 (elsize 4) plan"
+                  : "%s: a Float64 (elsize 8) plan, or PA_FFT_F32 for Float32", who);
+    return PA_EINVAL;
+  }
+  return PA_OK;
+}
+
+static pa_status transpose_r2r(pa_plan* plan, pa_comm* comm, int kind, const void* src, void* dst,
+                               unsigned flags, void* stream) {
+  const char* who = "pa_transpose_r2r";
+  if (!plan) {
+    set_error("%s: null plan", who);
+    return PA_EINVAL;
+  }
+  pa_status s = fused_flags(who, flags);
+  if (s != PA_OK) return s;
+  if (kind != PA_REDFT10 && kind != PA_REDFT01 && kind != PA_RODFT10 && kind != PA_RODFT01) {
+    set_error("%s: kind %d is not PA_REDFT10, PA_REDFT01, PA_RODFT10 or PA_RODFT01", who, kind);
+    return PA_EINVAL;
+  }
+  Plan& P = *plan->p;
+  const bool f32 = (flags & PA_FFT_F32) != 0;
+  s = real_plan(who, P, f32);
+  if (s != PA_OK) return s;
+  int ax = 0;  // the transform axis, the output pencil's first memory dim, must be whole (as pa_r2r)
+  s = line_axis(who, *P.pout, &ax);
+  if (s != PA_OK) return s;
+  s = fused_pointers(who, src, P.length_in * P.elsize, dst, P.length_out * P.elsize);
+  if (s != PA_OK) return s;
+  // the same verdict on every rank of the grid line: a refusal launches nothing anywhere
+  s = plan_real_check(&P, f32);
+  if (s != PA_OK) return s;
+  s = need_gpu();
+  if (s != PA_OK) return s;
+  return transpose(&P, comm ? comm->p : nullptr, src, dst, flags, stream, FusedMode::r2r, kind);
+}
+
+pa_status pa_transpose_r2r(pa_plan* plan, pa_comm* comm, int kind, const void* src, void* dst,
+                           unsigned flags, void* stream) {
+  GUARD({ return transpose_r2r(plan, comm, kind, src, dst, flags, stream); })
+}
+
+static pa_status transpose_rfft(pa_plan* plan, pa_comm* comm, const pa_pencil* cplx, const void* src,
+                                void* dst, unsigned flags, void* stream) {
+  const char* who = "pa_transpose_rfft";
+  if (!plan) {
+    set_error("%s: null plan", who);
+    return PA_EINVAL;
+  }
+  pa_status s = fused_flags(who, flags);
+  if (s != PA_OK) return s;
+  Plan& P = *plan->p;
+  const bool f32 = (flags & PA_FFT_F32) != 0;
+  s = real_plan(who, P, f32);
+  if (s != PA_OK) return s;
+  // `cplx` against the plan's output pencil, as pa_rfft relates them; the pointers below
+  const pa_pencil out{P.pout};
+  int N = 0;
+  i64 nlines = 0;
+  s = rfft_checks(who, &out, cplx, P.n_extra, P.extra, PA_FFT_FORWARD | (flags & PA_FFT_F32), nullptr,
+                  nullptr, false, &N, &nlines);
+  if (s != PA_OK) return s;
+  const i64 dst_bytes = nlines * (N / 2 + 1) * 2 * P.elsize;
+  s = fused_pointers(who, src, P.length_in * P.elsize, dst, dst_bytes);
+  if (s != PA_OK) return s;
+  s = plan_real_check(&P, f32);
+  if (s != PA_OK) return s;
+  s = need_gpu();
+  if (s != PA_OK) return s;
+  return transpose(&P, comm ? comm->p : nullptr, src, dst, flags, stream, FusedMode::rfft);
+}
+
+pa_status pa_transpose_rfft(pa_plan* plan, pa_comm* comm, const pa_pencil* cplx, const void* src,
+                            void* dst, unsigned flags, void* stream) {
+  GUARD({ return transpose_rfft(plan, comm, cplx, src, dst, flags, stream); })
+}
+
+pa_status pa_plan_real_check(const pa_plan* plan, unsigned flags) {
+  GUARD({
+    if (!plan) {
+      set_error("pa_plan_real_check: null plan");
+      return PA_EINVAL;
+    }
+    return plan_real_check(plan->p, (flags & PA_FFT_F32) != 0);
   })
 }
 

@@ -92,6 +92,9 @@ struct FftParams {
                // threads then walk along a line instead of across the columns
   const void* tw;  // twiddle table of the kernel's precision (cplx or cplxf)
   unsigned tiles_x;
+  // k_unpack_r2r only (after the fields the other kernels read, which keep their offsets)
+  const void* tw4;  // W_4N^k, as R2rParams::tw4
+  int sine;         // DST (RODFT10 / RODFT01) instead of DCT
 };
 
 template <class T>
@@ -165,6 +168,62 @@ __device__ __forceinline__ void gather_rows(const FftParams& p, const long long*
         for (int k = 0; k < U; ++k) {
           const int yy = y + k * RS;
           if (c < ncol && yy < ey) line[pa_fft::pad_index(y0 + yy)] = cplx_t<T>{v[k].x, v[k].y};
+        }
+      }
+    }
+  }
+}
+
+// Where real n of a line goes in a shared-memory line of N = 2L reals (viewed as T: part i & 1
+// of complex slot i / 2 is entry 2 pad_index(i / 2) + (i & 1)) -- the maps k_rfft's and k_r2r's
+// loads apply, one real at a time, so a slot may be filled from two different blocks.
+enum class RealMap {
+  rfft,  // identity: z[n] = x[2n] + i x[2n+1]
+  dct2,  // Makhoul: v[m] = x[2m], v[N-1-m] = x[2m+1] (DST-II: -x[2m+1])
+  dct3,  // slot j holds (X[j], X[N-j]), j = 0 ... L (DST-III: X reversed)
+};
+
+template <RealMap MAP, int LOGL, class T>
+__device__ __forceinline__ void put_real(T* line, int n, T x, bool sine) {
+  constexpr int L = 1 << LOGL, N = 2 * L;
+  if constexpr (MAP == RealMap::rfft) {
+    line[2 * pa_fft::pad_index(n >> 1) + (n & 1)] = x;
+  } else if constexpr (MAP == RealMap::dct2) {
+    const int i = (n & 1) ? N - 1 - (n >> 1) : (n >> 1);
+    line[2 * pa_fft::pad_index(i >> 1) + (i & 1)] = ((n & 1) && sine) ? -x : x;
+  } else {
+    const int j = sine ? N - 1 - n : n;
+    if (j <= L) line[2 * pa_fft::pad_index(j)] = x;
+    if (j >= L) line[2 * pa_fft::pad_index(N - j) + 1] = x;
+  }
+}
+
+// gather_rows for real elements (8-byte Float64, 4-byte Float32): every block's rows of one line,
+// each real handed to put(n, x) with its position n along the line.  A block may start or end
+// at an odd position, so nothing here assumes pairs.
+template <int C, class T, class Put>
+__device__ __forceinline__ void gather_real_rows(const FftParams& p, const long long* so_off, long long x0,
+                                                 int c, int r, int ncol, const Put& put) {
+  constexpr int RS = FFT_THREADS / C;
+  constexpr int U = 8;
+#pragma unroll
+  for (int b = 0; b < FFT_MAXB; ++b) {
+    if (b < p.nb) {
+      const FftBlock& B = p.blk[b];
+      const char* s = B.src + so_off[b] + (x0 + c) * B.ssx;
+      const int ey = B.ey, y0 = B.y0;
+      const long long ssy = B.ssy;
+      for (int y = r; y < ey; y += U * RS) {
+        T v[U];
+#pragma unroll
+        for (int k = 0; k < U; ++k) {
+          const int yy = y + k * RS;
+          if (c < ncol && yy < ey) v[k] = __ldcs(reinterpret_cast<const T*>(s + (long long)yy * ssy));
+        }
+#pragma unroll
+        for (int k = 0; k < U; ++k) {
+          const int yy = y + k * RS;
+          if (c < ncol && yy < ey) put(y0 + yy, v[k]);
         }
       }
     }
@@ -291,6 +350,43 @@ struct RfftParams {
   const void* tw;  // W_N^k, k < N: the post- / pre-pass reads entry k, the L-point passes entry 2i
 };
 
+// The forward half of k_rfft after its load (k_unpack_rfft runs it after its gather): the L-point
+// passes on the C shared-memory lines z[n] = x[2n] + i x[2n+1], then the post-pass and the store
+// of the N/2 + 1 bins of line c at out(c).  tw = W_N.
+template <int LOGL, int C, class T, class Out>
+__device__ __forceinline__ void rfft_forward_tail(cplx_t<T>* sm, int pitch, int ncol, int t,
+                                                  const typename Vec2<T>::type* twp, const Out& out) {
+  using cx = cplx_t<T>;
+  using V = typename Vec2<T>::type;
+  constexpr int L = 1 << LOGL;
+  constexpr int P = L / 2 + 1;  // pairs (k, L - k) per line
+  auto twN = [twp](int k) {
+    const V w = __ldg(twp + k);
+    return cx{w.x, w.y};
+  };
+  auto twL = [twp](int i) {  // W_L^i = W_N^(2i)
+    const V w = __ldg(twp + 2 * i);
+    return cx{w.x, w.y};
+  };
+  fft_passes<LOGL, LOGL, C>(sm, pitch, ncol, -1, twL);
+
+  // ---- post-pass + store: N/2 + 1 bins per line, one contiguous run ----
+#pragma unroll
+  for (int w0 = 0; w0 < C * P; w0 += FFT_THREADS) {
+    const int w = w0 + t, c = w / P, k = w % P;
+    if (w < C * P && c < ncol) {
+      const cx* line = sm + c * pitch;
+      cx xk, xl;
+      pa_fft::rfft_post_pair(line[pa_fft::pad_index(fft_pos<LOGL, LOGL>(k & (L - 1)))],
+                             line[pa_fft::pad_index(fft_pos<LOGL, LOGL>((L - k) & (L - 1)))], twN(k),
+                             &xk, &xl);
+      V* o = reinterpret_cast<V*>(out(c));
+      __stcs(o + k, vec2(xk.x, xk.y));
+      if (k != L - k) __stcs(o + (L - k), vec2(xl.x, xl.y));
+    }
+  }
+}
+
 // Single precision: complex lines are 8 (N/2 + 1) bytes, an odd multiple of 8, so every other
 // line starts only 8-byte aligned; every access is one 8-byte element (float2) on both sides.
 template <int LOGL, int C, bool FWD, class T>
@@ -336,7 +432,10 @@ __global__ void __launch_bounds__(FFT_THREADS) k_rfft(const __grid_constant__ Rf
   }
   __syncthreads();
 
-  if constexpr (!FWD) {
+  if constexpr (FWD) {
+    rfft_forward_tail<LOGL, C, T>(sm, pitch, ncol, t, twp,
+                                  [&p, l0](int c) { return p.dst + (l0 + c) * p.dst_line; });
+  } else {
     // ---- pre-pass in place: a thread owns the slots k and L - k of its pair ----
 #pragma unroll
     for (int w0 = 0; w0 < C * P; w0 += FFT_THREADS) {
@@ -351,27 +450,9 @@ __global__ void __launch_bounds__(FFT_THREADS) k_rfft(const __grid_constant__ Rf
       }
     }
     __syncthreads();
-  }
 
-  fft_passes<LOGL, LOGL, C>(sm, pitch, ncol, FWD ? -1 : 1, twL);
+    fft_passes<LOGL, LOGL, C>(sm, pitch, ncol, 1, twL);
 
-  if constexpr (FWD) {
-    // ---- post-pass + store: N/2 + 1 bins per line, one contiguous run ----
-#pragma unroll
-    for (int w0 = 0; w0 < C * P; w0 += FFT_THREADS) {
-      const int w = w0 + t, c = w / P, k = w % P;
-      if (w < C * P && c < ncol) {
-        const cx* line = sm + c * pitch;
-        cx xk, xl;
-        pa_fft::rfft_post_pair(line[pa_fft::pad_index(fft_pos<LOGL, LOGL>(k & (L - 1)))],
-                               line[pa_fft::pad_index(fft_pos<LOGL, LOGL>((L - k) & (L - 1)))], twN(k),
-                               &xk, &xl);
-        V* out = reinterpret_cast<V*>(p.dst + (l0 + c) * p.dst_line);
-        __stcs(out + k, vec2(xk.x, xk.y));
-        if (k != L - k) __stcs(out + (L - k), vec2(xl.x, xl.y));
-      }
-    }
-  } else {
     // ---- store: z[n] = x[2n] + i x[2n+1], the N reals of a line as L pair stores ----
 #pragma unroll
     for (int w0 = 0; w0 < C * L; w0 += FFT_THREADS) {
@@ -464,22 +545,17 @@ struct R2rParams {
   const void* tw4;  // W_4N^k: w_k = exp(-i pi k / 2N), k <= N/2
 };
 
-template <int LOGL, int C, bool FWD, class T>
-__global__ void __launch_bounds__(FFT_THREADS) k_r2r(const __grid_constant__ R2rParams p) {
+// k_r2r after its load (k_unpack_r2r runs it after its gather): the DCT-III pre-pass for the 01
+// kinds, the L-point passes, and the DCT-II post-pass and store (10 kinds) or the store of the N
+// reals (01 kinds) of line c at out(c).  tw = W_N, tw4 = W_4N.
+template <int LOGL, int C, bool FWD, class T, class Out>
+__device__ __forceinline__ void r2r_tail(cplx_t<T>* sm, int pitch, int ncol, int t, bool sine,
+                                         const typename Vec2<T>::type* twp,
+                                         const typename Vec2<T>::type* tw4p, const Out& out) {
   using cx = cplx_t<T>;
   using V = typename Vec2<T>::type;
   constexpr int L = 1 << LOGL, N = 2 * L;
-  constexpr int RS = FFT_THREADS / C;  // threads per line
-  constexpr int P = L / 2 + 1;         // pairs (k, L - k) per line
-  extern __shared__ __align__(16) unsigned char fft_smem[];
-  cx* sm = reinterpret_cast<cx*>(fft_smem);
-  const int t = threadIdx.x;
-  const long long l0 = (long long)blockIdx.x * C;
-  const int ncol = (int)((p.nlines - l0) < C ? (p.nlines - l0) : C);
-  const int pitch = p.pitch;
-  const bool sine = p.sine != 0;
-  const V* twp = reinterpret_cast<const V*>(p.tw);
-  const V* tw4p = reinterpret_cast<const V*>(p.tw4);
+  constexpr int P = L / 2 + 1;  // pairs (k, L - k) per line
   auto twN = [twp](int k) {
     const V w = __ldg(twp + k);
     return cx{w.x, w.y};
@@ -492,6 +568,81 @@ __global__ void __launch_bounds__(FFT_THREADS) k_r2r(const __grid_constant__ R2r
     const V w = __ldg(tw4p + k);
     return cx{w.x, w.y};
   };
+
+  if constexpr (!FWD) {
+    // ---- pre-pass in place: a thread owns the slots k and L - k of its pair ----
+#pragma unroll
+    for (int w0 = 0; w0 < C * P; w0 += FFT_THREADS) {
+      const int w = w0 + t, c = w / P, k = w % P;
+      if (w < C * P && c < ncol) {
+        cx* line = sm + c * pitch;
+        const cx vk = pa_fft::dct3_pre_pair(line[pa_fft::pad_index(k)], w4(k));
+        const cx vl = pa_fft::dct3_pre_pair(line[pa_fft::pad_index(L - k)], w4(L - k));
+        cx zk, zl;
+        pa_fft::brfft_pre_pair(k, vk, vl, twN(k), &zk, &zl);
+        line[pa_fft::pad_index(k)] = zk;
+        if (k > 0) line[pa_fft::pad_index(L - k)] = zl;
+      }
+    }
+    __syncthreads();
+  }
+
+  fft_passes<LOGL, LOGL, C>(sm, pitch, ncol, FWD ? -1 : 1, twL);
+
+  if constexpr (FWD) {
+    // ---- post-pass + store: the pair k yields V[k] and V[L-k], hence Y[k], Y[N-k], Y[L-k] and
+    //      Y[L+k]; each of the N outputs is stored once.  DST-II stores Y[j] at N-1-j ----
+#pragma unroll
+    for (int w0 = 0; w0 < C * P; w0 += FFT_THREADS) {
+      const int w = w0 + t, c = w / P, k = w % P;
+      if (w < C * P && c < ncol) {
+        const cx* line = sm + c * pitch;
+        cx vk, vl;
+        pa_fft::rfft_post_pair(line[pa_fft::pad_index(fft_pos<LOGL, LOGL>(k & (L - 1)))],
+                               line[pa_fft::pad_index(fft_pos<LOGL, LOGL>((L - k) & (L - 1)))], twN(k),
+                               &vk, &vl);
+        T yk, ynk, yl, ynl;
+        pa_fft::dct2_post_pair(vk, w4(k), &yk, &ynk);      // Y[k], Y[N-k]
+        pa_fft::dct2_post_pair(vl, w4(L - k), &yl, &ynl);  // Y[L-k], Y[L+k]
+        T* o = reinterpret_cast<T*>(out(c));
+        auto put = [o, sine](int j, T y) { __stcs(o + (sine ? N - 1 - j : j), y); };
+        put(k, yk);
+        if (k > 0 && k < L / 2) put(N - k, ynk);
+        if (k < L / 2) put(L - k, yl);
+        if (k > 0) put(L + k, ynl);
+      }
+    }
+  } else {
+    // ---- store: x[2m] = v[m], x[2m+1] = v[N-1-m] as L pair stores; DST-III: times (-1)^n ----
+#pragma unroll
+    for (int w0 = 0; w0 < C * L; w0 += FFT_THREADS) {
+      const int w = w0 + t, c = w >> LOGL, m = w & (L - 1);
+      if (c < ncol) {
+        const T* line = reinterpret_cast<const T*>(sm + c * pitch);
+        const int i = N - 1 - m;
+        const T a = line[2 * pa_fft::pad_index(fft_pos<LOGL, LOGL>(m >> 1)) + (m & 1)];
+        const T b = line[2 * pa_fft::pad_index(fft_pos<LOGL, LOGL>(i >> 1)) + (i & 1)];
+        __stcs(reinterpret_cast<V*>(out(c)) + m, vec2(a, sine ? -b : b));
+      }
+    }
+  }
+}
+
+template <int LOGL, int C, bool FWD, class T>
+__global__ void __launch_bounds__(FFT_THREADS) k_r2r(const __grid_constant__ R2rParams p) {
+  using cx = cplx_t<T>;
+  using V = typename Vec2<T>::type;
+  constexpr int L = 1 << LOGL, N = 2 * L;
+  constexpr int RS = FFT_THREADS / C;  // threads per line
+  extern __shared__ __align__(16) unsigned char fft_smem[];
+  cx* sm = reinterpret_cast<cx*>(fft_smem);
+  const int t = threadIdx.x;
+  const long long l0 = (long long)blockIdx.x * C;
+  const int ncol = (int)((p.nlines - l0) < C ? (p.nlines - l0) : C);
+  const int pitch = p.pitch;
+  const bool sine = p.sine != 0;
+  const V* twp = reinterpret_cast<const V*>(p.tw);
+  const V* tw4p = reinterpret_cast<const V*>(p.tw4);
 
   // ---- load (linear gather, as k_rfft): the reals (x[2m], x[2m+1]) of a line, one element per
   //      load, reordered on their way into shared memory ----
@@ -530,63 +681,74 @@ __global__ void __launch_bounds__(FFT_THREADS) k_r2r(const __grid_constant__ R2r
   }
   __syncthreads();
 
-  if constexpr (!FWD) {
-    // ---- pre-pass in place: a thread owns the slots k and L - k of its pair ----
-#pragma unroll
-    for (int w0 = 0; w0 < C * P; w0 += FFT_THREADS) {
-      const int w = w0 + t, c = w / P, k = w % P;
-      if (w < C * P && c < ncol) {
-        cx* line = sm + c * pitch;
-        const cx vk = pa_fft::dct3_pre_pair(line[pa_fft::pad_index(k)], w4(k));
-        const cx vl = pa_fft::dct3_pre_pair(line[pa_fft::pad_index(L - k)], w4(L - k));
-        cx zk, zl;
-        pa_fft::brfft_pre_pair(k, vk, vl, twN(k), &zk, &zl);
-        line[pa_fft::pad_index(k)] = zk;
-        if (k > 0) line[pa_fft::pad_index(L - k)] = zl;
-      }
-    }
-    __syncthreads();
-  }
+  r2r_tail<LOGL, C, FWD, T>(sm, pitch, ncol, t, sine, twp, tw4p,
+                            [&p, l0](int c) { return p.dst + (l0 + c) * p.line; });
+}
 
-  fft_passes<LOGL, LOGL, C>(sm, pitch, ncol, FWD ? -1 : 1, twL);
+// ---- fused unpack + real line transforms (pa_transpose_r2r / pa_transpose_rfft, DESIGN §3g) ----
+// The blocks of a transposition of REAL arrays tile lines of N reals.  A CTA gathers C lines with
+// gather_real_rows, placing every real where k_r2r's / k_rfft's load would, then runs their
+// post-load stages (r2r_tail / rfft_forward_tail) on the shared-memory lines: the same
+// fft_core.hpp calls in the same order on the same tables, so the output equals the unfused
+// r2r_(transpose_(...)) / rfft_(transpose_(...)) bit for bit.  p.L = N / 2; p.tw = W_N.
+// r2r: p.tw4 = W_4N, p.sine; dst / dsx / dso address the real destination.
+// rfft: dst / dsx / dso address the COMPLEX destination of N/2 + 1 bins per line (fft_geometry
+// converts them).  Same lines per CTA and pitch as k_r2r / k_rfft for that N.
+template <int LOGL, int C, bool FWD, class T>
+__global__ void __launch_bounds__(FFT_THREADS) k_unpack_r2r(const __grid_constant__ FftParams p) {
+  using cx = cplx_t<T>;
+  using V = typename Vec2<T>::type;
+  constexpr int RS = FFT_THREADS / C;
+  extern __shared__ __align__(16) unsigned char fft_smem[];
+  cx* sm = reinterpret_cast<cx*>(fft_smem);
+  const int t = threadIdx.x;
+  long long so_off[FFT_MAXB], d_off;
+  const long long x0 = cta_offsets(p, C, so_off, &d_off);
+  const int ncol = (int)((p.ex - x0) < C ? (p.ex - x0) : C);
+  const int pitch = p.pitch;
+  const bool sine = p.sine != 0;
 
-  if constexpr (FWD) {
-    // ---- post-pass + store: the pair k yields V[k] and V[L-k], hence Y[k], Y[N-k], Y[L-k] and
-    //      Y[L+k]; each of the N outputs is stored once.  DST-II stores Y[j] at N-1-j ----
-#pragma unroll
-    for (int w0 = 0; w0 < C * P; w0 += FFT_THREADS) {
-      const int w = w0 + t, c = w / P, k = w % P;
-      if (w < C * P && c < ncol) {
-        const cx* line = sm + c * pitch;
-        cx vk, vl;
-        pa_fft::rfft_post_pair(line[pa_fft::pad_index(fft_pos<LOGL, LOGL>(k & (L - 1)))],
-                               line[pa_fft::pad_index(fft_pos<LOGL, LOGL>((L - k) & (L - 1)))], twN(k),
-                               &vk, &vl);
-        T yk, ynk, yl, ynl;
-        pa_fft::dct2_post_pair(vk, w4(k), &yk, &ynk);      // Y[k], Y[N-k]
-        pa_fft::dct2_post_pair(vl, w4(L - k), &yl, &ynl);  // Y[L-k], Y[L+k]
-        T* out = reinterpret_cast<T*>(p.dst + (l0 + c) * p.line);
-        auto put = [out, sine](int j, T y) { __stcs(out + (sine ? N - 1 - j : j), y); };
-        put(k, yk);
-        if (k > 0 && k < L / 2) put(N - k, ynk);
-        if (k < L / 2) put(L - k, yl);
-        if (k > 0) put(L + k, ynl);
-      }
-    }
-  } else {
-    // ---- store: x[2m] = v[m], x[2m+1] = v[N-1-m] as L pair stores; DST-III: times (-1)^n ----
-#pragma unroll
-    for (int w0 = 0; w0 < C * L; w0 += FFT_THREADS) {
-      const int w = w0 + t, c = w >> LOGL, m = w & (L - 1);
-      if (c < ncol) {
-        const T* line = reinterpret_cast<const T*>(sm + c * pitch);
-        const int i = N - 1 - m;
-        const T a = line[2 * pa_fft::pad_index(fft_pos<LOGL, LOGL>(m >> 1)) + (m & 1)];
-        const T b = line[2 * pa_fft::pad_index(fft_pos<LOGL, LOGL>(i >> 1)) + (i & 1)];
-        __stcs(reinterpret_cast<V*>(p.dst + (l0 + c) * p.line) + m, vec2(a, sine ? -b : b));
-      }
-    }
+  // ---- gather: transposing, or linear (lines contiguous in the source) ----
+  {
+    const int c = p.linear ? t / RS : t % C, r = p.linear ? t % RS : t / C;
+    T* line = reinterpret_cast<T*>(sm + c * pitch);
+    gather_real_rows<C, T>(p, so_off, x0, c, r, ncol, [line, sine](int n, T x) {
+      put_real<FWD ? RealMap::dct2 : RealMap::dct3, LOGL>(line, n, x, sine);
+    });
+    if (!FWD && r == 0 && c < ncol) line[1] = T(0);  // X[N] := 0 (slot 0)
   }
+  __syncthreads();
+
+  char* d = p.dst + x0 * p.dsx + d_off;
+  r2r_tail<LOGL, C, FWD, T>(sm, pitch, ncol, t, sine, reinterpret_cast<const V*>(p.tw),
+                            reinterpret_cast<const V*>(p.tw4),
+                            [&p, d](int c) { return d + c * p.dsx; });
+}
+
+template <int LOGL, int C, class T>
+__global__ void __launch_bounds__(FFT_THREADS) k_unpack_rfft(const __grid_constant__ FftParams p) {
+  using cx = cplx_t<T>;
+  using V = typename Vec2<T>::type;
+  constexpr int RS = FFT_THREADS / C;
+  extern __shared__ __align__(16) unsigned char fft_smem[];
+  cx* sm = reinterpret_cast<cx*>(fft_smem);
+  const int t = threadIdx.x;
+  long long so_off[FFT_MAXB], d_off;
+  const long long x0 = cta_offsets(p, C, so_off, &d_off);
+  const int ncol = (int)((p.ex - x0) < C ? (p.ex - x0) : C);
+  const int pitch = p.pitch;
+
+  {
+    const int c = p.linear ? t / RS : t % C, r = p.linear ? t % RS : t / C;
+    T* line = reinterpret_cast<T*>(sm + c * pitch);
+    gather_real_rows<C, T>(p, so_off, x0, c, r, ncol,
+                           [line](int n, T x) { put_real<RealMap::rfft, LOGL>(line, n, x, false); });
+  }
+  __syncthreads();
+
+  char* d = p.dst + x0 * p.dsx + d_off;
+  rfft_forward_tail<LOGL, C, T>(sm, pitch, ncol, t, reinterpret_cast<const V*>(p.tw),
+                                [&p, d](int c) { return d + c * p.dsx; });
 }
 
 // forward twiddle table W_L^k per (device, L, precision), computed once in extended precision
@@ -635,10 +797,15 @@ static const void* twiddles(int L, bool f32) {
 // nothing to do on this rank.  f32: ComplexF32 elements (PA_FFT_F32), else ComplexF64.
 // brfft (k_unpack_brfft): the lines are M = N/2 + 1 bins, and `dst` is the REAL array of N
 // reals per line in place of the complex one the blocks describe (DESIGN §3e).
+// r2r / rfft (k_unpack_r2r / k_unpack_rfft): the elements are reals (Float64, or Float32 with
+// f32) and the lines N reals; rfft: `dst` is the COMPLEX array of N/2 + 1 bins per line in place
+// of the real one the blocks describe (DESIGN §3g).
 static pa_status fft_geometry(int nb, const BlockCopy* const* blocks, const void* const* srcs,
-                              void* dst, bool f32, bool brfft, FftParams& p, int* C_out,
+                              void* dst, bool f32, FusedMode mode, FftParams& p, int* C_out,
                               unsigned long long* grid_out) {
-  const i64 es = f32 ? 8 : 16;  // element bytes
+  const bool brfft = mode == FusedMode::brfft;
+  const bool real = mode == FusedMode::r2r || mode == FusedMode::rfft;  // real source elements
+  const i64 es = real ? (f32 ? 4 : 8) : (f32 ? 8 : 16);  // element bytes
   memset(&p, 0, sizeof p);
   *grid_out = 0;
   // the line dim: destination stride 1 (and extent > 1) in some block
@@ -692,8 +859,12 @@ static pa_status fft_geometry(int nb, const BlockCopy* const* blocks, const void
     const BlockCopy& B = *blocks[b];
     if (B.count == 0) continue;
     if (B.elsize != es) {
-      set_error(f32 ? "fused FFT: PA_FFT_F32 takes ComplexF32 (8-byte) elements only"
-                    : "fused FFT: ComplexF64 (16-byte) elements only");
+      if (real)
+        set_error(f32 ? "fused real transform: PA_FFT_F32 takes Float32 (4-byte) elements only"
+                      : "fused real transform: Float64 (8-byte) elements only");
+      else
+        set_error(f32 ? "fused FFT: PA_FFT_F32 takes ComplexF32 (8-byte) elements only"
+                      : "fused FFT: ComplexF64 (16-byte) elements only");
       return PA_EINVAL;
     }
     if (B.raw[0].ss != 1) {
@@ -736,13 +907,17 @@ static pa_status fft_geometry(int nb, const BlockCopy* const* blocks, const void
       if (i != jy && i != jx && B.raw[i].e > 1) F.so[o++] = B.raw[i].ss * es;
     L += B.raw[jy].e;
   }
-  const i64 M = L;  // rows per line (brfft: bins)
+  const i64 M = L;  // rows per line (brfft: bins; r2r / rfft: reals)
   if (brfft) L = M - 1;  // the N/2-point complex FFT of a real line of N = 2 (M - 1)
+  if (real) L = M / 2;   // the N/2-point complex FFT of a real line of N = M
   int logL = 0;
   while ((1LL << logL) < L) ++logL;
-  if ((1LL << logL) != L || L < 8 || L > 1024) {
+  if ((1LL << logL) != L || L < 8 || L > 1024 || (real && 2 * L != M)) {
     if (brfft)
       set_error("fused brfft: %lld bins per line are not N/2+1 with N a power of two in 16..2048",
+                (long long)M);
+    else if (real)
+      set_error("fused real transform: line length N = %lld is not a power of two in 16..2048",
                 (long long)M);
     else
       set_error("fused FFT: line length %lld is not a power of two in 8..1024", (long long)L);
@@ -779,7 +954,7 @@ static pa_status fft_geometry(int nb, const BlockCopy* const* blocks, const void
     }
   p.L = (int)L;
   p.logL = logL;
-  p.pitch = pa_fft::padded_pitch((int)M);
+  p.pitch = real ? 0 : pa_fft::padded_pitch((int)M);  // r2r / rfft: the launcher's, by direction
   if (brfft) {
     // The line dim is the destination's first memory dim (stride 1) and whole (the blocks tile
     // [0, M)), so every other destination offset and stride is a multiple of M elements: line k
@@ -803,11 +978,33 @@ static pa_status fft_geometry(int nb, const BlockCopy* const* blocks, const void
     for (int o = 0; o < p.no; ++o)
       if (!to_real(p.dso[o] / es, &p.dso[o])) return PA_EINVAL;
   }
+  if (mode == FusedMode::rfft) {
+    // brfft's rescale the other way round: line k of the real array starts at k N reals, and at
+    // k M complex bins in the complex array of the same shape otherwise
+    const i64 N = M, Mc = L + 1, cs = 2 * es;
+    auto to_cplx = [&](long long off, long long* out) {
+      if (off % N != 0) {
+        set_error("fused rfft: a destination stride or offset is not a multiple of the %lld reals "
+                  "of a line", (long long)N);
+        return false;
+      }
+      *out = off / N * Mc * cs;
+      return true;
+    };
+    long long v = 0;
+    if (!to_cplx(min_doff, &v)) return PA_EINVAL;
+    p.dst = dst ? (char*)dst + v : nullptr;
+    p.dsx = Mc * cs;
+    if (jx >= 0 && p.ex > 1 && !to_cplx(ref->raw[jx].ds, &p.dsx)) return PA_EINVAL;
+    for (int o = 0; o < p.no; ++o)
+      if (!to_cplx(p.dso[o] / es, &p.dso[o])) return PA_EINVAL;
+  }
   // tunable "fft_lines" = 4: 4 lines per CTA also for 256- / 512-point lines (64-byte gathers,
   // first pass of radix 4 / 8 in registers, half the shared memory per CTA); double precision
-  // only -- single precision always takes fft_lines_f32.  brfft: the lines per CTA of k_rfft
+  // only -- single precision always takes fft_lines_f32.  brfft, r2r, rfft: the lines per CTA of
+  // k_rfft
   const int C = f32 ? fft_lines_f32(logL)
-                    : ((!brfft && g_tun.fft_lines == 4 && logL >= 8) ? 4 : fft_lines(logL));
+                    : ((mode == FusedMode::fft && g_tun.fft_lines == 4 && logL >= 8) ? 4 : fft_lines(logL));
   p.tiles_x = (unsigned)((p.ex + C - 1) / C);
   unsigned long long grid = p.tiles_x;
   for (int i = 0; i < p.no; ++i) grid *= (unsigned long long)p.oe[i];
@@ -827,7 +1024,7 @@ pa_status unpack_fft(int nb, const BlockCopy* const* blocks, const void* const* 
   FftParams p;
   int C = 0;
   unsigned long long grid = 0;
-  pa_status s = fft_geometry(nb, blocks, srcs, dst, f32, false, p, &C, &grid);
+  pa_status s = fft_geometry(nb, blocks, srcs, dst, f32, FusedMode::fft, p, &C, &grid);
   if (s != PA_OK || grid == 0) return s;
   const int logL = p.logL;
   p.sign = sign < 0 ? -1 : 1;
@@ -888,7 +1085,7 @@ pa_status unpack_brfft(int nb, const BlockCopy* const* blocks, const void* const
   FftParams p;
   int C = 0;
   unsigned long long grid = 0;
-  pa_status s = fft_geometry(nb, blocks, srcs, dst, f32, true, p, &C, &grid);
+  pa_status s = fft_geometry(nb, blocks, srcs, dst, f32, FusedMode::brfft, p, &C, &grid);
   if (s != PA_OK || grid == 0) return s;
   const int logL = p.logL;
   p.sign = 1;
@@ -939,18 +1136,142 @@ pa_status unpack_brfft(int nb, const BlockCopy* const* blocks, const void* const
   return PA_OK;
 }
 
+// kind: FFTW's REDFT10 (DCT-II), REDFT01 (DCT-III), RODFT10 (DST-II) or RODFT01 (DST-III)
+pa_status unpack_r2r(int nb, const BlockCopy* const* blocks, const void* const* srcs, void* dst,
+                     int kind, bool f32, void* stream) {
+  // (pa_transpose_r2r has already asked plan_real_check for every rank of the line)
+  const bool forward = kind == PA_REDFT10 || kind == PA_RODFT10;
+  FftParams p;
+  int C = 0;
+  unsigned long long grid = 0;
+  pa_status s = fft_geometry(nb, blocks, srcs, dst, f32, FusedMode::r2r, p, &C, &grid);
+  if (s != PA_OK || grid == 0) return s;
+  const int logL = p.logL, N = 2 * p.L;
+  p.pitch = pa_fft::padded_pitch(forward ? p.L : p.L + 1);  // as r2r_lines
+  p.sine = (kind == PA_RODFT10 || kind == PA_RODFT01) ? 1 : 0;
+  p.tw = twiddles(N, f32);
+  p.tw4 = twiddles(4 * N, f32);
+  if (!p.tw || !p.tw4) {
+    set_error("fused r2r: twiddle table allocation failed");
+    cudaGetLastError();
+    return PA_ENOMEM;
+  }
+  const size_t smem = (f32 ? sizeof(pa_fft::cplxf) : sizeof(cplx)) * (size_t)C * p.pitch;
+  cudaError_t e = cudaSuccess;
+  auto launch = [&](auto kern) {
+    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout,
+                         cudaSharedmemCarveoutMaxShared);
+    cudaGetLastError();
+    kern<<<(unsigned)grid, FFT_THREADS, smem, (cudaStream_t)stream>>>(p);
+    e = cudaGetLastError();
+  };
+  auto launch_dir = [&](auto fwd_kern, auto bwd_kern) { forward ? launch(fwd_kern) : launch(bwd_kern); };
+  if (f32) {
+    switch (logL) {
+      case 3: launch_dir(k_unpack_r2r<3, 16, true, float>, k_unpack_r2r<3, 16, false, float>); break;
+      case 4: launch_dir(k_unpack_r2r<4, 16, true, float>, k_unpack_r2r<4, 16, false, float>); break;
+      case 5: launch_dir(k_unpack_r2r<5, 16, true, float>, k_unpack_r2r<5, 16, false, float>); break;
+      case 6: launch_dir(k_unpack_r2r<6, 16, true, float>, k_unpack_r2r<6, 16, false, float>); break;
+      case 7: launch_dir(k_unpack_r2r<7, 16, true, float>, k_unpack_r2r<7, 16, false, float>); break;
+      case 8: launch_dir(k_unpack_r2r<8, 16, true, float>, k_unpack_r2r<8, 16, false, float>); break;
+      case 9: launch_dir(k_unpack_r2r<9, 16, true, float>, k_unpack_r2r<9, 16, false, float>); break;
+      default: launch_dir(k_unpack_r2r<10, 8, true, float>, k_unpack_r2r<10, 8, false, float>); break;
+    }
+  } else {
+    switch (logL) {
+      case 3: launch_dir(k_unpack_r2r<3, 8, true, double>, k_unpack_r2r<3, 8, false, double>); break;
+      case 4: launch_dir(k_unpack_r2r<4, 8, true, double>, k_unpack_r2r<4, 8, false, double>); break;
+      case 5: launch_dir(k_unpack_r2r<5, 8, true, double>, k_unpack_r2r<5, 8, false, double>); break;
+      case 6: launch_dir(k_unpack_r2r<6, 8, true, double>, k_unpack_r2r<6, 8, false, double>); break;
+      case 7: launch_dir(k_unpack_r2r<7, 8, true, double>, k_unpack_r2r<7, 8, false, double>); break;
+      case 8: launch_dir(k_unpack_r2r<8, 8, true, double>, k_unpack_r2r<8, 8, false, double>); break;
+      case 9: launch_dir(k_unpack_r2r<9, 8, true, double>, k_unpack_r2r<9, 8, false, double>); break;
+      default: launch_dir(k_unpack_r2r<10, 4, true, double>, k_unpack_r2r<10, 4, false, double>); break;
+    }
+  }
+  if (e != cudaSuccess) {
+    set_error("fused r2r kernel launch failed: %s", cudaGetErrorString(e));
+    return PA_ECUDA;
+  }
+  count_launch();
+  return PA_OK;
+}
+
+pa_status unpack_rfft(int nb, const BlockCopy* const* blocks, const void* const* srcs, void* dst,
+                      bool f32, void* stream) {
+  // (pa_transpose_rfft has already asked plan_real_check for every rank of the line)
+  FftParams p;
+  int C = 0;
+  unsigned long long grid = 0;
+  pa_status s = fft_geometry(nb, blocks, srcs, dst, f32, FusedMode::rfft, p, &C, &grid);
+  if (s != PA_OK || grid == 0) return s;
+  const int logL = p.logL;
+  p.pitch = pa_fft::padded_pitch(p.L);  // as rfft_lines, forward
+  p.tw = twiddles(2 * p.L, f32);
+  if (!p.tw) {
+    set_error("fused rfft: twiddle table allocation failed");
+    cudaGetLastError();
+    return PA_ENOMEM;
+  }
+  const size_t smem = (f32 ? sizeof(pa_fft::cplxf) : sizeof(cplx)) * (size_t)C * p.pitch;
+  cudaError_t e = cudaSuccess;
+  auto launch = [&](auto kern) {
+    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout,
+                         cudaSharedmemCarveoutMaxShared);
+    cudaGetLastError();
+    kern<<<(unsigned)grid, FFT_THREADS, smem, (cudaStream_t)stream>>>(p);
+    e = cudaGetLastError();
+  };
+  if (f32) {
+    switch (logL) {
+      case 3: launch(k_unpack_rfft<3, 16, float>); break;
+      case 4: launch(k_unpack_rfft<4, 16, float>); break;
+      case 5: launch(k_unpack_rfft<5, 16, float>); break;
+      case 6: launch(k_unpack_rfft<6, 16, float>); break;
+      case 7: launch(k_unpack_rfft<7, 16, float>); break;
+      case 8: launch(k_unpack_rfft<8, 16, float>); break;
+      case 9: launch(k_unpack_rfft<9, 16, float>); break;
+      default: launch(k_unpack_rfft<10, 8, float>); break;
+    }
+  } else {
+    switch (logL) {
+      case 3: launch(k_unpack_rfft<3, 8, double>); break;
+      case 4: launch(k_unpack_rfft<4, 8, double>); break;
+      case 5: launch(k_unpack_rfft<5, 8, double>); break;
+      case 6: launch(k_unpack_rfft<6, 8, double>); break;
+      case 7: launch(k_unpack_rfft<7, 8, double>); break;
+      case 8: launch(k_unpack_rfft<8, 8, double>); break;
+      case 9: launch(k_unpack_rfft<9, 8, double>); break;
+      default: launch(k_unpack_rfft<10, 4, double>); break;
+    }
+  }
+  if (e != cudaSuccess) {
+    set_error("fused rfft kernel launch failed: %s", cudaGetErrorString(e));
+    return PA_ECUDA;
+  }
+  count_launch();
+  return PA_OK;
+}
+
 // Can pa_transpose fuse the FFT (brfft: pa_transpose_brfft the complex-to-real transform) into
 // this plan's unpack?  Every rank of a grid line must get the same answer: a rank that refused
 // before the exchange while its peers went ahead would leave them waiting on flags it never
 // sets.  So the answer depends on the global geometry only: the blocks that EVERY rank of the
 // line would gather -- each rank's plan rebuilt from the pencils with that rank's coordinates --
 // with the self block read from src and staged through recv_buf alike.
-static pa_status fused_check(Plan* P, bool f32, bool brfft) {
-  if (!f32 && P->elsize != 16) {
+static pa_status fused_check(Plan* P, bool f32, FusedMode mode) {
+  if (mode == FusedMode::r2r || mode == FusedMode::rfft) {
+    if (P->elsize != (f32 ? 4 : 8)) {
+      set_error(f32 ? "fused real transform: PA_FFT_F32 takes Float32 (4-byte) elements only"
+                    : "fused real transform: Float64 (8-byte) elements only");
+      return PA_EINVAL;
+    }
+  } else if (!f32 && P->elsize != 16) {
     set_error("fused FFT: ComplexF64 (16-byte) elements only");
     return PA_EINVAL;
-  }
-  if (f32 && P->elsize != 8) {
+  } else if (f32 && P->elsize != 8) {
     set_error("fused FFT: PA_FFT_F32 takes ComplexF32 (8-byte) elements only");
     return PA_EINVAL;
   }
@@ -959,7 +1280,7 @@ static pa_status fused_check(Plan* P, bool f32, bool brfft) {
   unsigned long long grid = 0;
   if (P->dim < 0 || P->nproc == 1) {
     const BlockCopy* b = &P->self_fused;
-    return fft_geometry(1, &b, nullptr, nullptr, f32, brfft, p, &C, &grid);
+    return fft_geometry(1, &b, nullptr, nullptr, f32, mode, p, &C, &grid);
   }
   for (int n = 0; n < P->nproc; ++n) {
     std::unique_ptr<Plan> hold;
@@ -982,7 +1303,7 @@ static pa_status fused_check(Plan* P, bool f32, bool brfft) {
       std::vector<const BlockCopy*> bl;
       for (int k = 0; k < Q->nproc; ++k)
         bl.push_back(k == Q->self_index && !staged_self ? &Q->self_fused : &Q->peers[k].unpack);
-      pa_status s = fft_geometry(Q->nproc, bl.data(), nullptr, nullptr, f32, brfft, p, &C, &grid);
+      pa_status s = fft_geometry(Q->nproc, bl.data(), nullptr, nullptr, f32, mode, p, &C, &grid);
       if (s != PA_OK) {
         if (n != P->self_index) {
           const std::string why = last_error();
@@ -999,7 +1320,7 @@ static pa_status fused_check(Plan* P, bool f32, bool brfft) {
 pa_status plan_fft_check(Plan* P, bool f32) {
   const int q = f32 ? 1 : 0;
   if (P->fft_check_lines[q] != g_tun.fft_lines) {
-    P->fft_check[q] = fused_check(P, f32, false);
+    P->fft_check[q] = fused_check(P, f32, FusedMode::fft);
     P->fft_check_err[q] = P->fft_check[q] == PA_OK ? std::string() : std::string(last_error());
     P->fft_check_lines[q] = g_tun.fft_lines;
   } else if (P->fft_check[q] != PA_OK) {
@@ -1019,7 +1340,7 @@ pa_status plan_brfft_check(Plan* P, bool f32) {
                 "PointToPoint / Alltoallv");
       P->brfft_check[q] = PA_EINVAL;
     } else {
-      P->brfft_check[q] = fused_check(P, f32, true);
+      P->brfft_check[q] = fused_check(P, f32, FusedMode::brfft);
     }
     P->brfft_check_err[q] = P->brfft_check[q] == PA_OK ? std::string() : std::string(last_error());
     P->brfft_checked[q] = true;
@@ -1027,6 +1348,29 @@ pa_status plan_brfft_check(Plan* P, bool f32) {
     set_error("%s", P->brfft_check_err[q].c_str());
   }
   return P->brfft_check[q];
+}
+
+// Can pa_transpose_r2r / pa_transpose_rfft run on this real plan?  Both kernels gather the same
+// blocks (N reals per line), so one verdict answers for both: the rfft geometry, which checks
+// everything the r2r geometry does plus the rescale of the destination to N/2 + 1 bins per line.
+// Cached per plan and per precision, apart from the fft and brfft verdicts.
+pa_status plan_real_check(Plan* P, bool f32) {
+  const int q = f32 ? 1 : 0;
+  if (!P->real_checked[q]) {
+    if (P->dim >= 0 && P->nproc > 1 && (P->method == PA_PEER_PUT || P->method == PA_PEER_GET)) {
+      // (src and dst never overlap, so these methods never fall back to a staged schedule)
+      set_error("fused real transform: the one-sided methods have no unpack pass to fuse with; "
+                "use PointToPoint / Alltoallv");
+      P->real_check[q] = PA_EINVAL;
+    } else {
+      P->real_check[q] = fused_check(P, f32, FusedMode::rfft);
+    }
+    P->real_check_err[q] = P->real_check[q] == PA_OK ? std::string() : std::string(last_error());
+    P->real_checked[q] = true;
+  } else if (P->real_check[q] != PA_OK) {
+    set_error("%s", P->real_check_err[q].c_str());
+  }
+  return P->real_check[q];
 }
 
 pa_status rfft_lines(int N, bool forward, bool f32, i64 nlines, const void* src, void* dst,

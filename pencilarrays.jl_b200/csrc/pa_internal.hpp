@@ -229,6 +229,10 @@ struct Plan {
   bool brfft_checked[2] = {false, false};
   pa_status brfft_check[2] = {PA_OK, PA_OK};
   std::string brfft_check_err[2];
+  // cached answers of plan_real_check, [0] Float64 and [1] Float32 (PA_FFT_F32)
+  bool real_checked[2] = {false, false};
+  pa_status real_check[2] = {PA_OK, PA_OK};
+  std::string real_check_err[2];
   ~Plan();
 };
 
@@ -244,10 +248,19 @@ void comm_destroy(Comm* c);
 pa_status comm_flags_export(Comm* c, void* handle64, i64* offset);
 pa_status comm_flags_import(Comm* c, int rank, const void* handle64, i64 offset);
 
-// brfft: dst (the real array) = brfft(transpose(src)) through unpack_brfft (pa_transpose_brfft);
-// flags then hold no FFT direction, PA_FFT_F32 selects the precision
+// What the fused unpack of a transposition computes from the gathered lines
+enum class FusedMode {
+  fft,    // the complex FFT (pa_transpose with PA_FFT_FORWARD / PA_FFT_BACKWARD)
+  brfft,  // N/2 + 1 complex bins -> N reals (pa_transpose_brfft, unpack_brfft)
+  r2r,    // N reals -> N reals, a DCT / DST (pa_transpose_r2r, unpack_r2r)
+  rfft,   // N reals -> N/2 + 1 complex bins (pa_transpose_rfft, unpack_rfft)
+};
+
+// mode brfft / r2r / rfft: dst = brfft / r2r / rfft(transpose(src)) through the fused unpack;
+// flags then hold no FFT direction, PA_FFT_F32 selects the precision; r2r_kind: the PA_*ODFT*
+// kind of r2r
 pa_status transpose(Plan* plan, Comm* comm, const void* src, void* dst, unsigned flags,
-                    void* stream, bool brfft = false);
+                    void* stream, FusedMode mode = FusedMode::fft, int r2r_kind = 0);
 pa_status wait_sends(Plan* plan, void* stream);
 pa_status permute_local(Plan* plan, const void* src, void* dst, void* scratch, void* stream);
 pa_status transpose_host(Plan* plan, Comm* comm, const void* hsrc, void* hdst, unsigned flags);
@@ -288,6 +301,17 @@ pa_status unpack_brfft(int nb, const BlockCopy* const* blocks, const void* const
                        bool f32, void* stream);
 // plan_fft_check's question for unpack_brfft; its own cache, the same uniformity over the line
 pa_status plan_brfft_check(Plan* plan, bool f32);
+// fused unpack + real line transforms (fft.cu, k_unpack_r2r / k_unpack_rfft): the blocks tile
+// lines of N reals (Float32 with f32, else Float64) of the real destination box.  r2r: `dst` is
+// that box, kind one of PA_REDFT10 / PA_REDFT01 / PA_RODFT10 / PA_RODFT01.  rfft: `dst` is the
+// complex array of N/2 + 1 bins per line that replaces it (same layout otherwise)
+pa_status unpack_r2r(int nb, const BlockCopy* const* blocks, const void* const* srcs, void* dst,
+                     int kind, bool f32, void* stream);
+pa_status unpack_rfft(int nb, const BlockCopy* const* blocks, const void* const* srcs, void* dst,
+                      bool f32, void* stream);
+// plan_fft_check's question for unpack_r2r and unpack_rfft (one verdict for both); its own
+// cache, the same uniformity over the line
+pa_status plan_real_check(Plan* plan, bool f32);
 // real-line transforms (fft.cu): `nlines` dense, consecutive lines of N reals (src when forward,
 // dst when backward) <-> N/2 + 1 complex bins; N a power of two in 16..2048.  f32: Float32 <->
 // ComplexF32, else Float64 <-> ComplexF64

@@ -811,9 +811,21 @@ static pa_status one_sided(Plan* P, Comm* comm, const void* src, void* dst, unsi
   return PA_OK;
 }
 
+// the fused unpack of `mode` (fft_sign: the direction of FusedMode::fft)
+static pa_status unpack_fused(FusedMode mode, int r2r_kind, int nb, const BlockCopy* const* blocks,
+                              const void* const* srcs, void* dst, int fft_sign, bool f32,
+                              void* stream) {
+  switch (mode) {
+    case FusedMode::brfft: return unpack_brfft(nb, blocks, srcs, dst, f32, stream);
+    case FusedMode::r2r: return unpack_r2r(nb, blocks, srcs, dst, r2r_kind, f32, stream);
+    case FusedMode::rfft: return unpack_rfft(nb, blocks, srcs, dst, f32, stream);
+    default: return unpack_fft(nb, blocks, srcs, dst, fft_sign, f32, stream);
+  }
+}
+
 // ---- the staged schedules (PointToPoint / Alltoallv) --------------------------------
 static pa_status staged(Plan* P, Comm* comm, const void* src, void* dst, unsigned flags,
-                        bool brfft, bool stage_self, cudaStream_t user, cudaEvent_t buf_ev,
+                        FusedMode mode, int r2r_kind, bool stage_self, cudaStream_t user, cudaEvent_t buf_ev,
                         cudaEvent_t buf_unpack_ev) {
   TransposeState& S = *P->st;
   Buffers& B = *P->pout->bufs;
@@ -857,8 +869,9 @@ static pa_status staged(Plan* P, Comm* comm, const void* src, void* dst, unsigne
   // same stream (fused K3: src -> dest in one pass) and fills the HBM time the
   // NVLink-bound exchange leaves idle.  tunable "self_first" = 1 restores the
   // reference's order (self block packed first, :393-403).
-  // (brfft: the fused unpack is unpack_brfft, a backward transform)
-  const int fft_sign = brfft ? 1 : (flags & PA_FFT_FORWARD) ? -1 : ((flags & PA_FFT_BACKWARD) ? 1 : 0);
+  // (brfft / r2r / rfft: flags hold no direction, the fused unpack is that mode's)
+  const int fft_sign = mode != FusedMode::fft ? 1
+                       : (flags & PA_FFT_FORWARD) ? -1 : ((flags & PA_FFT_BACKWARD) ? 1 : 0);
   const bool self_first = stage_self || g_tun.self_first;
   if (stage_self) {
     RC(launch_block(self.pack, src, rbuf, S.pack_s, nullptr));  // tail of recv_buf (:393-403)
@@ -1043,8 +1056,7 @@ static pa_status staged(Plan* P, Comm* comm, const void* src, void* dst, unsigne
       sp.push_back(fused_self ? src : (const void*)rbuf);
     }
     const bool f32 = (flags & PA_FFT_F32) != 0;
-    RC(brfft ? unpack_brfft(nproc, bl.data(), sp.data(), dst, f32, S.unpack_s)
-             : unpack_fft(nproc, bl.data(), sp.data(), dst, fft_sign, f32, S.unpack_s));
+    RC(unpack_fused(mode, r2r_kind, nproc, bl.data(), sp.data(), dst, fft_sign, f32, S.unpack_s));
   } else if (stage_self) {
     RC(launch_block(self.unpack, rbuf, dst, S.unpack_s, nullptr));  // local data first (:511)
   }
@@ -1093,14 +1105,17 @@ static pa_status staged(Plan* P, Comm* comm, const void* src, void* dst, unsigne
 }
 
 pa_status transpose(Plan* P, Comm* comm, const void* src, void* dst, unsigned flags,
-                    void* stream, bool brfft) {
+                    void* stream, FusedMode mode, int r2r_kind) {
   // a rank may own nothing (more processes than points, Pencils.jl:193-218): its
   // empty arrays have no storage, yet it takes part in the exchange
   if ((!src && P->length_in > 0) || (!dst && P->length_out > 0)) {
     set_error("pa_transpose: null array pointer");
     return PA_EINVAL;
   }
-  const int fft_sign = brfft ? 1 : (flags & PA_FFT_FORWARD) ? -1 : ((flags & PA_FFT_BACKWARD) ? 1 : 0);
+  // (real_line -- brfft, r2r, rfft: a real array on one side; their entry points have checked src
+  //  against dst, whose element type or length the plan may not know)
+  const bool real_line = mode != FusedMode::fft;
+  const int fft_sign = real_line ? 1 : (flags & PA_FFT_FORWARD) ? -1 : ((flags & PA_FFT_BACKWARD) ? 1 : 0);
   const bool fft_f32 = (flags & PA_FFT_F32) != 0;  // ComplexF32 elements (elsize 8)
   if (fft_f32 && !fft_sign) {
     set_error("pa_transpose: PA_FFT_F32 without PA_FFT_FORWARD / PA_FFT_BACKWARD");
@@ -1108,8 +1123,10 @@ pa_status transpose(Plan* P, Comm* comm, const void* src, void* dst, unsigned fl
   }
   // a fused FFT this plan cannot run is refused before anything is enqueued -- and on every
   // rank of the line alike (the peers of a refusing rank must not start the exchange)
-  if (brfft)
+  if (mode == FusedMode::brfft)
     RC(plan_brfft_check(P, fft_f32));
+  else if (mode == FusedMode::r2r || mode == FusedMode::rfft)
+    RC(plan_real_check(P, fft_f32));
   else if (fft_sign)
     RC(plan_fft_check(P, fft_f32));
   RC(ensure_state(P));
@@ -1121,10 +1138,9 @@ pa_status transpose(Plan* P, Comm* comm, const void* src, void* dst, unsigned fl
 
   // src and dst may not alias -- except for the plain in-place transform along the contiguous
   // dim (same pencil on both sides, src == dst): a CTA reads its lines completely before it
-  // writes them back.  (brfft: pa_transpose_brfft has checked src against the REAL dst, whose
-  // length the plan does not know)
-  const bool fft_in_place = fft_sign && !brfft && src && src == dst && P->dim < 0 && P->same_perm;
-  if (fft_sign && !brfft && !fft_in_place && src && dst &&
+  // writes them back.  (real_line: checked by the entry point)
+  const bool fft_in_place = fft_sign && !real_line && src && src == dst && P->dim < 0 && P->same_perm;
+  if (fft_sign && !real_line && !fft_in_place && src && dst &&
       (src == dst || ranges_overlap(src, P->length_in * ES, dst, P->length_out * ES))) {
     set_error("fused FFT: src and dst must not alias (in place only between identical pencils)");
     return PA_EINVAL;
@@ -1133,8 +1149,7 @@ pa_status transpose(Plan* P, Comm* comm, const void* src, void* dst, unsigned fl
     // one block: the whole local array, src -> fft(permuted dest)
     if (P->length_out == 0) return PA_OK;
     const BlockCopy* b = &P->self_fused;
-    RC(brfft ? unpack_brfft(1, &b, &src, dst, fft_f32, user)
-             : unpack_fft(1, &b, &src, dst, fft_sign, fft_f32, user));
+    RC(unpack_fused(mode, r2r_kind, 1, &b, &src, dst, fft_sign, fft_f32, user));
     if (timing) {
       CU(cudaEventRecord(S.t[6], user));
       S.timed_once = true;
@@ -1171,7 +1186,7 @@ pa_status transpose(Plan* P, Comm* comm, const void* src, void* dst, unsigned fl
   Buffers& B = *P->pout->bufs;  // Po.send_buf / Po.recv_buf (:313-317)
   // (same base pointer counts even when one side is empty on this rank: every rank of
   //  an in-place transpose must take the same schedule)
-  const bool aliased = !brfft && src && dst &&
+  const bool aliased = !real_line && src && dst &&
       (src == dst || ranges_overlap(src, P->length_in * ES, dst, P->length_out * ES));
   const bool stage_self = aliased || (flags & PA_STAGE_SELF);
   const bool one = (P->method == PA_PEER_PUT || P->method == PA_PEER_GET) && !stage_self && nproc > 1;
@@ -1219,7 +1234,7 @@ pa_status transpose(Plan* P, Comm* comm, const void* src, void* dst, unsigned fl
     CU(cudaStreamWaitEvent(s, buf_unpack_ev, 0));
   }
   if (one) return one_sided(P, comm, src, dst, flags, user);
-  return staged(P, comm, src, dst, flags, brfft, stage_self, user, buf_ev, buf_unpack_ev);
+  return staged(P, comm, src, dst, flags, mode, r2r_kind, stage_self, user, buf_ev, buf_unpack_ev);
 }
 
 // MPI.Waitall(t::Transposition) (Transpositions.jl:127-130)

@@ -352,6 +352,60 @@ brfft_fusable(src::PencilArray{Complex{R}}, pc::Pencil; method = PointToPoint())
     ccall((:pa_plan_brfft_check, libpa), Cint, (Ptr{Cvoid}, Cuint), first(brfft_plan(src, pc, method)),
           fft_precision_flag(Complex{R})) == 0
 
+# Fused transposition of real arrays + a line transform along dest's first memory dimension, in
+# one kernel per GPU after the exchange (pa_transpose_r2r / pa_transpose_rfft): the steps of a
+# wall-bounded PencilFFTs transform without the real array in between.
+#   transpose_r2r!(dest, src, kind): dest = r2r(transpose(src), kind), both R on real pencils;
+#     kind FFTW.REDFT10 / REDFT01 / RODFT10 / RODFT01 as in r2r!.
+#   transpose_rfft!(dest, src, pr): dest = rfft(transpose(src)), `src` R on the real x-pencil,
+#     `dest` Complex{R} on the complex y-pencil; `pr`: the real y-pencil the plan transposes to,
+#     `Pencil(pencil(dest); size_global = (..., N, ...))` -- passed explicitly, as in
+#     transpose_brfft!.
+# Byte for byte the unfused pairs.  PointToPoint or Alltoallv; N a power of two in 16..2048.
+function real_plan(src::PencilArray{R}, pr::Pencil, method) where {R<:Union{Float64,Float32}}
+    H = handles(pencil(src).topology)
+    ex = Int64[extra_dims(src)...]
+    key = (objectid(pencil(src)), objectid(pr), Tuple(ex), sizeof(R), method_code(method))
+    plan = get!(H.plans, key) do
+        h = Ref{Ptr{Cvoid}}()
+        check(ccall((:pa_plan_create, libpa), Cint,
+            (Ptr{Cvoid}, Ptr{Cvoid}, Cint, Ptr{Int64}, Cint, Cint, Ptr{Ptr{Cvoid}}),
+            pencil_handle(H, pencil(src)), pencil_handle(H, pr), length(ex), ex, sizeof(R),
+            method_code(method), h))
+        h[]
+    end
+    plan, H
+end
+
+function transpose_r2r!(dest::PencilArray{R,N,<:CuArray}, src::PencilArray{R,N,<:CuArray},
+                        kind::Integer; method = PointToPoint(), waitall = true) where {R<:Union{Float64,Float32},N}
+    plan, H = real_plan(src, pencil(dest), method)
+    flags = (waitall ? Cuint(1) : Cuint(0)) | (R === Float32 ? Cuint(32) : Cuint(0))   # PA_WAITALL, PA_FFT_F32
+    ptr_or_null(A) = isempty(A) ? C_NULL : devptr(A)
+    check(ccall((:pa_transpose_r2r, libpa), Cint,
+        (Ptr{Cvoid}, Ptr{Cvoid}, Cint, Ptr{Cvoid}, Ptr{Cvoid}, Cuint, Ptr{Cvoid}),
+        plan, H.comm, Cint(kind), ptr_or_null(parent(src)), ptr_or_null(parent(dest)), flags, stream_ptr()))
+    dest
+end
+
+function transpose_rfft!(dest::PencilArray{Complex{R},N,<:CuArray}, src::PencilArray{R,N,<:CuArray},
+                         pr::Pencil; method = PointToPoint(), waitall = true) where {R<:Union{Float64,Float32},N}
+    plan, H = real_plan(src, pr, method)
+    flags = (waitall ? Cuint(1) : Cuint(0)) | (R === Float32 ? Cuint(32) : Cuint(0))   # PA_WAITALL, PA_FFT_F32
+    ptr_or_null(A) = isempty(A) ? C_NULL : devptr(A)
+    check(ccall((:pa_transpose_rfft, libpa), Cint,
+        (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Cuint, Ptr{Cvoid}),
+        plan, H.comm, pencil_handle(H, pencil(dest)), ptr_or_null(parent(src)), ptr_or_null(parent(dest)),
+        flags, stream_ptr()))
+    dest
+end
+
+# Whether transpose_r2r! / transpose_rfft! can run on this geometry (pa_plan_real_check, one
+# answer for both): the same answer on every rank of the grid line.
+real_fusable(src::PencilArray{R}, pr::Pencil; method = PointToPoint()) where {R<:Union{Float64,Float32}} =
+    ccall((:pa_plan_real_check, libpa), Cint, (Ptr{Cvoid}, Cuint), first(real_plan(src, pr, method)),
+          R === Float32 ? Cuint(32) : Cuint(0)) == 0
+
 # ---- host arrays: a chain of transpositions on `Array`-backed data ------------------
 # pa_host_chain_*: one submit = upload, every transpose! on the device, download;
 # asynchronous, double-buffered (download of one submit || upload of the next).

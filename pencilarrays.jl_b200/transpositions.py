@@ -6,6 +6,8 @@
     Waitall(t)                                            # MPI.Waitall(t)           :127-130
     transpose_(dest, src; method=...)                     # transpose!(dest, src)    :160-168
     t = Transposition(real_x, cplx_y; brfft=True)         # GPU extension: real = brfft(transpose)
+    t = Transposition(real_y, real_x; r2r="REDFT10")      # GPU extension: real = r2r(transpose)
+    t = Transposition(cplx_y, real_x; rfft=True)          # GPU extension: cplx = rfft(transpose)
 
 Python has no ``!`` in identifiers: ``transpose_`` (torch's in-place naming)
 stands for ``transpose!``; ``transpose_bang`` is an alias.  Errors follow the
@@ -254,7 +256,21 @@ def _brfft_pencil(real: Pencil) -> Pencil:
     return pc
 
 
+def _rfft_pencil(cplx: Pencil) -> Pencil:
+    """The real counterpart of a complex pencil of M points along its first memory dim -- N =
+    2 (M - 1) points there -- derived once per complex pencil, in the same family, like
+    :func:`_brfft_pencil`."""
+    pr = cplx.__dict__.get("_rfft_real")
+    if pr is None:
+        ax = as_tuple(cplx.perm, cplx.ndims)[0] - 1
+        pr = Pencil(cplx, size_global=tuple(2 * (n - 1) if d == ax else n
+                                            for d, n in enumerate(cplx.size_global)))
+        cplx._rfft_real = pr
+    return pr
+
+
 _BRFFT_PAIRS = {(torch.float64, torch.complex128): 0, (torch.float32, torch.complex64): _lib.PA_FFT_F32}
+_REAL_FLAGS = {torch.float64: 0, torch.float32: _lib.PA_FFT_F32}
 
 
 class Transposition:
@@ -264,17 +280,45 @@ class Transposition:
     along its first memory dim and ``Ai`` complex128 (complex64) on the complex y-pencil; the plan
     is the complex y -> x plan to the real pencil's N//2+1 counterpart, and ``transpose_(t)``
     writes ``Ao = brfft(transpose(Ai))`` in one kernel after the exchange (``pa_transpose_brfft``):
-    the last step of a PencilFFTs real-input backward transform, without the complex x array."""
+    the last step of a PencilFFTs real-input backward transform, without the complex x array.
 
-    def __init__(self, Ao: PencilArray, Ai: PencilArray, *, method=None, brfft=False):
+    ``r2r="REDFT10"`` (``"REDFT01"``, ``"RODFT10"``, ``"RODFT01"``; GPU extension): ``Ao`` and
+    ``Ai`` are float64 (float32) arrays on two real pencils, and ``transpose_(t)`` writes ``Ao =
+    r2r_(transpose(Ai), kind)`` along ``Ao``'s first memory dim in one kernel after the exchange
+    (``pa_transpose_r2r``).  ``rfft=True``: ``Ai`` is float64 (float32) on a real x-pencil and
+    ``Ao`` complex128 (complex64) on the complex y-pencil of N//2+1 points along its first memory
+    dim; the plan is the real x -> y plan to ``Ao``'s real counterpart, and ``transpose_(t)``
+    writes ``Ao = rfft_(transpose(Ai))`` (``pa_transpose_rfft``).  Both are byte for byte the
+    unfused pair, without the array in between.  ``brfft``, ``r2r`` and ``rfft`` exclude each
+    other."""
+
+    def __init__(self, Ao: PencilArray, Ai: PencilArray, *, method=None, brfft=False, r2r=None,
+                 rfft=False):
         method = PointToPoint() if method is None else method
         Pi, Po = Ai.pencil, Ao.pencil
         self.brfft = bool(brfft)
+        self.r2r = r2r
+        self.rfft = bool(rfft)
+        if self.brfft + (r2r is not None) + self.rfft > 1:
+            raise ArgumentError(_lib.PA_EINVAL, "brfft=, r2r= and rfft= exclude each other")
         if Ai.extra_dims != Ao.extra_dims:  # :99-103
             raise ArgumentError(_lib.PA_EINVAL,
                                 "incompatible number of extra dimensions of PencilArrays: "
                                 f"{Ai.extra_dims} != {Ao.extra_dims}")
-        if self.brfft:
+        if r2r is not None:
+            if r2r not in _R2R_KINDS:
+                raise ArgumentError(_lib.PA_EINVAL,
+                                    f"r2r must be one of {sorted(_R2R_KINDS)}: got {r2r!r}")
+            if Ai.dtype != Ao.dtype or Ai.dtype not in _REAL_FLAGS:
+                raise ArgumentError(_lib.PA_EINVAL, "r2r: dest and src must be two float64 or two "
+                                    f"float32 arrays: got {Ao.dtype} and {Ai.dtype}")
+        elif self.rfft:
+            if (Ai.dtype, Ao.dtype) not in _BRFFT_PAIRS:
+                raise ArgumentError(_lib.PA_EINVAL, "rfft: src and dest must be float64 and "
+                                    "complex128, or float32 and complex64: got "
+                                    f"{Ai.dtype} and {Ao.dtype}")
+            Po = _rfft_pencil(Ao.pencil)  # the plan's output: the real y-pencil
+        elif self.brfft:
             if (Ao.dtype, Ai.dtype) not in _BRFFT_PAIRS:
                 raise ArgumentError(_lib.PA_EINVAL, "brfft: dest and src must be float64 and "
                                     "complex128, or float32 and complex64: got "
@@ -289,10 +333,11 @@ class Transposition:
         self._plan = _get_plan(Pi, Po, Ai.extra_dims, Ai.elsize, method)  # remaining checks in C
         d = self._plan.info.dim
         self.dim = None if d == 0 else d  # :110
-        if self.brfft and d != 0 and self._plan.info.nproc > 1 and isinstance(method, (PeerPut, PeerGet)):
+        fused = "brfft" if self.brfft else "rfft" if self.rfft else "r2r" if r2r is not None else None
+        if fused and d != 0 and self._plan.info.nproc > 1 and isinstance(method, (PeerPut, PeerGet)):
             # (the same on every rank of the line: refused before the collective window setup)
-            raise ArgumentError(_lib.PA_EINVAL, "brfft: the one-sided methods have no unpack pass "
-                                "to fuse with; use PointToPoint / Alltoallv")
+            raise ArgumentError(_lib.PA_EINVAL, f"{fused}: the one-sided methods have no unpack "
+                                "pass to fuse with; use PointToPoint / Alltoallv")
         if d != 0 and self._plan.info.nproc > 1 and Pi.topology.comm.handle is not None:
             comm = Pi.topology.comm
             if isinstance(method, PeerPut):
@@ -320,7 +365,10 @@ class Transposition:
         is the same on every rank of the grid line; when it is False, transpose and transform
         separately.  complex64 arrays are asked about in single precision (``PA_FFT_F32``).
         For a ``brfft=True`` transposition: whether ``pa_transpose_brfft`` can run
-        (``pa_plan_brfft_check``)."""
+        (``pa_plan_brfft_check``); for ``r2r=`` / ``rfft=True``: whether ``pa_transpose_r2r`` /
+        ``pa_transpose_rfft`` can (``pa_plan_real_check``, one answer for both)."""
+        if self.r2r is not None or self.rfft:
+            return lib.pa_plan_real_check(self._plan.h, _REAL_FLAGS[self.Ai.dtype]) == _lib.PA_OK
         if self.brfft:
             return lib.pa_plan_brfft_check(self._plan.h, _fft_precision_flag(self.Ai)) == _lib.PA_OK
         return lib.pa_plan_fft_check_ex(self._plan.h, _fft_precision_flag(self.Ai)) == _lib.PA_OK
@@ -346,8 +394,8 @@ def transpose_(*args, method=None, waitall=True, overlap=True, stage_self=False,
     plan runs next -- execute as one kernel; ``dest`` receives the transformed array.
     complex128 arrays are transformed in double precision, complex64 in single.
 
-    A ``Transposition(..., brfft=True)`` runs the fused transpose + complex-to-real transform
-    (``fft=`` does not apply to it)."""
+    A ``Transposition(..., brfft=True)`` (``r2r=``, ``rfft=True``) runs the fused transpose +
+    complex-to-real (real-to-real, real-to-complex) transform; ``fft=`` does not apply to it."""
     if len(args) == 1 and isinstance(args[0], Transposition):
         t = args[0]
     elif len(args) == 2:
@@ -368,6 +416,20 @@ def transpose_(*args, method=None, waitall=True, overlap=True, stage_self=False,
                                      C.c_void_p(t.Ai.data_ptr() or None),
                                      C.c_void_p(t.Ao.data_ptr() or None),
                                      flags | _fft_precision_flag(t.Ai), _stream_ptr()))
+        return t if len(args) == 1 else args[0]
+    if t.r2r is not None or t.rfft:
+        what = "an rfft" if t.rfft else "an r2r"
+        if fft is not None:
+            raise ArgumentError(_lib.PA_EINVAL, f"{what} transposition implies its transform: "
+                                "transpose_(t) without fft=")
+        comm = t.Pi.topology.comm.handle
+        src, dst = C.c_void_p(t.Ai.data_ptr() or None), C.c_void_p(t.Ao.data_ptr() or None)
+        flags |= _REAL_FLAGS[t.Ai.dtype]
+        if t.rfft:
+            check(lib.pa_transpose_rfft(t.plan.h, comm, t.Ao.pencil._h, src, dst, flags, _stream_ptr()))
+        else:
+            check(lib.pa_transpose_r2r(t.plan.h, comm, _R2R_KINDS[t.r2r], src, dst, flags,
+                                       _stream_ptr()))
         return t if len(args) == 1 else args[0]
     if fft is not None:
         if fft in ("forward", -1):
