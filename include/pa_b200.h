@@ -74,9 +74,13 @@ typedef enum pa_method {
  * the reason the pencil is permuted, docs/src/Pencils.md:210-214) run as ONE kernel --
  * `dst` receives fft(transposed array) (forward: exp(-2*pi*i*jk/n); backward: the
  * unnormalised inverse, as FFTW / PencilFFTs).  ComplexF64 (or ComplexF32 with
- * PA_FFT_F32), power-of-two lines of 8..1024 points, staged methods or local
+ * PA_FFT_F32), power-of-two lines of 8..1024 points, staged methods, PA_PEER_GET or local
  * transposes, src and dst not aliased;
- * PA_EINVAL otherwise (transpose, then transform, separately).  A plan between
+ * PA_EINVAL otherwise (transpose, then transform, separately; PA_PEER_PUT has no pass to
+ * fuse with).  On a PA_PEER_GET plan the fused step is ONE kernel per rank that gathers every
+ * line straight out of the peers' src arrays (and the local src), transforms and stores it,
+ * with the window protocol inside the launch; without PA_WAITALL only the wait that guards
+ * the reuse of src is deferred to pa_wait, as for the plain PeerGet.  A plan between
  * IDENTICAL pencils with src == dst is the plain in-place transform along the
  * contiguous dim -- the first step of a PencilFFTs-style 3-d transform, whose other
  * two steps are the fused transposes.                                               */
@@ -272,6 +276,18 @@ pa_status pa_get(pa_plan* plan, int n, const void* peer_src, void* dst, void* st
 pa_status pa_put_all(pa_plan* plan, const void* src, void* const* peers, int max_ctas,
                      void* stream);
 pa_status pa_get_all(pa_plan* plan, void* const* peers, void* dst, int max_ctas, void* stream);
+/* K2-get of every remote block, the self block and the 1-d FFT along dst's contiguous dim in ONE
+ * launch: the kernel a PA_PEER_GET pa_transpose with PA_FFT_FORWARD / PA_FFT_BACKWARD runs, here
+ * without the window protocol.  dst = fft(transpose(...)) gathered from `src` (this rank's src
+ * parent, for the self block) and `peers[n-1]` = peer n's src parent array (its layout, as
+ * mapped here; the self entry is ignored).  flags: PA_FFT_FORWARD or PA_FFT_BACKWARD, optionally
+ * with PA_FFT_F32 (ComplexF32, elsize-8 plan); anything else is PA_EINVAL.  The plan's
+ * pa_plan_fft_check_ex verdict is asked first; NULL pointers are allowed only for empty blocks /
+ * arrays, arrays element-aligned (dst 16 bytes), src and dst not overlapping.  Every refusal
+ * happens on the host before anything is enqueued; without a device PA_ENOGPU after those
+ * checks.  The result equals the staged fused transpose byte for byte.                        */
+pa_status pa_get_all_fft(pa_plan* plan, const void* src, void* const* peers, void* dst,
+                         unsigned flags, void* stream);
 /* transpose_impl!(::Nothing) / permute_local! (:213-270).  `scratch` must hold
  * length_out elements when src and dst alias, may be NULL otherwise.        */
 pa_status pa_permute_local(pa_plan* plan, const void* src, void* dst,

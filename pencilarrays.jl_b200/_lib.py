@@ -110,6 +110,7 @@ SIGNATURES = {
     "pa_get": (C.c_int, [_P, C.c_int, _P, _P, _P]),
     "pa_put_all": (C.c_int, [_P, _P, C.POINTER(_P), C.c_int, _P]),
     "pa_get_all": (C.c_int, [_P, C.POINTER(_P), _P, C.c_int, _P]),
+    "pa_get_all_fft": (C.c_int, [_P, _P, C.POINTER(_P), _P, C.c_uint, _P]),
     "pa_copy_self": (C.c_int, [_P, _P, _P, _P]),
     "pa_permute_local": (C.c_int, [_P, _P, _P, _P, _P]),
     "pa_box_copy": (C.c_int, [C.c_int, _I64P, _I64P, _I64P, C.c_int, _P, _P, _P,

@@ -496,6 +496,67 @@ pa_status pa_get_all(pa_plan* plan, void* const* peers, void* dst, int max_ctas,
   GUARD({ return all_blocks(plan, true, dst, peers, max_ctas, stream); })
 }
 
+static pa_status fused_pointers(const char* who, const void* src, i64 src_bytes, const void* dst,
+                                i64 dst_bytes);
+
+// The one-sided fused gather + FFT without the window protocol.  Every check runs on the host
+// before any device call.
+static pa_status get_all_fft(pa_plan* plan, const void* src, void* const* peers, void* dst,
+                             unsigned flags, void* stream) {
+  const char* who = "pa_get_all_fft";
+  if (!plan) {
+    set_error("%s: null plan", who);
+    return PA_EINVAL;
+  }
+  Plan& P = *plan->p;
+  if (P.dim < 0) {
+    set_error("%s: plan has no exchange", who);
+    return PA_EINVAL;
+  }
+  const unsigned dir = flags & ~PA_FFT_F32;
+  if (dir != PA_FFT_FORWARD && dir != PA_FFT_BACKWARD) {
+    set_error("%s: flags must be exactly PA_FFT_FORWARD or PA_FFT_BACKWARD, optionally with "
+              "PA_FFT_F32", who);
+    return PA_EINVAL;
+  }
+  const bool f32 = (flags & PA_FFT_F32) != 0;
+  // the verdict pa_transpose asks (for a PeerGet plan it covers this gather)
+  pa_status s = plan_fft_check(&P, f32);
+  if (s != PA_OK) return s;
+  const i64 es = P.elsize;
+  const i64 src_bytes = P.length_in * es, dst_bytes = P.length_out * es;
+  std::vector<const BlockCopy*> blocks;
+  std::vector<const void*> srcs;
+  for (int n = 0; n < P.nproc; ++n) {
+    const bool self = n == P.self_index;
+    const BlockCopy& b = self ? P.self_fused : P.peers[n].get;
+    const void* p = self ? src : (peers ? peers[n] : nullptr);
+    if (b.count > 0 && !p) {
+      set_error(self ? "%s: null src for a non-empty self block"
+                     : "%s: null peer array for a non-empty block (peer %d)", who, n + 1);
+      return PA_EINVAL;
+    }
+    if (b.count > 0 && ((uintptr_t)p % es)) {
+      set_error("%s: arrays must be aligned to the %lld-byte element", who, (long long)es);
+      return PA_EINVAL;
+    }
+    blocks.push_back(&b);
+    srcs.push_back(p);
+  }
+  s = fused_pointers(who, src, src_bytes, dst, dst_bytes);
+  if (s != PA_OK) return s;
+  s = need_gpu();
+  if (s != PA_OK) return s;
+  bool launched = false;
+  return get_fft(P.nproc, blocks.data(), srcs.data(), dst, dir == PA_FFT_FORWARD ? -1 : 1, f32, nullptr,
+                 stream, &launched);
+}
+
+pa_status pa_get_all_fft(pa_plan* plan, const void* src, void* const* peers, void* dst, unsigned flags,
+                         void* stream) {
+  GUARD({ return get_all_fft(plan, src, peers, dst, flags, stream); })
+}
+
 pa_status pa_copy_self(pa_plan* plan, const void* src, void* dst, void* stream) {
   if (!plan) return PA_EINVAL;
   pa_status s = need_gpu();

@@ -41,6 +41,7 @@
 #define PA_FFT_TWIDDLE_LOOKUPS 1
 #endif
 #include "fft_core.hpp"
+#include "flags.cuh"
 #include "pa_internal.hpp"
 
 namespace pa {
@@ -251,8 +252,9 @@ __device__ __forceinline__ long long cta_offsets(const FftParams& p, int C, long
   return x0;
 }
 
+// One CTA of the fused unpack + FFT: gather its C lines from every block, transform, store.
 template <int LOGL, int C, class T>
-__global__ void __launch_bounds__(FFT_THREADS) k_unpack_fft(const __grid_constant__ FftParams p) {
+__device__ __forceinline__ void unpack_fft_cta(const FftParams& p) {
   using cx = cplx_t<T>;
   using V = typename Vec2<T>::type;
   constexpr int L = 1 << LOGL;
@@ -335,6 +337,59 @@ __global__ void __launch_bounds__(FFT_THREADS) k_unpack_fft(const __grid_constan
         __stcs(out + k, vec2(v.x, v.y));
       }
     }
+  }
+}
+
+template <int LOGL, int C, class T>
+__global__ void __launch_bounds__(FFT_THREADS) k_unpack_fft(const __grid_constant__ FftParams p) {
+  unpack_fft_cta<LOGL, C, T>(p);
+}
+
+// ---- one-sided fused unpack + FFT (PeerGet, DESIGN §3h) ----
+// The same CTA as k_unpack_fft, its remote blocks read straight out of the peers' src arrays
+// through their peer mappings, bracketed by k_multi's window protocol: the first CTAs tell every
+// peer READY ("my src is final and may be read"), and every CTA waits for READY from every peer
+// before its first remote load (each line gathers from every block).  The CTA that finishes last
+// tells every peer DONE ("I have finished reading your src"); the wait for the peers' DONE only
+// guards the reuse of my src, so it is not in the kernel (get flavour: mf.wait_done is ignored).
+// Empty flag sets: the plain gather from the mapped arrays (pa_get_all_fft, or a launch that
+// standalone flag kernels bracket).
+struct FftGetParams {
+  FftParams p;
+  MultiFlags mf;
+};
+static_assert(sizeof(FftGetParams) <= 4096, "FftParams + MultiFlags must fit the kernel parameters");
+
+// (a register cap instead of __launch_bounds__(FFT_THREADS): under the launch bound ptxas
+//  spills 4 bytes in the 64- and 128-point double-precision instantiations, as it does in
+//  k_unpack_fft; with the cap no instantiation spills)
+template <int LOGL, int C, class T>
+__global__ void __maxnreg__(128) k_get_fft(const __grid_constant__ FftGetParams gp) {
+  const MultiFlags& mf = gp.mf;
+  if (mf.ready.n > 0) {
+    if ((int)threadIdx.x < mf.ready.n) {
+      if (blockIdx.x < 8) flag_signal(mf.ready.remote[threadIdx.x], mf.ready.seq[threadIdx.x]);
+      flag_wait(mf.ready.local[threadIdx.x], mf.ready.seq[threadIdx.x], mf.timeout_ns, mf.err);
+    }
+    __syncthreads();
+  }
+  unpack_fft_cta<LOGL, C, T>(gp.p);
+  if (mf.done.n > 0) {
+    // every load of this CTA has been consumed (its lines are in shared memory or stored);
+    // the last CTA to get here closes the window.  (No static shared memory: the 1024-point
+    // instantiations fill three CTAs per SM with their dynamic shared memory alone)
+    __syncthreads();
+    int last = 0;
+    if (threadIdx.x == 0) {
+      __threadfence_system();
+      last = atomicAdd(mf.counter, 1u) == gridDim.x - 1;
+      if (last) {
+        *mf.counter = 0;  // ready for the next launch (stream-ordered after this one)
+        __threadfence_system();
+      }
+    }
+    if (__syncthreads_or(last) && (int)threadIdx.x < mf.done.n)
+      flag_signal(mf.done.remote[threadIdx.x], mf.done.seq[threadIdx.x]);
   }
 }
 
@@ -1079,6 +1134,68 @@ pa_status unpack_fft(int nb, const BlockCopy* const* blocks, const void* const* 
   return PA_OK;
 }
 
+pa_status get_fft(int nb, const BlockCopy* const* blocks, const void* const* srcs, void* dst, int sign,
+                  bool f32, const MultiFlags* mf, void* stream, bool* launched) {
+  // (pa_transpose and pa_get_all_fft have already asked plan_fft_check)
+  *launched = false;
+  FftGetParams gp;
+  int C = 0;
+  unsigned long long grid = 0;
+  pa_status s = fft_geometry(nb, blocks, srcs, dst, f32, FusedMode::fft, gp.p, &C, &grid);
+  if (s != PA_OK || grid == 0) return s;
+  FftParams& p = gp.p;
+  memset(&gp.mf, 0, sizeof gp.mf);
+  if (mf) gp.mf = *mf;
+  const int logL = p.logL;
+  p.sign = sign < 0 ? -1 : 1;
+  p.tw = twiddles(p.L, f32);
+  if (!p.tw) {
+    set_error("fused FFT: twiddle table allocation failed");
+    cudaGetLastError();
+    return PA_ENOMEM;
+  }
+  const size_t smem = (f32 ? sizeof(pa_fft::cplxf) : sizeof(cplx)) * (size_t)C * p.pitch;
+  cudaError_t e = cudaSuccess;
+  auto launch = [&](auto kern) {
+    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout,
+                         cudaSharedmemCarveoutMaxShared);
+    cudaGetLastError();
+    kern<<<(unsigned)grid, FFT_THREADS, smem, (cudaStream_t)stream>>>(gp);
+    e = cudaGetLastError();
+  };
+  if (f32) {
+    switch (logL) {
+      case 3: launch(k_get_fft<3, 16, float>); break;
+      case 4: launch(k_get_fft<4, 16, float>); break;
+      case 5: launch(k_get_fft<5, 16, float>); break;
+      case 6: launch(k_get_fft<6, 16, float>); break;
+      case 7: launch(k_get_fft<7, 16, float>); break;
+      case 8: launch(k_get_fft<8, 16, float>); break;
+      case 9: launch(k_get_fft<9, 16, float>); break;
+      default: launch(k_get_fft<10, 8, float>); break;
+    }
+  } else {
+    switch (logL) {
+      case 3: launch(k_get_fft<3, 8, double>); break;
+      case 4: launch(k_get_fft<4, 8, double>); break;
+      case 5: launch(k_get_fft<5, 8, double>); break;
+      case 6: launch(k_get_fft<6, 8, double>); break;
+      case 7: launch(k_get_fft<7, 8, double>); break;
+      case 8: if (C == 4) launch(k_get_fft<8, 4, double>); else launch(k_get_fft<8, 8, double>); break;
+      case 9: if (C == 4) launch(k_get_fft<9, 4, double>); else launch(k_get_fft<9, 8, double>); break;
+      default: launch(k_get_fft<10, 4, double>); break;
+    }
+  }
+  if (e != cudaSuccess) {
+    set_error("one-sided fused FFT kernel launch failed: %s", cudaGetErrorString(e));
+    return PA_ECUDA;
+  }
+  count_launch();
+  *launched = true;
+  return PA_OK;
+}
+
 pa_status unpack_brfft(int nb, const BlockCopy* const* blocks, const void* const* srcs, void* dst,
                        bool f32, void* stream) {
   // (pa_transpose_brfft has already asked plan_brfft_check for every rank of the line)
@@ -1260,7 +1377,9 @@ pa_status unpack_rfft(int nb, const BlockCopy* const* blocks, const void* const*
 // before the exchange while its peers went ahead would leave them waiting on flags it never
 // sets.  So the answer depends on the global geometry only: the blocks that EVERY rank of the
 // line would gather -- each rank's plan rebuilt from the pencils with that rank's coordinates --
-// with the self block read from src and staged through recv_buf alike.
+// with the self block read from src and staged through recv_buf alike.  A PeerGet plan may also
+// run the complex FFT one-sided (k_get_fft): its blocks are then the peers' get blocks, read from
+// their src arrays, and the self block from src, so that configuration is checked as well.
 static pa_status fused_check(Plan* P, bool f32, FusedMode mode) {
   if (mode == FusedMode::r2r || mode == FusedMode::rfft) {
     if (P->elsize != (f32 ? 4 : 8)) {
@@ -1299,10 +1418,13 @@ static pa_status fused_check(Plan* P, bool f32, FusedMode mode) {
       hold.reset(q);
       Q = q;
     }
-    for (int staged_self = 0; staged_self < 2; ++staged_self) {
+    // 0: self block from src, 1: self block staged through recv_buf, 2: one-sided get
+    const int configs = (mode == FusedMode::fft && P->method == PA_PEER_GET) ? 3 : 2;
+    for (int cfg = 0; cfg < configs; ++cfg) {
       std::vector<const BlockCopy*> bl;
       for (int k = 0; k < Q->nproc; ++k)
-        bl.push_back(k == Q->self_index && !staged_self ? &Q->self_fused : &Q->peers[k].unpack);
+        bl.push_back(k == Q->self_index && cfg != 1 ? &Q->self_fused
+                                                    : cfg == 2 ? &Q->peers[k].get : &Q->peers[k].unpack);
       pa_status s = fft_geometry(Q->nproc, bl.data(), nullptr, nullptr, f32, mode, p, &C, &grid);
       if (s != PA_OK) {
         if (n != P->self_index) {

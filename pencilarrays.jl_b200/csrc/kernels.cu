@@ -36,6 +36,7 @@
 #include <atomic>
 #include <cstdint>
 
+#include "flags.cuh"
 #include "pa_internal.hpp"
 
 namespace pa {
@@ -441,34 +442,7 @@ __global__ void __launch_bounds__(256) k_box(const __grid_constant__ KParams p) 
   }
 }
 
-// ---- flag words over NVLink ---------------------------------------------------
-// A word only ever increases: signals are max-reductions with release semantics
-// at system scope (every earlier store of this GPU, peer memory included, is
-// visible before the new value), waits are acquire loads.  A wait that exceeds
-// the time-out records the failure in mapped host memory and traps: nothing that
-// depends on the missing peer may run on.
-__device__ __forceinline__ void flag_signal(ull* remote, ull seq) {
-  __threadfence_system();
-  asm volatile("red.release.sys.global.max.u64 [%0], %1;" ::"l"(remote), "l"(seq) : "memory");
-}
-__device__ __forceinline__ void flag_wait(const ull* local, ull seq, ull timeout_ns, int* err) {
-  ull t0, now, v;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
-  for (;;) {
-    asm volatile("ld.acquire.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(local) : "memory");
-    if (v >= seq) return;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now));
-    if (timeout_ns && now - t0 > timeout_ns) {
-      if (err) {
-        *(volatile int*)err = 1;
-        __threadfence_system();
-      }
-      __trap();
-    }
-    __nanosleep(100);
-  }
-}
-
+// ---- flag words over NVLink (flag_signal / flag_wait: flags.cuh) ----------------
 struct FlagKernelParams {
   int n;
   ull* remote[64];

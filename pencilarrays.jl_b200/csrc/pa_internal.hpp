@@ -290,9 +290,15 @@ pa_status host_chain_time_end(HostChain* c, float* ms);
 // f32: ComplexF32 elements and fp32 arithmetic (PA_FFT_F32), else ComplexF64
 pa_status unpack_fft(int nb, const BlockCopy* const* blocks, const void* const* srcs, void* dst,
                      int sign, bool f32, void* stream);
+// the same kernel one-sided (fft.cu, k_get_fft): srcs[i] are the peers' src arrays as mapped here
+// (the self block's: the local src), read in place, and `mf` (NULL: none) the window protocol
+// spoken inside the launch.  *launched = false: this rank has no destination lines and nothing
+// was launched -- the caller then speaks the protocol with flag kernels
+pa_status get_fft(int nb, const BlockCopy* const* blocks, const void* const* srcs, void* dst, int sign,
+                  bool f32, const MultiFlags* mf, void* stream, bool* launched);
 // can pa_transpose fuse a FFT of the given precision into this plan's unpack?  The same answer
 // on every rank of the grid line (global geometry only); PA_EINVAL + last_error otherwise.
-// No device call.
+// PeerGet plans: the one-sided gather of get_fft too.  No device call.
 pa_status plan_fft_check(Plan* plan, bool f32);
 // fused unpack + complex-to-real line transform (fft.cu, k_unpack_brfft): the blocks tile lines
 // of N/2 + 1 bins of the complex destination box; `dst` is the real array of N reals per line

@@ -675,11 +675,15 @@ static BlockCopy contiguous_block(i64 bytes, const void* src, const void* dst) {
 // READY ("my side of the window may be touched": my dest may be overwritten /
 // my src is final) before the first remote access, DONE ("all my accesses to
 // your memory are complete") after the last.
+// fft_sign != 0 (PeerGet only): the fused gather + FFT (k_get_fft) replaces the get kernel and
+// the self block -- ONE kernel reads every line from the peers' src and the local src,
+// transforms and stores it; the protocol around it is the same.
 static pa_status one_sided(Plan* P, Comm* comm, const void* src, void* dst, unsigned flags,
-                           cudaStream_t user) {
+                           int fft_sign, cudaStream_t user) {
   TransposeState& S = *P->st;
   const int nproc = P->nproc, me = P->self_index;
   const bool get = P->method == PA_PEER_GET;
+  const bool fft = fft_sign != 0;
   const bool timing = S.timing;
   // (a rank none of whose peers owns anything has no window to register: nothing will be
   //  put / got, but it still speaks the protocol)
@@ -695,12 +699,15 @@ static pa_status one_sided(Plan* P, Comm* comm, const void* src, void* dst, unsi
     }
   RC(check_fence_err(comm));
 
-  // self block: fused K3 on the low-priority stream, beside the remote kernels
-  if (timing) CU(cudaEventRecord(S.t[4], S.unpack_s));
-  RC(launch_block(P->self_fused, src, dst, S.unpack_s, nullptr, g_tun.oneside_self_ctas));
-  CU(cudaEventRecord(S.ev_unpack_done, S.unpack_s));
-  if (timing) CU(cudaEventRecord(S.t[5], S.unpack_s));
+  if (!fft) {
+    // self block: fused K3 on the low-priority stream, beside the remote kernels
+    if (timing) CU(cudaEventRecord(S.t[4], S.unpack_s));
+    RC(launch_block(P->self_fused, src, dst, S.unpack_s, nullptr, g_tun.oneside_self_ctas));
+    CU(cudaEventRecord(S.ev_unpack_done, S.unpack_s));
+    if (timing) CU(cudaEventRecord(S.t[5], S.unpack_s));
+  }
   if (timing) CU(cudaEventRecord(S.t[2], S.comm_s));
+  if (timing && fft) CU(cudaEventRecord(S.t[4], S.comm_s));
 
   const bool use_flags = comm->flags_ready && !g_tun.nccl_fences;
   if (!use_flags && !comm->comm) {
@@ -722,6 +729,19 @@ static pa_status one_sided(Plan* P, Comm* comm, const void* src, void* dst, unsi
     peer_rank.push_back(P->peers[n].world_rank);
   }
   const int np = nproc - 1;
+  // fft: every get block and the self block in one kernel, `mf` spoken inside it (NULL: none);
+  // *launched = false on a rank without destination lines
+  std::vector<const BlockCopy*> fb;
+  std::vector<const void*> fs;
+  for (int n = 0; fft && n < nproc; ++n) {
+    fb.push_back(n == me ? &P->self_fused : &P->peers[n].get);
+    fs.push_back(n == me ? src : (const void*)win[n]);
+  }
+  auto fused = [&](const MultiFlags* mf, bool* launched) {
+    return get_fft(nproc, fb.data(), fs.data(), dst, fft_sign, (flags & PA_FFT_F32) != 0, mf, S.comm_s,
+                   launched);
+  };
+  bool launched = false;
 
   if (use_flags) {
     std::vector<ull*> rr(np), rl(np), dr(np), dl(np);
@@ -748,8 +768,15 @@ static pa_status one_sided(Plan* P, Comm* comm, const void* src, void* dst, unsi
       mf.counter = S.counter;
       mf.timeout_ns = timeout_ns();
       mf.err = comm->fence_err;
-      rc = launch_multi(np, blocks.data(), srcs.data(), dsts.data(), S.comm_s, g_tun.remote_ctas,
-                        &mf);
+      if (fft) {
+        RC(fused(&mf, &launched));
+        // (no destination lines on this rank: its src is still read, so the flag kernels below
+        //  speak the protocol without a kernel between them)
+        rc = launched ? PA_OK : PA_EINCOMPAT;
+      } else {
+        rc = launch_multi(np, blocks.data(), srcs.data(), dsts.data(), S.comm_s, g_tun.remote_ctas,
+                          &mf);
+      }
       if (rc != PA_OK && rc != PA_EINCOMPAT) return rc;
       if (rc == PA_OK) {
         CU(cudaEventRecord(S.ev_allpacked, S.comm_s));
@@ -764,8 +791,11 @@ static pa_status one_sided(Plan* P, Comm* comm, const void* src, void* dst, unsi
       // spoken by standalone flag kernels around per-block launches
       RC(launch_flags(np, rr.data(), rl.data(), rs.data(), true, true, timeout_ns(),
                       comm->fence_err, S.comm_s));
-      for (int i = 0; i < np; ++i)
-        RC(launch_block(*blocks[i], srcs[i], dsts[i], S.comm_s, nullptr, g_tun.remote_ctas));
+      if (fft)
+        RC(fused(nullptr, &launched));
+      else
+        for (int i = 0; i < np; ++i)
+          RC(launch_block(*blocks[i], srcs[i], dsts[i], S.comm_s, nullptr, g_tun.remote_ctas));
       CU(cudaEventRecord(S.ev_allpacked, S.comm_s));
       if (timing) CU(cudaEventRecord(S.t[1], S.comm_s));
       RC(launch_flags(np, dr.data(), dl.data(), ds.data(), true, true, timeout_ns(),
@@ -785,11 +815,21 @@ static pa_status one_sided(Plan* P, Comm* comm, const void* src, void* dst, unsi
       return PA_OK;
     };
     RC(line_barrier());
-    for (int i = 0; i < np; ++i)
-      RC(launch_block(*blocks[i], srcs[i], dsts[i], S.comm_s, nullptr, g_tun.remote_ctas));
+    if (fft)
+      RC(fused(nullptr, &launched));
+    else
+      for (int i = 0; i < np; ++i)
+        RC(launch_block(*blocks[i], srcs[i], dsts[i], S.comm_s, nullptr, g_tun.remote_ctas));
     CU(cudaEventRecord(S.ev_allpacked, S.comm_s));
     if (timing) CU(cudaEventRecord(S.t[1], S.comm_s));
     RC(line_barrier());
+  }
+  if (fft) {
+    // dst is complete once the fused kernel is (ev_allpacked); the DONE steps behind it on the
+    // comm stream only guard the reuse of src
+    CU(cudaStreamWaitEvent(S.unpack_s, S.ev_allpacked, 0));
+    CU(cudaEventRecord(S.ev_unpack_done, S.unpack_s));
+    if (timing) CU(cudaEventRecord(S.t[5], S.unpack_s));
   }
   CU(cudaEventRecord(S.ev_comm_done, S.comm_s));
   if (timing) CU(cudaEventRecord(S.t[3], S.comm_s));
@@ -1190,7 +1230,9 @@ pa_status transpose(Plan* P, Comm* comm, const void* src, void* dst, unsigned fl
       (src == dst || ranges_overlap(src, P->length_in * ES, dst, P->length_out * ES));
   const bool stage_self = aliased || (flags & PA_STAGE_SELF);
   const bool one = (P->method == PA_PEER_PUT || P->method == PA_PEER_GET) && !stage_self && nproc > 1;
-  if (fft_sign && one) {
+  // (PeerGet runs the complex FFT one-sided, k_get_fft; a put has nothing to fuse with, and the
+  //  real-line modes have been refused for both methods by their plan checks)
+  if (fft_sign && one && (P->method == PA_PEER_PUT || real_line)) {
     set_error("fused FFT: the one-sided methods have no unpack pass to fuse with; use "
               "PointToPoint / Alltoallv");
     return PA_EINVAL;
@@ -1233,7 +1275,7 @@ pa_status transpose(Plan* P, Comm* comm, const void* src, void* dst, unsigned fl
     CU(cudaStreamWaitEvent(s, buf_ev, 0));
     CU(cudaStreamWaitEvent(s, buf_unpack_ev, 0));
   }
-  if (one) return one_sided(P, comm, src, dst, flags, user);
+  if (one) return one_sided(P, comm, src, dst, flags, fft_sign, user);
   return staged(P, comm, src, dst, flags, mode, r2r_kind, stage_self, user, buf_ev, buf_unpack_ev);
 }
 

@@ -230,7 +230,8 @@ const DeviceTransposition{T,N} = Transposition{T,N,<:Pencil,<:Pencil,
 # `fft = :forward | :backward` (GPU extension, PA_FFT_FORWARD / PA_FFT_BACKWARD): the unpack
 # and the 1-d FFT along dest's contiguous dimension -- the next step of a PencilFFTs plan --
 # run as ONE kernel (ComplexF64, or ComplexF32 in single precision; power-of-two lines of
-# 8..1024 points, staged methods).
+# 8..1024 points, staged methods or PeerGet -- there the kernel reads every line straight out
+# of the peers' src arrays, with no staging; PeerPut is refused).
 # PA_FFT_F32 for ComplexF32 elements: the plan only knows sizeof(T), and 8 bytes is Float64 too
 fft_precision_flag(::Type{T}) where {T} = T === ComplexF32 ? Cuint(32) : Cuint(0)
 

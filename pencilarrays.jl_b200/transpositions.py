@@ -66,7 +66,9 @@ class PeerGet(AbstractTransposeMethod):
     """Pull flavour of :class:`PeerPut`: the unpack kernel of each remote block
     loads straight out of the source rank's ``src`` array over NVLink.  The
     window is on ``src``; ``waitall=False`` defers only the fence that guards
-    the reuse of ``src`` -- the role ``MPI.Waitall(t)`` has in the reference."""
+    the reuse of ``src`` -- the role ``MPI.Waitall(t)`` has in the reference.
+    ``transpose_(t, fft=...)`` fuses the FFT here too: one kernel per rank gathers
+    every line from the peers' ``src`` arrays and its own, transforms and stores it."""
     code = _lib.PA_PEER_GET
 
 
@@ -364,6 +366,8 @@ class Transposition:
         kernel (``pa_plan_fft_check``).  The answer depends on the global geometry only, so it
         is the same on every rank of the grid line; when it is False, transpose and transform
         separately.  complex64 arrays are asked about in single precision (``PA_FFT_F32``).
+        With ``PeerGet`` the answer covers the one-sided fused kernel as well; ``PeerPut`` has
+        nothing to fuse with, and ``transpose_(t, fft=...)`` refuses it whatever this says.
         For a ``brfft=True`` transposition: whether ``pa_transpose_brfft`` can run
         (``pa_plan_brfft_check``); for ``r2r=`` / ``rfft=True``: whether ``pa_transpose_r2r`` /
         ``pa_transpose_rfft`` can (``pa_plan_real_check``, one answer for both)."""
@@ -392,7 +396,10 @@ def transpose_(*args, method=None, waitall=True, overlap=True, stage_self=False,
     ``fft="forward"`` / ``"backward"`` (GPU extension, SURVEY 8 f2): the unpack and the
     1-d complex FFT along ``dest``'s contiguous dimension -- the step a PencilFFTs-style
     plan runs next -- execute as one kernel; ``dest`` receives the transformed array.
-    complex128 arrays are transformed in double precision, complex64 in single.
+    complex128 arrays are transformed in double precision, complex64 in single.  With the
+    staged methods the fused kernel is the unpack; with ``PeerGet`` it reads every line straight
+    out of the peers' ``src`` arrays (one kernel per rank, no staging; ``waitall=False`` defers
+    only the fence that guards the reuse of ``src``).  ``PeerPut`` is refused.
 
     A ``Transposition(..., brfft=True)`` (``r2r=``, ``rfft=True``) runs the fused transpose +
     complex-to-real (real-to-real, real-to-complex) transform; ``fft=`` does not apply to it."""
