@@ -475,6 +475,53 @@ pa_status pa_transpose_rfft(pa_plan* plan, pa_comm* comm, const pa_pencil* cplx,
  * pa_plan_brfft_check verdicts.  Host-only; no device needed.                             */
 pa_status pa_plan_real_check(const pa_plan* plan, unsigned flags);
 
+/* ---- send-side fused transform + transposition (PA_PEER_PUT) -------------------------
+ * dst = transpose(T(src)), T along the FIRST memory dim of the plan's input pencil (not
+ * decomposed), in ONE kernel per rank: it loads whole local source lines, transforms them in
+ * shared memory and stores every output bin into the block that owns it -- the self block into
+ * dst, every other block straight into its rank's dst through the PeerPut window (pa_plan_set_window).
+ * The window protocol runs inside the launch (standalone flag kernels around it when tunable
+ * multi_put = 0 or the line has more than 8 peers; NCCL line barriers under nccl_fences); a rank
+ * without source lines launches no transform but still takes part in the protocol.  Events and
+ * PA_WAITALL behave as for the plain PeerPut transposition.  Local plans (no exchange, or a grid
+ * line of one rank) of any method run the kernel on `stream` alone.  Other methods that exchange
+ * data are refused: there the receive-side fusion (pa_transpose with PA_FFT_*, pa_transpose_rfft)
+ * covers the chain.  The result equals the unfused pair under the same tunables byte for byte.
+ *
+ * pa_fft_put: T is the complex FFT (PA_FFT_FORWARD, or the unnormalised PA_FFT_BACKWARD) of a
+ *   ComplexF64 plan (with PA_FFT_F32 ComplexF32, elsize 8), L a power of two in 8..1024;
+ *   dst equals fft_ on a copy of src followed by pa_transpose.
+ * pa_rfft_put: T is the r2c transform of pa_rfft; `plan` is the COMPLEX plan from the N/2+1-bin
+ *   counterpart of `real` (related to it as `cplx` to `real` in pa_rfft) to dst's pencil; src is the
+ *   Float64 (Float32 with PA_FFT_F32) array on `real`, N a power of two in 16..2048; dst equals
+ *   pa_rfft followed by pa_transpose of the complex array.
+ *
+ * flags: pa_fft_put exactly one of PA_FFT_FORWARD / PA_FFT_BACKWARD, optionally with PA_FFT_F32
+ * and PA_WAITALL; pa_rfft_put any of PA_FFT_F32 and PA_WAITALL (the direction is implied).  Any
+ * other bit (PA_STAGE_SELF included: there is no staged schedule) is PA_EINVAL.  src and dst must
+ * not overlap, NULL only when empty, aligned to the complex element.  Every refusal (PA_EINVAL; a
+ * `real` not related to the plan's input pencil: PA_EINCOMPAT) happens on the host before anything
+ * is enqueued, and a refused geometry is refused on every rank of the grid line; without a device
+ * PA_ENOGPU after those checks.                                                            */
+pa_status pa_fft_put(pa_plan* plan, pa_comm* comm, const void* src, void* dst, unsigned flags,
+                     void* stream);
+pa_status pa_rfft_put(pa_plan* plan, pa_comm* comm, const pa_pencil* real, const void* src, void* dst,
+                      unsigned flags, void* stream);
+/* The same kernels without the window protocol (the counterparts of pa_get_all_fft): the self
+ * block into `dst`, the block of peer n into `peers[n-1]` (its dst parent array, as mapped here;
+ * the self entry is ignored).  flags: pa_put_all_fft PA_FFT_FORWARD or PA_FFT_BACKWARD, optionally
+ * with PA_FFT_F32; pa_put_all_rfft 0 or PA_FFT_F32.  The plan must exchange data; checks as above. */
+pa_status pa_put_all_fft(pa_plan* plan, const void* src, void* const* peers, void* dst, unsigned flags,
+                         void* stream);
+pa_status pa_put_all_rfft(pa_plan* plan, const pa_pencil* real, const void* src, void* const* peers,
+                          void* dst, unsigned flags, void* stream);
+/* Can pa_fft_put (pa_rfft_put) run on this plan?  Element size, line length, at most 8 blocks per
+ * line that tile it and share every other dim, and PA_PEER_PUT when the plan exchanges data: the
+ * same answer on every rank of the grid line (each rank's plan is rebuilt).  Only PA_FFT_F32 of
+ * `flags` matters.  Cached per plan and precision, apart from every other verdict.  Host-only.  */
+pa_status pa_plan_fft_put_check(const pa_plan* plan, unsigned flags);
+pa_status pa_plan_rfft_put_check(const pa_plan* plan, unsigned flags);
+
 /* ---- host chains -----------------------------------------------------------
  * A sequence of transpositions applied to HOST arrays (plan i+1 consumes what
  * plan i produces): one submit = upload of `host_src`, every transpose! on the

@@ -1090,6 +1090,166 @@ pa_status pa_plan_real_check(const pa_plan* plan, unsigned flags) {
   })
 }
 
+// ---- send-side fused transform + put (pa_fft_put, pa_rfft_put, pa_put_all_fft / _rfft) ----------
+// The checks they share, all on the host: the plan's verdict, then (rfft) `real` against the plan's
+// INPUT pencil as pa_rfft relates them, then src / dst (NULL only when empty, not overlapping,
+// aligned to the complex element).
+static pa_status put_args(const char* who, Plan& P, const pa_pencil* real, const void* src,
+                          const void* dst, bool rfft, bool f32) {
+  pa_status s = rfft ? plan_rfft_put_check(&P, f32) : plan_fft_put_check(&P, f32);
+  if (s != PA_OK) return s;
+  const i64 es = P.elsize;
+  i64 src_bytes = P.length_in * es;
+  if (rfft) {
+    const pa_pencil in{P.pin};
+    int N = 0;
+    i64 nlines = 0;
+    s = rfft_checks(who, real, &in, P.n_extra, P.extra, PA_FFT_FORWARD | (f32 ? PA_FFT_F32 : 0u), nullptr,
+                    nullptr, false, &N, &nlines);
+    if (s != PA_OK) return s;
+    src_bytes = nlines * N * (es / 2);
+  }
+  const i64 dst_bytes = P.length_out * es;
+  if ((!src && src_bytes > 0) || (!dst && dst_bytes > 0)) {
+    set_error("%s: null array pointer for a non-empty local array", who);
+    return PA_EINVAL;
+  }
+  const uintptr_t a = (uintptr_t)src, b = (uintptr_t)dst;
+  if (src_bytes > 0 && dst_bytes > 0 && a < b + (uintptr_t)dst_bytes && b < a + (uintptr_t)src_bytes) {
+    set_error("%s: src and dst overlap (the send-side fusion has no staged schedule: transform in "
+              "place with %s, then transpose)", who, rfft ? "rfft_" : "fft_");
+    return PA_EINVAL;
+  }
+  if ((src_bytes > 0 && a % es) || (dst_bytes > 0 && b % es)) {
+    set_error("%s: src and dst must be aligned to the %lld-byte complex element", who, (long long)es);
+    return PA_EINVAL;
+  }
+  return PA_OK;
+}
+
+// flags: exactly one of PA_FFT_FORWARD / PA_FFT_BACKWARD (rfft: none, the direction is implied),
+// with any of `extra`
+static pa_status put_flags(const char* who, unsigned flags, bool rfft, unsigned extra) {
+  if (flags & PA_STAGE_SELF) {
+    set_error("%s: PA_STAGE_SELF does not apply: the send-side fusion stores the self block "
+              "straight into dst", who);
+    return PA_EINVAL;
+  }
+  const unsigned dir = flags & ~extra;
+  if (rfft ? dir != 0 : (dir != PA_FFT_FORWARD && dir != PA_FFT_BACKWARD)) {
+    if (rfft)
+      set_error("%s: flags may combine %s only (the direction is implied)", who,
+                (extra & PA_WAITALL) ? "PA_WAITALL and PA_FFT_F32" : "PA_FFT_F32");
+    else
+      set_error("%s: flags must be exactly PA_FFT_FORWARD or PA_FFT_BACKWARD, optionally with %s", who,
+                (extra & PA_WAITALL) ? "PA_FFT_F32 and PA_WAITALL" : "PA_FFT_F32");
+    return PA_EINVAL;
+  }
+  return PA_OK;
+}
+
+static pa_status fft_put(pa_plan* plan, pa_comm* comm, const pa_pencil* real, const void* src, void* dst,
+                         unsigned flags, void* stream, bool rfft) {
+  const char* who = rfft ? "pa_rfft_put" : "pa_fft_put";
+  if (!plan) {
+    set_error("%s: null plan", who);
+    return PA_EINVAL;
+  }
+  pa_status s = put_flags(who, flags, rfft, PA_FFT_F32 | PA_WAITALL);
+  if (s != PA_OK) return s;
+  Plan& P = *plan->p;
+  const bool f32 = (flags & PA_FFT_F32) != 0;
+  s = put_args(who, P, real, src, dst, rfft, f32);
+  if (s != PA_OK) return s;
+  s = need_gpu();
+  if (s != PA_OK) return s;
+  return transpose_put_fft(&P, comm ? comm->p : nullptr, src, dst, flags, rfft, stream);
+}
+
+pa_status pa_fft_put(pa_plan* plan, pa_comm* comm, const void* src, void* dst, unsigned flags,
+                     void* stream) {
+  GUARD({ return fft_put(plan, comm, nullptr, src, dst, flags, stream, false); })
+}
+
+pa_status pa_rfft_put(pa_plan* plan, pa_comm* comm, const pa_pencil* real, const void* src, void* dst,
+                      unsigned flags, void* stream) {
+  GUARD({ return fft_put(plan, comm, real, src, dst, flags, stream, true); })
+}
+
+// The send-side fused kernel without the window protocol: the self block into `dst`, the put
+// block of peer n into peers[n - 1] (its dst, as mapped here; the self entry is ignored).
+static pa_status put_all_fft(pa_plan* plan, const pa_pencil* real, const void* src, void* const* peers,
+                             void* dst, unsigned flags, void* stream, bool rfft) {
+  const char* who = rfft ? "pa_put_all_rfft" : "pa_put_all_fft";
+  if (!plan) {
+    set_error("%s: null plan", who);
+    return PA_EINVAL;
+  }
+  Plan& P = *plan->p;
+  if (P.dim < 0) {
+    set_error("%s: plan has no exchange", who);
+    return PA_EINVAL;
+  }
+  pa_status s = put_flags(who, flags, rfft, PA_FFT_F32);
+  if (s != PA_OK) return s;
+  const bool f32 = (flags & PA_FFT_F32) != 0;
+  s = put_args(who, P, real, src, dst, rfft, f32);
+  if (s != PA_OK) return s;
+  const i64 es = P.elsize;
+  std::vector<const BlockCopy*> blocks;
+  std::vector<void*> dsts;
+  for (int n = 0; n < P.nproc; ++n) {
+    const bool self = n == P.self_index;
+    const BlockCopy& b = self ? P.self_fused : P.peers[n].put;
+    void* d = self ? dst : (peers ? peers[n] : nullptr);
+    if (!self && b.count > 0 && !d) {
+      set_error("%s: null peer array for a non-empty block (peer %d)", who, n + 1);
+      return PA_EINVAL;
+    }
+    if (b.count > 0 && ((uintptr_t)d % es)) {
+      set_error("%s: arrays must be aligned to the %lld-byte element", who, (long long)es);
+      return PA_EINVAL;
+    }
+    blocks.push_back(&b);
+    dsts.push_back(d);
+  }
+  s = need_gpu();
+  if (s != PA_OK) return s;
+  bool launched = false;
+  return put_fft(P.nproc, blocks.data(), src, dsts.data(), (flags & PA_FFT_BACKWARD) ? 1 : -1, rfft, f32,
+                 nullptr, stream, &launched);
+}
+
+pa_status pa_put_all_fft(pa_plan* plan, const void* src, void* const* peers, void* dst, unsigned flags,
+                         void* stream) {
+  GUARD({ return put_all_fft(plan, nullptr, src, peers, dst, flags, stream, false); })
+}
+
+pa_status pa_put_all_rfft(pa_plan* plan, const pa_pencil* real, const void* src, void* const* peers,
+                          void* dst, unsigned flags, void* stream) {
+  GUARD({ return put_all_fft(plan, real, src, peers, dst, flags, stream, true); })
+}
+
+pa_status pa_plan_fft_put_check(const pa_plan* plan, unsigned flags) {
+  GUARD({
+    if (!plan) {
+      set_error("pa_plan_fft_put_check: null plan");
+      return PA_EINVAL;
+    }
+    return plan_fft_put_check(plan->p, (flags & PA_FFT_F32) != 0);
+  })
+}
+
+pa_status pa_plan_rfft_put_check(const pa_plan* plan, unsigned flags) {
+  GUARD({
+    if (!plan) {
+      set_error("pa_plan_rfft_put_check: null plan");
+      return PA_EINVAL;
+    }
+    return plan_rfft_put_check(plan->p, (flags & PA_FFT_F32) != 0);
+  })
+}
+
 pa_status pa_host_chain_create(int n, pa_plan* const* plans, pa_comm* comm, pa_host_chain** out) {
   GUARD({
     if (n < 1 || n > 64 || !plans || !out) {

@@ -252,34 +252,40 @@ __device__ __forceinline__ long long cta_offsets(const FftParams& p, int C, long
   return x0;
 }
 
-// One CTA of the fused unpack + FFT: gather its C lines from every block, transform, store.
+// The first pass of a CTA of C lines that runs in registers on the gathered values: radix
+// 2^LOGR1 (0: none).  A thread owns the rows r, r + RS, r + 2 RS, ... of its line: exactly the
+// inputs of one butterfly of a first pass of radix R1 = L / RS.  (Only for 1024-point lines,
+// where shared memory bounds the CTAs per SM; for 512-point lines the radix-16 butterfly's
+// registers would cost the third resident CTA.  Single precision holds 8 1024-point lines: a
+// sweep of 32 rows would need a radix-32 pass, which does not exist, so every pass runs in
+// shared memory there)
 template <int LOGL, int C, class T>
-__device__ __forceinline__ void unpack_fft_cta(const FftParams& p) {
+struct FftCtaShape {
+  static constexpr int RS = FFT_THREADS / C;  // rows per sweep
+  static constexpr int LOGRS = (C == 16) ? 4 : (C == 8) ? 5 : 6;
+  static_assert((1 << LOGRS) == RS, "rows per sweep");
+  static constexpr int LOGR1 = (sizeof(T) == 8 && C == 4 && LOGL > LOGRS) ? (LOGL - LOGRS) : 0;
+  static_assert(LOGR1 == 0 || LOGL - LOGR1 == LOGRS, "first-pass stride must equal the sweep");
+  static_assert(LOGR1 <= 4, "the register first pass is at most radix 16");
+};
+
+// The load and the passes of one CTA of the complex FFT (k_unpack_fft, k_get_fft, k_fft_put): the
+// C lines gathered from every block of p into shared memory (+ the register first pass), then the
+// remaining passes.  Output frequency k of line c is then at fft_out_pos<LOGL, LOGR1>(k).
+template <int LOGL, int C, class T>
+__device__ __forceinline__ void fft_cta_lines(const FftParams& p, const long long* so_off, long long x0,
+                                              int ncol, cplx_t<T>* sm) {
   using cx = cplx_t<T>;
   using V = typename Vec2<T>::type;
   constexpr int L = 1 << LOGL;
-  extern __shared__ __align__(16) unsigned char fft_smem[];
-  cx* sm = reinterpret_cast<cx*>(fft_smem);
   const int t = threadIdx.x;
-  long long so_off[FFT_MAXB], d_off;
-  const long long x0 = cta_offsets(p, C, so_off, &d_off);
-  const int ncol = (int)((p.ex - x0) < C ? (p.ex - x0) : C);
   const int pitch = p.pitch;
 
   // ---- gather (+ first pass): C threads read C consecutive columns (C x sizeof(cx)) of one
-  //      source row.  A thread owns the rows r, r + RS, r + 2 RS, ... of its column: exactly
-  //      the inputs of one butterfly of a first pass of radix R1 = L / RS -- so that pass runs
-  //      on the values as they arrive from HBM, before they ever touch shared memory ----
-  constexpr int RS = FFT_THREADS / C;  // rows per sweep
-  constexpr int LOGRS = (C == 16) ? 4 : (C == 8) ? 5 : 6;
-  static_assert((1 << LOGRS) == RS, "rows per sweep");
-  // (only for 1024-point lines, where shared memory bounds the CTAs per SM; for 512-point
-  //  lines the radix-16 butterfly's registers would cost the third resident CTA.  Single
-  //  precision holds 8 1024-point lines: a sweep of 32 rows would need a radix-32 pass, which
-  //  does not exist, so every pass runs in shared memory there)
-  constexpr int LOGR1 = (sizeof(T) == 8 && C == 4 && LOGL > LOGRS) ? (LOGL - LOGRS) : 0;
-  static_assert(LOGR1 == 0 || LOGL - LOGR1 == LOGRS, "first-pass stride must equal the sweep");
-  static_assert(LOGR1 <= 4, "the register first pass is at most radix 16");
+  //      source row; the first pass (FftCtaShape) runs on the values as they arrive from HBM,
+  //      before they ever touch shared memory ----
+  constexpr int RS = FftCtaShape<LOGL, C, T>::RS;
+  constexpr int LOGR1 = FftCtaShape<LOGL, C, T>::LOGR1;
   const V* twp = reinterpret_cast<const V*>(p.tw);
   auto tw = [twp](int i) {
     const V w = __ldg(twp + i);
@@ -320,6 +326,31 @@ __device__ __forceinline__ void unpack_fft_cta(const FftParams& p) {
 
   // ---- remaining passes in shared memory (radices and strides are compile-time constants) ----
   fft_passes<LOGL, LOGL - LOGR1, C>(sm, pitch, ncol, p.sign, tw);
+}
+
+// storage position of output frequency k after fft_cta_lines: first-pass digit, then the digits
+// of the later passes
+template <int LOGL, int LOGR1>
+__device__ __forceinline__ int fft_out_pos(int k) {
+  return ((k & ((1 << LOGR1) - 1)) << (LOGL - LOGR1)) + fft_pos<LOGL, LOGL - LOGR1>(k >> LOGR1);
+}
+
+// One CTA of the fused unpack + FFT: gather its C lines from every block, transform, store.
+template <int LOGL, int C, class T>
+__device__ __forceinline__ void unpack_fft_cta(const FftParams& p) {
+  using cx = cplx_t<T>;
+  using V = typename Vec2<T>::type;
+  constexpr int L = 1 << LOGL;
+  extern __shared__ __align__(16) unsigned char fft_smem[];
+  cx* sm = reinterpret_cast<cx*>(fft_smem);
+  const int t = threadIdx.x;
+  long long so_off[FFT_MAXB], d_off;
+  const long long x0 = cta_offsets(p, C, so_off, &d_off);
+  const int ncol = (int)((p.ex - x0) < C ? (p.ex - x0) : C);
+  const int pitch = p.pitch;
+  constexpr int LOGR1 = FftCtaShape<LOGL, C, T>::LOGR1;
+
+  fft_cta_lines<LOGL, C, T>(p, so_off, x0, ncol, sm);
 
   // ---- store: natural order, every line one contiguous run ----
   char* d = p.dst + x0 * p.dsx + d_off;
@@ -442,6 +473,31 @@ __device__ __forceinline__ void rfft_forward_tail(cplx_t<T>* sm, int pitch, int 
   }
 }
 
+// The load of k_rfft (k_rfft_put loads its lines with it too), linear: consecutive threads walk
+// along a line, one element per load, the RS threads of line c reading it from src(c).
+// Forward: the N reals ARE the complex line z[n] = x[2n] + i x[2n+1]; backward: N/2+1 bins.
+template <int LOGL, int C, bool FWD, class T, class Src>
+__device__ __forceinline__ void rfft_load(cplx_t<T>* sm, int pitch, int ncol, int t, const Src& src) {
+  using cx = cplx_t<T>;
+  using V = typename Vec2<T>::type;
+  constexpr int L = 1 << LOGL;
+  constexpr int RS = FFT_THREADS / C;
+  constexpr int NIN = FWD ? L : L + 1;
+  constexpr int U = (NIN + RS - 1) / RS;
+  const int c = t / RS, r = t % RS;
+  if (c < ncol) {
+    const V* s = src(c);
+    cx* line = sm + c * pitch;
+    V v[U];
+#pragma unroll
+    for (int q = 0; q < U; ++q)
+      if (r + q * RS < NIN) v[q] = __ldcs(s + r + q * RS);
+#pragma unroll
+    for (int q = 0; q < U; ++q)
+      if (r + q * RS < NIN) line[pa_fft::pad_index(r + q * RS)] = cx{v[q].x, v[q].y};
+  }
+}
+
 // Single precision: complex lines are 8 (N/2 + 1) bytes, an odd multiple of 8, so every other
 // line starts only 8-byte aligned; every access is one 8-byte element (float2) on both sides.
 template <int LOGL, int C, bool FWD, class T>
@@ -449,8 +505,7 @@ __global__ void __launch_bounds__(FFT_THREADS) k_rfft(const __grid_constant__ Rf
   using cx = cplx_t<T>;
   using V = typename Vec2<T>::type;
   constexpr int L = 1 << LOGL;
-  constexpr int RS = FFT_THREADS / C;  // threads per line
-  constexpr int P = L / 2 + 1;         // pairs (k, L - k) per line
+  constexpr int P = L / 2 + 1;  // pairs (k, L - k) per line
   extern __shared__ __align__(16) unsigned char fft_smem[];
   cx* sm = reinterpret_cast<cx*>(fft_smem);
   const int t = threadIdx.x;
@@ -467,24 +522,10 @@ __global__ void __launch_bounds__(FFT_THREADS) k_rfft(const __grid_constant__ Rf
     return cx{w.x, w.y};
   };
 
-  // ---- load (linear gather): consecutive threads walk along a line, one element per load.
-  //      Forward: the N reals ARE the complex line z[n] = x[2n] + i x[2n+1]; backward: N/2+1 bins ----
-  {
-    constexpr int NIN = FWD ? L : L + 1;
-    constexpr int U = (NIN + RS - 1) / RS;
-    const int c = t / RS, r = t % RS;
-    if (c < ncol) {
-      const V* s = reinterpret_cast<const V*>(p.src + (l0 + c) * p.src_line);
-      cx* line = sm + c * pitch;
-      V v[U];
-#pragma unroll
-      for (int q = 0; q < U; ++q)
-        if (r + q * RS < NIN) v[q] = __ldcs(s + r + q * RS);
-#pragma unroll
-      for (int q = 0; q < U; ++q)
-        if (r + q * RS < NIN) line[pa_fft::pad_index(r + q * RS)] = cx{v[q].x, v[q].y};
-    }
-  }
+  // ---- load (linear gather): consecutive threads walk along a line, one element per load ----
+  rfft_load<LOGL, C, FWD, T>(sm, pitch, ncol, t, [&p, l0](int c) {
+    return reinterpret_cast<const V*>(p.src + (l0 + c) * p.src_line);
+  });
   __syncthreads();
 
   if constexpr (FWD) {
@@ -804,6 +845,185 @@ __global__ void __launch_bounds__(FFT_THREADS) k_unpack_rfft(const __grid_consta
   char* d = p.dst + x0 * p.dsx + d_off;
   rfft_forward_tail<LOGL, C, T>(sm, pitch, ncol, t, reinterpret_cast<const V*>(p.tw),
                                 [&p, d](int c) { return d + c * p.dsx; });
+}
+
+// ---- send-side fused transform + put (pa_fft_put / pa_rfft_put, DESIGN §3i) ----
+// The mirror of k_get_fft: the dim a PencilFFTs leg transforms first is the first memory dim of
+// its src, local and contiguous.  A CTA loads C whole source lines with the linear load of fft_
+// (k_rfft's for r2c), runs the same passes in shared memory, and stores every output bin straight
+// into the block that owns it: the self block into the local dst, every other block into its
+// peer's dst through the peer mapping.  So dst = transpose(fft_(src)) (transpose(rfft_(src))) byte
+// for byte, with one read of src and one write of dst.
+//   Window protocol (k_multi's, with the put flavour's wait for the peers' DONE): the first CTAs
+// signal READY at the start, every CTA waits for READY from every peer only after its transform,
+// before its first store -- the load and the passes never touch peer memory, so the wait hides
+// behind them -- and the CTA that finishes last signals DONE and waits for the peers' DONE (only
+// then has every peer's store into my dst landed).  Empty flag sets: the plain kernel
+// (pa_put_all_fft / pa_put_all_rfft, or a launch that standalone flag kernels bracket).
+struct FftPutBlock {
+  char* dst;        // the block's origin in its destination array (dst, or a peer's as mapped here)
+  int y0, ey;       // the bins [y0, y0 + ey) of every line that this block receives
+  long long dsy;    // destination byte stride of a bin step
+  long long dsx;    // destination byte stride of a column step (consecutive lines of a CTA)
+  long long dso[FFT_MAXO];
+};
+struct FftPutParams {
+  FftParams p;  // the load: ONE linear block, the whole source lines (p.dst / p.dsx / p.dso unused)
+  int nb;
+  int across;   // the columns have destination stride 1: C consecutive threads store one bin of
+                // C consecutive lines (128 bytes); else consecutive threads walk along a line
+  FftPutBlock blk[FFT_MAXB];
+  MultiFlags mf;
+};
+static_assert(sizeof(FftPutParams) <= 4096, "FftPutParams must fit the kernel parameters");
+
+__device__ __forceinline__ void put_ready_signal(const MultiFlags& mf) {
+  if (mf.ready.n > 0 && blockIdx.x < 8 && (int)threadIdx.x < mf.ready.n)
+    flag_signal(mf.ready.remote[threadIdx.x], mf.ready.seq[threadIdx.x]);
+}
+__device__ __forceinline__ void put_ready_wait(const MultiFlags& mf) {
+  if (mf.ready.n > 0) {
+    if ((int)threadIdx.x < mf.ready.n)
+      flag_wait(mf.ready.local[threadIdx.x], mf.ready.seq[threadIdx.x], mf.timeout_ns, mf.err);
+    __syncthreads();
+  }
+}
+__device__ __forceinline__ void put_done(const MultiFlags& mf) {
+  if (mf.done.n > 0) {
+    // every store of this CTA has been issued; the last CTA to get here closes the window.  (No
+    // static shared memory, as in k_get_fft)
+    __syncthreads();
+    int last = 0;
+    if (threadIdx.x == 0) {
+      __threadfence_system();
+      last = atomicAdd(mf.counter, 1u) == gridDim.x - 1;
+      if (last) {
+        *mf.counter = 0;  // ready for the next launch (stream-ordered after this one)
+        __threadfence_system();
+      }
+    }
+    if (__syncthreads_or(last) && (int)threadIdx.x < mf.done.n) {
+      flag_signal(mf.done.remote[threadIdx.x], mf.done.seq[threadIdx.x]);
+      if (mf.wait_done) flag_wait(mf.done.local[threadIdx.x], mf.done.seq[threadIdx.x], mf.timeout_ns, mf.err);
+    }
+  }
+}
+
+// The destination of bin k of the CTA's lines: the block that owns it, at its CTA origin `base`
+// (every block is tried with a compile-time index, so `base` stays in registers)
+template <class T>
+__device__ __forceinline__ typename Vec2<T>::type* put_target(const FftPutParams& pp, char* const* base,
+                                                              int c, int k) {
+  char* o = nullptr;
+#pragma unroll
+  for (int b = 0; b < FFT_MAXB; ++b)
+    if (b < pp.nb && k >= pp.blk[b].y0 && k < pp.blk[b].y0 + pp.blk[b].ey)
+      o = base[b] + (long long)(k - pp.blk[b].y0) * pp.blk[b].dsy + c * pp.blk[b].dsx;
+  return reinterpret_cast<typename Vec2<T>::type*>(o);
+}
+
+// Every block's origin for this CTA's first line: its outer offsets (from the CTA index, as
+// cta_offsets) and the first column x0
+__device__ __forceinline__ void put_bases(const FftPutParams& pp, long long x0, char** base) {
+  long long off[FFT_MAXB];
+#pragma unroll
+  for (int b = 0; b < FFT_MAXB; ++b) off[b] = 0;
+  unsigned long long bid = blockIdx.x / pp.p.tiles_x;
+#pragma unroll 1
+  for (int i = 0; i < pp.p.no; ++i) {
+    const long long k = (long long)(bid % (unsigned long long)pp.p.oe[i]);
+    bid /= (unsigned long long)pp.p.oe[i];
+#pragma unroll
+    for (int b = 0; b < FFT_MAXB; ++b)
+      if (b < pp.nb) off[b] += k * pp.blk[b].dso[i];
+  }
+#pragma unroll
+  for (int b = 0; b < FFT_MAXB; ++b) base[b] = pp.blk[b].dst + off[b] + x0 * pp.blk[b].dsx;
+}
+
+// (a register cap as k_get_fft's)
+template <int LOGL, int C, class T>
+__global__ void __maxnreg__(128) k_fft_put(const __grid_constant__ FftPutParams pp) {
+  using cx = cplx_t<T>;
+  constexpr int L = 1 << LOGL;
+  constexpr int LOGR1 = FftCtaShape<LOGL, C, T>::LOGR1;
+  extern __shared__ __align__(16) unsigned char fft_smem[];
+  cx* sm = reinterpret_cast<cx*>(fft_smem);
+  const FftParams& p = pp.p;
+  const int t = threadIdx.x;
+  put_ready_signal(pp.mf);
+  long long so_off[FFT_MAXB], d_off;
+  const long long x0 = cta_offsets(p, C, so_off, &d_off);
+  const int ncol = (int)((p.ex - x0) < C ? (p.ex - x0) : C);
+  fft_cta_lines<LOGL, C, T>(p, so_off, x0, ncol, sm);
+  put_ready_wait(pp.mf);
+
+  // ---- store: bin k of line c into the block that owns k ----
+  char* base[FFT_MAXB];
+  put_bases(pp, x0, base);
+  const bool across = pp.across != 0;
+  for (int w0 = 0; w0 < C * L; w0 += FFT_THREADS) {
+    const int w = w0 + t;
+    const int c = across ? (w & (C - 1)) : (w >> LOGL), k = across ? (w / C) : (w & (L - 1));
+    if (w < C * L && c < ncol) {
+      const cx v = sm[c * p.pitch + pa_fft::pad_index(fft_out_pos<LOGL, LOGR1>(k))];
+      __stcs(put_target<T>(pp, base, c, k), vec2(v.x, v.y));
+    }
+  }
+  put_done(pp.mf);
+}
+
+// r2c: k_rfft's load (forward) and its passes, then rfft_post_pair on the pairs (k, L - k), the
+// N/2 + 1 = L + 1 bins of a line stored into the blocks that own them.  p.L = N / 2, p.tw = W_N.
+template <int LOGL, int C, class T>
+__global__ void __maxnreg__(128) k_rfft_put(const __grid_constant__ FftPutParams pp) {
+  using cx = cplx_t<T>;
+  using V = typename Vec2<T>::type;
+  constexpr int L = 1 << LOGL;
+  constexpr int P = L / 2 + 1;  // pairs (k, L - k) per line
+  extern __shared__ __align__(16) unsigned char fft_smem[];
+  cx* sm = reinterpret_cast<cx*>(fft_smem);
+  const FftParams& p = pp.p;
+  const int t = threadIdx.x;
+  put_ready_signal(pp.mf);
+  long long so_off[FFT_MAXB], d_off;
+  const long long x0 = cta_offsets(p, C, so_off, &d_off);
+  const int ncol = (int)((p.ex - x0) < C ? (p.ex - x0) : C);
+  const int pitch = p.pitch;
+  rfft_load<LOGL, C, true, T>(sm, pitch, ncol, t, [&p, &so_off, x0](int c) {
+    return reinterpret_cast<const V*>(p.blk[0].src + so_off[0] + (x0 + c) * p.blk[0].ssx);
+  });
+  __syncthreads();
+  const V* twp = reinterpret_cast<const V*>(p.tw);
+  auto twN = [twp](int k) {
+    const V w = __ldg(twp + k);
+    return cx{w.x, w.y};
+  };
+  auto twL = [twp](int i) {  // W_L^i = W_N^(2i)
+    const V w = __ldg(twp + 2 * i);
+    return cx{w.x, w.y};
+  };
+  fft_passes<LOGL, LOGL, C>(sm, pitch, ncol, -1, twL);
+  put_ready_wait(pp.mf);
+
+  // ---- post-pass + store: the pair k yields bins k and L - k ----
+  char* base[FFT_MAXB];
+  put_bases(pp, x0, base);
+  const bool across = pp.across != 0;
+  for (int w0 = 0; w0 < C * P; w0 += FFT_THREADS) {
+    const int w = w0 + t;
+    const int c = across ? (w & (C - 1)) : (w / P), k = across ? (w / C) : (w % P);
+    if (w < C * P && c < ncol) {
+      const cx* line = sm + c * pitch;
+      cx xk, xl;
+      pa_fft::rfft_post_pair(line[pa_fft::pad_index(fft_pos<LOGL, LOGL>(k & (L - 1)))],
+                             line[pa_fft::pad_index(fft_pos<LOGL, LOGL>((L - k) & (L - 1)))], twN(k),
+                             &xk, &xl);
+      __stcs(put_target<T>(pp, base, c, k), vec2(xk.x, xk.y));
+      if (k != L - k) __stcs(put_target<T>(pp, base, c, L - k), vec2(xl.x, xl.y));
+    }
+  }
+  put_done(pp.mf);
 }
 
 // forward twiddle table W_L^k per (device, L, precision), computed once in extended precision
@@ -1196,6 +1416,238 @@ pa_status get_fft(int nb, const BlockCopy* const* blocks, const void* const* src
   return PA_OK;
 }
 
+// Launch geometry of k_fft_put / k_rfft_put from the blocks of one rank -- the mirror of
+// fft_geometry on the source side.  `blocks[i]` moves a box of the local `src` into `dsts[i]`
+// (the local dst for the self block, a peer's dst as mapped here otherwise); together they must
+// tile the source lines.  The line dim is the source dim of stride 1 (raw dim 0); the blocks
+// must tile [0, M) along it (M = L points; rfft: M = N/2 + 1 bins) and share every other dim,
+// whose destination strides may differ (the peers' arrays have their own layouts).  The column
+// dim is the destination's stride-1 dim when that is not the line dim.  src / dsts may be NULL:
+// plan_fft_put_check runs this without arrays.  *grid = 0: this rank has no source lines.
+// rfft: the plan is the COMPLEX plan of M bins per line, and `src` the REAL array of N reals per
+// line that replaces its source (same layout otherwise): the source offsets and strides, multiples
+// of M, are rescaled to N reals -- brfft's destination rescale, mirrored.
+static pa_status put_fft_geometry(int nb, const BlockCopy* const* blocks, const void* src,
+                                  void* const* dsts, bool f32, bool rfft, FftPutParams& pp, int* C_out,
+                                  unsigned long long* grid_out) {
+  const char* what = rfft ? "fused rfft + put" : "fused FFT + put";
+  const i64 es = f32 ? 8 : 16;  // complex element bytes (the plan's elements)
+  memset(&pp, 0, sizeof pp);
+  *grid_out = 0;
+  const BlockCopy* ref = nullptr;
+  i64 min_soff = -1;
+  for (int b = 0; b < nb; ++b) {
+    const BlockCopy& B = *blocks[b];
+    if (B.count == 0) continue;
+    if (B.elsize != es) {
+      set_error(f32 ? "%s: PA_FFT_F32 takes ComplexF32 (8-byte) elements only"
+                    : "%s: ComplexF64 (16-byte) elements only", what);
+      return PA_EINVAL;
+    }
+    if (B.raw[0].ss != 1) {
+      set_error("%s: unexpected source layout", what);
+      return PA_EINVAL;
+    }
+    if (!ref) ref = &B;
+    if (B.nd_raw != ref->nd_raw) {
+      set_error("%s: the blocks do not share their line set", what);
+      return PA_EINVAL;
+    }
+    for (int i = 1; i < B.nd_raw; ++i)
+      if (B.raw[i].e != ref->raw[i].e || B.raw[i].ss != ref->raw[i].ss) {
+        set_error("%s: the blocks do not share their line set", what);
+        return PA_EINVAL;
+      }
+    if (min_soff < 0 || B.src_off < min_soff) min_soff = B.src_off;
+  }
+  if (!ref) return PA_OK;  // no source lines on this rank (*grid = 0)
+  i64 M = 0;
+  for (int b = 0; b < nb; ++b) {
+    const BlockCopy& B = *blocks[b];
+    if (B.count == 0) continue;
+    if (pp.nb >= FFT_MAXB) {
+      set_error("%s: more than %d blocks", what, FFT_MAXB);
+      return PA_EINVAL;
+    }
+    FftPutBlock& F = pp.blk[pp.nb++];
+    F.dst = dsts && dsts[b] ? (char*)dsts[b] + B.dst_off * es : nullptr;
+    F.y0 = (int)(B.src_off - min_soff);
+    F.ey = (int)B.raw[0].e;
+    F.dsy = B.raw[0].ds * es;
+    M += B.raw[0].e;
+  }
+  const i64 L = rfft ? M - 1 : M;  // rfft: the N/2-point complex FFT of a real line of N = 2 (M - 1)
+  int logL = 0;
+  while ((1LL << logL) < L) ++logL;
+  if ((1LL << logL) != L || L < 8 || L > 1024) {
+    if (rfft)
+      set_error("%s: %lld bins per line are not N/2+1 with N a power of two in 16..2048", what,
+                (long long)M);
+    else
+      set_error("%s: line length %lld is not a power of two in 8..1024", what, (long long)L);
+    return PA_EINVAL;
+  }
+  {
+    std::vector<std::pair<int, int>> seg;
+    for (int b = 0; b < pp.nb; ++b) seg.push_back({pp.blk[b].y0, pp.blk[b].ey});
+    std::sort(seg.begin(), seg.end());
+    int pos = 0;
+    for (auto& s : seg) {
+      if (s.first != pos) {
+        set_error("%s: the blocks do not tile the transform axis", what);
+        return PA_EINVAL;
+      }
+      pos += s.second;
+    }
+  }
+  // the column dim: the destination's stride-1 dim (in every block) when the line dim is not it;
+  // otherwise (or when no such dim is longer than 1) the next dim longer than 1
+  int jx = -1;
+  bool across = false;
+  if (ref->raw[0].ds != 1)
+    for (int i = 1; i < ref->nd_raw && jx < 0; ++i) {
+      if (ref->raw[i].e <= 1) continue;
+      bool unit = true;
+      for (int b = 0; b < nb; ++b)
+        if (blocks[b]->count > 0) unit = unit && blocks[b]->raw[i].ds == 1;
+      if (unit) jx = i, across = true;
+    }
+  for (int i = 1; i < ref->nd_raw && jx < 0; ++i)
+    if (ref->raw[i].e > 1) jx = i;
+  // source offsets and strides: complex elements, or (rfft) multiples of M bins that become
+  // multiples of N reals
+  const i64 N = 2 * L, rs = es / 2;
+  auto src_bytes = [&](long long off, long long* out) {
+    if (!rfft) {
+      *out = off * es;
+      return true;
+    }
+    if (off % M != 0) {
+      set_error("%s: a source stride or offset is not a multiple of the %lld bins of a line", what,
+                (long long)M);
+      return false;
+    }
+    *out = off / M * N * rs;
+    return true;
+  };
+  FftParams& p = pp.p;
+  FftBlock& S = p.blk[0];
+  p.nb = 1;
+  long long v = 0;
+  if (!src_bytes(min_soff, &v)) return PA_EINVAL;
+  S.src = src ? (const char*)src + v : nullptr;
+  S.y0 = 0;
+  S.ey = (int)L;
+  S.ssy = rfft ? 2 * rs : es;
+  S.ssx = rfft ? N * rs : L * es;
+  if (jx >= 0 && !src_bytes(ref->raw[jx].ss, &S.ssx)) return PA_EINVAL;
+  for (int i = 1; i < ref->nd_raw; ++i)
+    if (i != jx && ref->raw[i].e > 1) {
+      if (p.no >= FFT_MAXO) {
+        set_error("%s: more than %d outer dims", what, FFT_MAXO);
+        return PA_EINVAL;
+      }
+      if (!src_bytes(ref->raw[i].ss, &S.so[p.no])) return PA_EINVAL;
+      p.oe[p.no] = ref->raw[i].e;
+      int o = 0;
+      for (int b = 0; b < nb; ++b)
+        if (blocks[b]->count > 0) pp.blk[o++].dso[p.no] = blocks[b]->raw[i].ds * es;
+      ++p.no;
+    }
+  {
+    int o = 0;
+    for (int b = 0; b < nb; ++b)
+      if (blocks[b]->count > 0) pp.blk[o++].dsx = jx >= 0 ? blocks[b]->raw[jx].ds * es : 0;
+  }
+  pp.across = across ? 1 : 0;
+  p.linear = 1;
+  p.ex = jx >= 0 ? ref->raw[jx].e : 1;
+  p.L = (int)L;
+  p.logL = logL;
+  p.pitch = pa_fft::padded_pitch((int)L);  // fft_ / k_rfft (forward): L points per shared line
+  // the lines per CTA of fft_ (tunable fft_lines included) / of k_rfft
+  const int C = f32 ? fft_lines_f32(logL)
+                    : ((!rfft && g_tun.fft_lines == 4 && logL >= 8) ? 4 : fft_lines(logL));
+  p.tiles_x = (unsigned)((p.ex + C - 1) / C);
+  unsigned long long grid = p.tiles_x;
+  for (int i = 0; i < p.no; ++i) grid *= (unsigned long long)p.oe[i];
+  if (grid > 0x7fffffffULL) {
+    set_error("%s: too many lines for one launch", what);
+    return PA_EINVAL;
+  }
+  *C_out = C;
+  *grid_out = grid;
+  return PA_OK;
+}
+
+pa_status put_fft(int nb, const BlockCopy* const* blocks, const void* src, void* const* dsts, int sign,
+                  bool rfft, bool f32, const MultiFlags* mf, void* stream, bool* launched) {
+  // (the entry points have already asked plan_fft_put_check / plan_rfft_put_check)
+  *launched = false;
+  FftPutParams pp;
+  int C = 0;
+  unsigned long long grid = 0;
+  pa_status s = put_fft_geometry(nb, blocks, src, dsts, f32, rfft, pp, &C, &grid);
+  if (s != PA_OK || grid == 0) return s;
+  if (mf) pp.mf = *mf;
+  FftParams& p = pp.p;
+  const int logL = p.logL;
+  p.sign = rfft ? -1 : (sign < 0 ? -1 : 1);
+  p.tw = twiddles(rfft ? 2 * p.L : p.L, f32);
+  if (!p.tw) {
+    set_error("fused put: twiddle table allocation failed");
+    cudaGetLastError();
+    return PA_ENOMEM;
+  }
+  const size_t smem = (f32 ? sizeof(pa_fft::cplxf) : sizeof(cplx)) * (size_t)C * p.pitch;
+  cudaError_t e = cudaSuccess;
+  auto launch = [&](auto kern) {
+    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout,
+                         cudaSharedmemCarveoutMaxShared);
+    cudaGetLastError();
+    kern<<<(unsigned)grid, FFT_THREADS, smem, (cudaStream_t)stream>>>(pp);
+    e = cudaGetLastError();
+  };
+  auto launch_mode = [&](auto fft_kern, auto rfft_kern) { rfft ? launch(rfft_kern) : launch(fft_kern); };
+  if (f32) {
+    switch (logL) {
+      case 3: launch_mode(k_fft_put<3, 16, float>, k_rfft_put<3, 16, float>); break;
+      case 4: launch_mode(k_fft_put<4, 16, float>, k_rfft_put<4, 16, float>); break;
+      case 5: launch_mode(k_fft_put<5, 16, float>, k_rfft_put<5, 16, float>); break;
+      case 6: launch_mode(k_fft_put<6, 16, float>, k_rfft_put<6, 16, float>); break;
+      case 7: launch_mode(k_fft_put<7, 16, float>, k_rfft_put<7, 16, float>); break;
+      case 8: launch_mode(k_fft_put<8, 16, float>, k_rfft_put<8, 16, float>); break;
+      case 9: launch_mode(k_fft_put<9, 16, float>, k_rfft_put<9, 16, float>); break;
+      default: launch_mode(k_fft_put<10, 8, float>, k_rfft_put<10, 8, float>); break;
+    }
+  } else {
+    switch (logL) {
+      case 3: launch_mode(k_fft_put<3, 8, double>, k_rfft_put<3, 8, double>); break;
+      case 4: launch_mode(k_fft_put<4, 8, double>, k_rfft_put<4, 8, double>); break;
+      case 5: launch_mode(k_fft_put<5, 8, double>, k_rfft_put<5, 8, double>); break;
+      case 6: launch_mode(k_fft_put<6, 8, double>, k_rfft_put<6, 8, double>); break;
+      case 7: launch_mode(k_fft_put<7, 8, double>, k_rfft_put<7, 8, double>); break;
+      case 8:
+        if (C == 4) launch(k_fft_put<8, 4, double>);
+        else launch_mode(k_fft_put<8, 8, double>, k_rfft_put<8, 8, double>);
+        break;
+      case 9:
+        if (C == 4) launch(k_fft_put<9, 4, double>);
+        else launch_mode(k_fft_put<9, 8, double>, k_rfft_put<9, 8, double>);
+        break;
+      default: launch_mode(k_fft_put<10, 4, double>, k_rfft_put<10, 4, double>); break;
+    }
+  }
+  if (e != cudaSuccess) {
+    set_error("fused put kernel launch failed: %s", cudaGetErrorString(e));
+    return PA_ECUDA;
+  }
+  count_launch();
+  *launched = true;
+  return PA_OK;
+}
+
 pa_status unpack_brfft(int nb, const BlockCopy* const* blocks, const void* const* srcs, void* dst,
                        bool f32, void* stream) {
   // (pa_transpose_brfft has already asked plan_brfft_check for every rank of the line)
@@ -1380,6 +1832,26 @@ pa_status unpack_rfft(int nb, const BlockCopy* const* blocks, const void* const*
 // with the self block read from src and staged through recv_buf alike.  A PeerGet plan may also
 // run the complex FFT one-sided (k_get_fft): its blocks are then the peers' get blocks, read from
 // their src arrays, and the self block from src, so that configuration is checked as well.
+// The plan rank n of P's grid line holds: P itself for this rank, else rebuilt from the pencils
+// with that rank's coordinates (owned by `hold`).
+static pa_status line_plan(Plan* P, int n, std::unique_ptr<Plan>& hold, const Plan** Q) {
+  *Q = P;
+  if (n == P->self_index) return PA_OK;
+  auto topo = std::make_shared<Topology>(*P->pin->topo);
+  topo->coords[P->dim] = n;
+  topo->rank = topo->rank_of(topo->coords);
+  auto pin = std::make_shared<Pencil>(*P->pin);
+  auto pout = std::make_shared<Pencil>(*P->pout);
+  pin->topo = topo;
+  pout->topo = topo;
+  Plan* q = nullptr;
+  pa_status s = build_plan(pin, pout, P->n_extra, P->extra, P->elsize, P->method, &q);
+  if (s != PA_OK) return s;
+  hold.reset(q);
+  *Q = q;
+  return PA_OK;
+}
+
 static pa_status fused_check(Plan* P, bool f32, FusedMode mode) {
   if (mode == FusedMode::r2r || mode == FusedMode::rfft) {
     if (P->elsize != (f32 ? 4 : 8)) {
@@ -1403,20 +1875,10 @@ static pa_status fused_check(Plan* P, bool f32, FusedMode mode) {
   }
   for (int n = 0; n < P->nproc; ++n) {
     std::unique_ptr<Plan> hold;
-    const Plan* Q = P;
-    if (n != P->self_index) {
-      auto topo = std::make_shared<Topology>(*P->pin->topo);
-      topo->coords[P->dim] = n;
-      topo->rank = topo->rank_of(topo->coords);
-      auto pin = std::make_shared<Pencil>(*P->pin);
-      auto pout = std::make_shared<Pencil>(*P->pout);
-      pin->topo = topo;
-      pout->topo = topo;
-      Plan* q = nullptr;
-      pa_status s = build_plan(pin, pout, P->n_extra, P->extra, P->elsize, P->method, &q);
+    const Plan* Q = nullptr;
+    {
+      pa_status s = line_plan(P, n, hold, &Q);
       if (s != PA_OK) return s;
-      hold.reset(q);
-      Q = q;
     }
     // 0: self block from src, 1: self block staged through recv_buf, 2: one-sided get
     const int configs = (mode == FusedMode::fft && P->method == PA_PEER_GET) ? 3 : 2;
@@ -1493,6 +1955,84 @@ pa_status plan_real_check(Plan* P, bool f32) {
     set_error("%s", P->real_check_err[q].c_str());
   }
   return P->real_check[q];
+}
+
+// Can pa_fft_put (rfft: pa_rfft_put) run on this plan?  The send-side kernel runs on PeerPut plans
+// and on local transposes (no exchange, or a line of one rank) of any method.  As fused_check,
+// every rank of the grid line gets the same answer: its plan is rebuilt and its blocks -- the
+// self block and the put blocks -- checked.
+static pa_status put_check(Plan* P, bool f32, bool rfft) {
+  const char* what = rfft ? "fused rfft + put" : "fused FFT + put";
+  if (P->elsize != (f32 ? 8 : 16)) {
+    set_error(f32 ? "%s: PA_FFT_F32 takes a ComplexF32 (elsize 8) plan"
+                  : "%s: a ComplexF64 (elsize 16) plan, or PA_FFT_F32 for ComplexF32", what);
+    return PA_EINVAL;
+  }
+  const Pencil& Pi = *P->pin;
+  for (int i = 0; i < Pi.topo->M; ++i)
+    if (Pi.decomp[i] == Pi.perm[0]) {
+      set_error("%s: the transform axis (logical dim %d, the first memory dim of src) is decomposed",
+                what, Pi.perm[0] + 1);
+      return PA_EINVAL;
+    }
+  FftPutParams pp;
+  int C = 0;
+  unsigned long long grid = 0;
+  if (P->dim < 0 || P->nproc == 1) {
+    const BlockCopy* b = &P->self_fused;
+    return put_fft_geometry(1, &b, nullptr, nullptr, f32, rfft, pp, &C, &grid);
+  }
+  if (P->method != PA_PEER_PUT) {
+    set_error("%s: the send-side fusion needs PeerPut (or a local transposition); with "
+              "PointToPoint, Alltoallv or PeerGet transform src first and fuse the next transform "
+              "into the receive side (pa_transpose with PA_FFT_FORWARD / PA_FFT_BACKWARD)", what);
+    return PA_EINVAL;
+  }
+  for (int n = 0; n < P->nproc; ++n) {
+    std::unique_ptr<Plan> hold;
+    const Plan* Q = nullptr;
+    pa_status s = line_plan(P, n, hold, &Q);
+    if (s != PA_OK) return s;
+    std::vector<const BlockCopy*> bl;
+    for (int k = 0; k < Q->nproc; ++k)
+      bl.push_back(k == Q->self_index ? &Q->self_fused : &Q->peers[k].put);
+    s = put_fft_geometry(Q->nproc, bl.data(), nullptr, nullptr, f32, rfft, pp, &C, &grid);
+    if (s != PA_OK) {
+      if (n != P->self_index) {
+        const std::string why = last_error();
+        set_error("%s (on rank %d of the grid line)", why.c_str(), n + 1);
+      }
+      return s;
+    }
+  }
+  return PA_OK;
+}
+
+// Cached per plan, per precision and (lines per CTA of fft_) per value of tunable fft_lines, apart
+// from every other verdict.
+pa_status plan_fft_put_check(Plan* P, bool f32) {
+  const int q = f32 ? 1 : 0;
+  if (P->fft_put_check_lines[q] != g_tun.fft_lines) {
+    P->fft_put_check[q] = put_check(P, f32, false);
+    P->fft_put_check_err[q] = P->fft_put_check[q] == PA_OK ? std::string() : std::string(last_error());
+    P->fft_put_check_lines[q] = g_tun.fft_lines;
+  } else if (P->fft_put_check[q] != PA_OK) {
+    set_error("%s", P->fft_put_check_err[q].c_str());
+  }
+  return P->fft_put_check[q];
+}
+
+// Cached per plan and per precision, apart from every other verdict.
+pa_status plan_rfft_put_check(Plan* P, bool f32) {
+  const int q = f32 ? 1 : 0;
+  if (!P->rfft_put_checked[q]) {
+    P->rfft_put_check[q] = put_check(P, f32, true);
+    P->rfft_put_check_err[q] = P->rfft_put_check[q] == PA_OK ? std::string() : std::string(last_error());
+    P->rfft_put_checked[q] = true;
+  } else if (P->rfft_put_check[q] != PA_OK) {
+    set_error("%s", P->rfft_put_check_err[q].c_str());
+  }
+  return P->rfft_put_check[q];
 }
 
 pa_status rfft_lines(int N, bool forward, bool f32, i64 nlines, const void* src, void* dst,

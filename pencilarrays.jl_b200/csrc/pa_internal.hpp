@@ -233,6 +233,15 @@ struct Plan {
   bool real_checked[2] = {false, false};
   pa_status real_check[2] = {PA_OK, PA_OK};
   std::string real_check_err[2];
+  // cached answers of plan_fft_put_check ([0] ComplexF64, [1] ComplexF32; each valid while tunable
+  // fft_lines == fft_put_check_lines[i]) and of plan_rfft_put_check ([0] Float64 -> ComplexF64,
+  // [1] Float32 -> ComplexF32)
+  int fft_put_check_lines[2] = {-1, -1};
+  pa_status fft_put_check[2] = {PA_OK, PA_OK};
+  std::string fft_put_check_err[2];
+  bool rfft_put_checked[2] = {false, false};
+  pa_status rfft_put_check[2] = {PA_OK, PA_OK};
+  std::string rfft_put_check_err[2];
   ~Plan();
 };
 
@@ -318,6 +327,24 @@ pa_status unpack_rfft(int nb, const BlockCopy* const* blocks, const void* const*
 // plan_fft_check's question for unpack_r2r and unpack_rfft (one verdict for both); its own
 // cache, the same uniformity over the line
 pa_status plan_real_check(Plan* plan, bool f32);
+// send-side fused transform + put (fft.cu, k_fft_put / k_rfft_put): the transform along the
+// first memory dim of the local `src`, every output bin stored into the block that owns it.
+// blocks[i] / dsts[i]: the self block (self_fused) into the local dst, the put block of every
+// other rank into that rank's dst as mapped here.  rfft: the plan is the complex plan of N/2 + 1
+// bins per line and `src` the real array of N reals per line; else sign -1 forward, +1 backward.
+// `mf` (NULL: none): the window protocol spoken inside the launch.  *launched = false: this rank
+// has no source lines and nothing was launched -- the caller then speaks the protocol with flag
+// kernels
+pa_status put_fft(int nb, const BlockCopy* const* blocks, const void* src, void* const* dsts, int sign,
+                  bool rfft, bool f32, const MultiFlags* mf, void* stream, bool* launched);
+// can put_fft run the complex FFT (rfft: the r2c transform) on this plan?  PeerPut plans and local
+// transposes only; the same answer on every rank of the grid line; own caches.  No device call.
+pa_status plan_fft_put_check(Plan* plan, bool f32);
+pa_status plan_rfft_put_check(Plan* plan, bool f32);
+// dst = transpose(fft_(src)) (rfft: transpose(rfft_(src)), src the real array) on the caller's
+// stream (local plans) or PeerPut's one-sided schedule; every argument has been checked
+pa_status transpose_put_fft(Plan* plan, Comm* comm, const void* src, void* dst, unsigned flags,
+                            bool rfft, void* stream);
 // real-line transforms (fft.cu): `nlines` dense, consecutive lines of N reals (src when forward,
 // dst when backward) <-> N/2 + 1 complex bins; N a power of two in 16..2048.  f32: Float32 <->
 // ComplexF32, else Float64 <-> ComplexF64

@@ -669,6 +669,9 @@ static BlockCopy contiguous_block(i64 bytes, const void* src, const void* dst) {
 }
 
 // ---- the one-sided methods --------------------------------------------------------
+// the send-side fused transform a PeerPut schedule runs in place of its put kernels
+enum class SendFft { none, fft, rfft };
+
 // PeerPut: each remote block is read from `src` and stored, already permuted,
 // into the destination rank's `dest` through its peer mapping.  PeerGet is the
 // pull flavour (window on `src`).  Protocol per transposition and pair of ranks:
@@ -678,12 +681,15 @@ static BlockCopy contiguous_block(i64 bytes, const void* src, const void* dst) {
 // fft_sign != 0 (PeerGet only): the fused gather + FFT (k_get_fft) replaces the get kernel and
 // the self block -- ONE kernel reads every line from the peers' src and the local src,
 // transforms and stores it; the protocol around it is the same.
+// send != none (PeerPut only): the send-side fused transform (k_fft_put / k_rfft_put) replaces
+// the put kernel and the self block -- ONE kernel loads every local source line, transforms it
+// and stores its bins into the local dst and the peers' dst (fft_sign: the FFT's direction).
 static pa_status one_sided(Plan* P, Comm* comm, const void* src, void* dst, unsigned flags,
-                           int fft_sign, cudaStream_t user) {
+                           int fft_sign, SendFft send, cudaStream_t user) {
   TransposeState& S = *P->st;
   const int nproc = P->nproc, me = P->self_index;
   const bool get = P->method == PA_PEER_GET;
-  const bool fft = fft_sign != 0;
+  const bool fft = fft_sign != 0 || send != SendFft::none;  // one fused kernel replaces the blocks
   const bool timing = S.timing;
   // (a rank none of whose peers owns anything has no window to register: nothing will be
   //  put / got, but it still speaks the protocol)
@@ -731,15 +737,21 @@ static pa_status one_sided(Plan* P, Comm* comm, const void* src, void* dst, unsi
   const int np = nproc - 1;
   // fft: every get block and the self block in one kernel, `mf` spoken inside it (NULL: none);
   // *launched = false on a rank without destination lines
+  // (send: the self block and every put block, stored into dst / the peers' dst)
   std::vector<const BlockCopy*> fb;
   std::vector<const void*> fs;
+  std::vector<void*> fd;
   for (int n = 0; fft && n < nproc; ++n) {
-    fb.push_back(n == me ? &P->self_fused : &P->peers[n].get);
+    fb.push_back(n == me ? &P->self_fused : get ? &P->peers[n].get : &P->peers[n].put);
     fs.push_back(n == me ? src : (const void*)win[n]);
+    fd.push_back(n == me ? dst : win[n]);
   }
   auto fused = [&](const MultiFlags* mf, bool* launched) {
-    return get_fft(nproc, fb.data(), fs.data(), dst, fft_sign, (flags & PA_FFT_F32) != 0, mf, S.comm_s,
-                   launched);
+    const bool f32 = (flags & PA_FFT_F32) != 0;
+    if (send != SendFft::none)
+      return put_fft(nproc, fb.data(), src, fd.data(), fft_sign, send == SendFft::rfft, f32, mf, S.comm_s,
+                     launched);
+    return get_fft(nproc, fb.data(), fs.data(), dst, fft_sign, f32, mf, S.comm_s, launched);
   };
   bool launched = false;
 
@@ -770,8 +782,9 @@ static pa_status one_sided(Plan* P, Comm* comm, const void* src, void* dst, unsi
       mf.err = comm->fence_err;
       if (fft) {
         RC(fused(&mf, &launched));
-        // (no destination lines on this rank: its src is still read, so the flag kernels below
-        //  speak the protocol without a kernel between them)
+        // (no destination lines on this rank -- send: no source lines -- yet its peers still
+        //  read its src / store into its dst, so the flag kernels below speak the protocol
+        //  without a kernel between them)
         rc = launched ? PA_OK : PA_EINCOMPAT;
       } else {
         rc = launch_multi(np, blocks.data(), srcs.data(), dsts.data(), S.comm_s, g_tun.remote_ctas,
@@ -825,8 +838,9 @@ static pa_status one_sided(Plan* P, Comm* comm, const void* src, void* dst, unsi
     RC(line_barrier());
   }
   if (fft) {
-    // dst is complete once the fused kernel is (ev_allpacked); the DONE steps behind it on the
-    // comm stream only guard the reuse of src
+    // get: dst is complete once the fused kernel is (ev_allpacked); the DONE steps behind it on
+    // the comm stream only guard the reuse of src.  send: the local part of dst is complete then,
+    // the peers' parts at ev_comm_done, which the caller's stream waits for below
     CU(cudaStreamWaitEvent(S.unpack_s, S.ev_allpacked, 0));
     CU(cudaEventRecord(S.ev_unpack_done, S.unpack_s));
     if (timing) CU(cudaEventRecord(S.t[5], S.unpack_s));
@@ -1275,8 +1289,48 @@ pa_status transpose(Plan* P, Comm* comm, const void* src, void* dst, unsigned fl
     CU(cudaStreamWaitEvent(s, buf_ev, 0));
     CU(cudaStreamWaitEvent(s, buf_unpack_ev, 0));
   }
-  if (one) return one_sided(P, comm, src, dst, flags, fft_sign, user);
+  if (one) return one_sided(P, comm, src, dst, flags, fft_sign, SendFft::none, user);
   return staged(P, comm, src, dst, flags, mode, r2r_kind, stage_self, user, buf_ev, buf_unpack_ev);
+}
+
+pa_status transpose_put_fft(Plan* P, Comm* comm, const void* src, void* dst, unsigned flags, bool rfft,
+                            void* stream) {
+  // (pa_fft_put / pa_rfft_put have checked the flags, the arrays and the plan's verdict, which
+  //  admits PeerPut plans and local transposes only)
+  RC(ensure_state(P));
+  TransposeState& S = *P->st;
+  cudaStream_t user = (cudaStream_t)stream;
+  const bool timing = S.timing;
+  const int sign = rfft || (flags & PA_FFT_FORWARD) ? -1 : 1;
+  const bool f32 = (flags & PA_FFT_F32) != 0;
+  if (timing) CU(cudaEventRecord(S.t[0], user));
+  if (P->dim < 0 || P->nproc == 1) {
+    // one block, the whole local array: one kernel on the caller's stream
+    const BlockCopy* b = &P->self_fused;
+    bool launched = false;
+    RC(put_fft(1, &b, src, &dst, sign, rfft, f32, nullptr, user, &launched));
+    if (timing) {
+      CU(cudaEventRecord(S.t[6], user));
+      S.timed_once = true;
+    }
+    return PA_OK;
+  }
+  if (!comm) {
+    set_error("this transposition exchanges data among %d ranks: a communicator is required",
+              P->nproc);
+    return PA_ESTATE;
+  }
+  // fork as transpose() does for the one-sided methods
+  Buffers& B = *P->pout->bufs;
+  cudaEvent_t buf_ev, buf_unpack_ev;
+  RC(buffer_events(B, &buf_ev, &buf_unpack_ev));
+  CU(cudaEventRecord(S.ev_start, user));
+  for (cudaStream_t s : {S.pack_s, S.comm_s, S.unpack_s}) {
+    CU(cudaStreamWaitEvent(s, S.ev_start, 0));
+    CU(cudaStreamWaitEvent(s, buf_ev, 0));
+    CU(cudaStreamWaitEvent(s, buf_unpack_ev, 0));
+  }
+  return one_sided(P, comm, src, dst, flags, sign, rfft ? SendFft::rfft : SendFft::fft, user);
 }
 
 // MPI.Waitall(t::Transposition) (Transpositions.jl:127-130)

@@ -181,17 +181,21 @@ method_code(::PeerGet) = Cint(3)
 function register_window!(t::Transposition)
     plan, H = plan_handle(t)
     A = t.method isa PeerGet ? parent(t.Ai) : parent(t.Ao)
-    comm = get_comm(t.Pi.topology)
+    register_window!(plan, A, t.Pi.topology, t.dim)
+    t
+end
+
+# the same for a bare plan: `A` is the window array, R the grid dim of the exchange
+function register_window!(plan::Ptr{Cvoid}, A, topo, R)
+    comm = get_comm(topo)
     handle = zeros(UInt8, 64)
     off = Ref{Int64}(0)
     check(ccall((:pa_ipc_export, libpa), Cint, (Ptr{Cvoid}, Ptr{UInt8}, Ptr{Int64}), devptr(A), handle, off))
     handles_all = MPI.Allgather(handle, comm)            # 64 bytes per rank
     offs_all = MPI.Allgather([off[]], comm)
-    R = t.dim
-    R === nothing && return t
+    R === nothing && return plan
     # ranks (in `comm`) of my grid line along R: topology.ranks maps Cartesian
     # coordinates to ranks (MPITopologies.jl:84-86,208-226); get_remote_indices (:539-549)
-    topo = t.Pi.topology
     coords = topo.coords_local
     line = [topo.ranks[ntuple(i -> i == R ? n : coords[i], length(coords))...] for n in 1:size(topo)[R]]
     me = MPI.Comm_rank(comm)
@@ -205,7 +209,7 @@ function register_window!(t::Transposition)
         # (each import holds a reference on the mapping: pair it with pa_ipc_release(handle)
         #  when the window array is freed)
     end
-    t
+    plan
 end
 
 function plan_handle(t::Transposition{T}) where {T}
@@ -463,5 +467,72 @@ function MPI.Waitall(t::DeviceTransposition)
     check(ccall((:pa_wait, libpa), Cint, (Ptr{Cvoid}, Ptr{Cvoid}), plan, stream_ptr()))
     nothing
 end
+
+# Send-side fused transform + transposition (pa_fft_put / pa_rfft_put): the transform along the
+# FIRST memory dimension of `src` (not decomposed) runs in the put kernel -- one kernel per GPU
+# loads every local source line, transforms it and stores the bins into the peers' dest through
+# the PeerPut window.  PeerPut, or a local transposition with any method; byte for byte the
+# unfused pair (fft_lines! on a copy / rfft!, then transpose!).
+#   fft_transpose!(t; direction = :forward | :backward): dest = transpose(fft(src)) on a complex
+#     Transposition (register_window! it first under PeerPut, as for transpose!).
+#   rfft_transpose!(dest, src, pc): dest = transpose(rfft(src)), `src` R on the real x-pencil,
+#     `dest` Complex{R} on the complex y-pencil; `pc`: the complex x-pencil the plan transposes
+#     from, `Pencil(pencil(src); size_global = (..., N÷2+1, ...))` -- passed explicitly, as in
+#     transpose_brfft!.  Under PeerPut it registers dest's window itself (collective).
+function fft_transpose!(t::DeviceTransposition{T}; direction = :forward, waitall = true) where {T}
+    plan, H = plan_handle(t)
+    dir = direction === :forward ? Cuint(8) : direction === :backward ? Cuint(16) :
+        throw(ArgumentError("direction must be :forward or :backward"))
+    flags = (waitall ? Cuint(1) : Cuint(0)) | dir | fft_precision_flag(T)   # PA_WAITALL, PA_FFT_*
+    ptr_or_null(A) = isempty(A) ? C_NULL : devptr(A)
+    check(ccall((:pa_fft_put, libpa), Cint,
+        (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Cuint, Ptr{Cvoid}),
+        plan, H.comm, ptr_or_null(parent(t.Ai)), ptr_or_null(parent(t.Ao)), flags, stream_ptr()))
+    t
+end
+
+function rfft_put_plan(pc::Pencil, dest::PencilArray{Complex{R}}, method) where {R}
+    H = handles(pc.topology)
+    ex = Int64[extra_dims(dest)...]
+    key = (objectid(pc), objectid(pencil(dest)), Tuple(ex), sizeof(Complex{R}), method_code(method))
+    plan = get!(H.plans, key) do
+        h = Ref{Ptr{Cvoid}}()
+        check(ccall((:pa_plan_create, libpa), Cint,
+            (Ptr{Cvoid}, Ptr{Cvoid}, Cint, Ptr{Int64}, Cint, Cint, Ptr{Ptr{Cvoid}}),
+            pencil_handle(H, pc), pencil_handle(H, pencil(dest)), length(ex), ex, sizeof(Complex{R}),
+            method_code(method), h))
+        h[]
+    end
+    plan, H
+end
+
+function rfft_transpose!(dest::PencilArray{Complex{R},N,<:CuArray}, src::PencilArray{R,N,<:CuArray},
+                         pc::Pencil; method = PeerPut(), waitall = true) where {R<:Union{Float64,Float32},N}
+    plan, H = rfft_put_plan(pc, dest, method)
+    flag = R === Float32 ? Cuint(32) : Cuint(0)   # PA_FFT_F32
+    # refused (on every rank of the line alike) before the collective window setup
+    check(ccall((:pa_plan_rfft_put_check, libpa), Cint, (Ptr{Cvoid}, Cuint), plan, flag))
+    if method isa PeerPut
+        R_dim = findfirst(i -> decomposition(pc)[i] != decomposition(pencil(dest))[i],
+                          1:length(decomposition(pc)))
+        register_window!(plan, parent(dest), pc.topology, R_dim)
+    end
+    flags = (waitall ? Cuint(1) : Cuint(0)) | flag   # PA_WAITALL
+    ptr_or_null(A) = isempty(A) ? C_NULL : devptr(A)
+    check(ccall((:pa_rfft_put, libpa), Cint,
+        (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Cuint, Ptr{Cvoid}),
+        plan, H.comm, pencil_handle(H, pencil(src)), ptr_or_null(parent(src)), ptr_or_null(parent(dest)),
+        flags, stream_ptr()))
+    dest
+end
+
+# Whether fft_transpose! / rfft_transpose! can run (pa_plan_fft_put_check / pa_plan_rfft_put_check):
+# the same answer on every rank of the grid line.
+fft_first_fusable(t::DeviceTransposition{T}) where {T} =
+    ccall((:pa_plan_fft_put_check, libpa), Cint, (Ptr{Cvoid}, Cuint), first(plan_handle(t)),
+          fft_precision_flag(T)) == 0
+rfft_first_fusable(dest::PencilArray{Complex{R}}, pc::Pencil; method = PeerPut()) where {R} =
+    ccall((:pa_plan_rfft_put_check, libpa), Cint, (Ptr{Cvoid}, Cuint), first(rfft_put_plan(pc, dest, method)),
+          R === Float32 ? Cuint(32) : Cuint(0)) == 0
 
 end # module

@@ -8,6 +8,8 @@
     t = Transposition(real_x, cplx_y; brfft=True)         # GPU extension: real = brfft(transpose)
     t = Transposition(real_y, real_x; r2r="REDFT10")      # GPU extension: real = r2r(transpose)
     t = Transposition(cplx_y, real_x; rfft=True)          # GPU extension: cplx = rfft(transpose)
+    transpose_(t; fft_first="forward")                    # GPU extension: dest = transpose(fft(src))
+    t = Transposition(cplx_y, real_x; rfft_first=True)    # GPU extension: cplx = transpose(rfft(src))
 
 Python has no ``!`` in identifiers: ``transpose_`` (torch's in-place naming)
 stands for ``transpose!``; ``transpose_bang`` is an alias.  Errors follow the
@@ -58,6 +60,9 @@ class PeerPut(AbstractTransposeMethod):
     is COLLECTIVE over the communicator (like ``MPI_Win_create``): it exchanges
     CUDA IPC handles of ``dest``.  Falls back to the staged PointToPoint
     schedule when ``src`` and ``dest`` alias (in-place transposes).
+    ``transpose_(t, fft_first=...)`` and ``Transposition(..., rfft_first=True)`` fuse the
+    transform along ``src``'s first memory dimension into the put kernel: one kernel per rank
+    loads every local source line, transforms it and stores the bins into the peers' ``dest``.
     """
     code = _lib.PA_PEER_PUT
 
@@ -291,18 +296,25 @@ class Transposition:
     ``Ao`` complex128 (complex64) on the complex y-pencil of N//2+1 points along its first memory
     dim; the plan is the real x -> y plan to ``Ao``'s real counterpart, and ``transpose_(t)``
     writes ``Ao = rfft_(transpose(Ai))`` (``pa_transpose_rfft``).  Both are byte for byte the
-    unfused pair, without the array in between.  ``brfft``, ``r2r`` and ``rfft`` exclude each
-    other."""
+    unfused pair, without the array in between.
+
+    ``rfft_first=True`` (GPU extension, send side): ``Ai`` is float64 (float32) on a real pencil of
+    N points along its first memory dim and ``Ao`` complex128 (complex64); the plan is the complex
+    plan from ``Ai``'s N//2+1 counterpart to ``Ao``'s pencil, and ``transpose_(t)`` writes ``Ao =
+    transpose(rfft_(Ai))`` in one kernel per rank (``pa_rfft_put``): ``PeerPut``, or a local
+    transposition with any method.  Byte for byte ``rfft_`` followed by the plain transposition.
+    ``brfft``, ``r2r``, ``rfft`` and ``rfft_first`` exclude each other."""
 
     def __init__(self, Ao: PencilArray, Ai: PencilArray, *, method=None, brfft=False, r2r=None,
-                 rfft=False):
+                 rfft=False, rfft_first=False):
         method = PointToPoint() if method is None else method
         Pi, Po = Ai.pencil, Ao.pencil
         self.brfft = bool(brfft)
         self.r2r = r2r
         self.rfft = bool(rfft)
-        if self.brfft + (r2r is not None) + self.rfft > 1:
-            raise ArgumentError(_lib.PA_EINVAL, "brfft=, r2r= and rfft= exclude each other")
+        self.rfft_first = bool(rfft_first)
+        if self.brfft + (r2r is not None) + self.rfft + self.rfft_first > 1:
+            raise ArgumentError(_lib.PA_EINVAL, "brfft=, r2r=, rfft= and rfft_first= exclude each other")
         if Ai.extra_dims != Ao.extra_dims:  # :99-103
             raise ArgumentError(_lib.PA_EINVAL,
                                 "incompatible number of extra dimensions of PencilArrays: "
@@ -320,6 +332,12 @@ class Transposition:
                                     "complex128, or float32 and complex64: got "
                                     f"{Ai.dtype} and {Ao.dtype}")
             Po = _rfft_pencil(Ao.pencil)  # the plan's output: the real y-pencil
+        elif self.rfft_first:
+            if (Ai.dtype, Ao.dtype) not in _BRFFT_PAIRS:
+                raise ArgumentError(_lib.PA_EINVAL, "rfft_first: src and dest must be float64 and "
+                                    "complex128, or float32 and complex64: got "
+                                    f"{Ai.dtype} and {Ao.dtype}")
+            Pi = _brfft_pencil(Ai.pencil)  # the plan's input: the complex counterpart of src
         elif self.brfft:
             if (Ao.dtype, Ai.dtype) not in _BRFFT_PAIRS:
                 raise ArgumentError(_lib.PA_EINVAL, "brfft: dest and src must be float64 and "
@@ -332,9 +350,13 @@ class Transposition:
             raise ArgumentError(_lib.PA_EINCOMPAT, "pencil topologies must be the same.")
         self.Pi, self.Po, self.Ai, self.Ao = Pi, Po, Ai, Ao
         self.method = method
-        self._plan = _get_plan(Pi, Po, Ai.extra_dims, Ai.elsize, method)  # remaining checks in C
+        elsize = Ao.elsize if self.rfft_first else Ai.elsize  # (rfft_first: the complex plan)
+        self._plan = _get_plan(Pi, Po, Ai.extra_dims, elsize, method)  # remaining checks in C
         d = self._plan.info.dim
         self.dim = None if d == 0 else d  # :110
+        if self.rfft_first:
+            # (the same verdict on every rank of the line: refused before the collective window setup)
+            check(lib.pa_plan_rfft_put_check(self._plan.h, _BRFFT_PAIRS[(Ai.dtype, Ao.dtype)]))
         fused = "brfft" if self.brfft else "rfft" if self.rfft else "r2r" if r2r is not None else None
         if fused and d != 0 and self._plan.info.nproc > 1 and isinstance(method, (PeerPut, PeerGet)):
             # (the same on every rank of the line: refused before the collective window setup)
@@ -370,12 +392,28 @@ class Transposition:
         nothing to fuse with, and ``transpose_(t, fft=...)`` refuses it whatever this says.
         For a ``brfft=True`` transposition: whether ``pa_transpose_brfft`` can run
         (``pa_plan_brfft_check``); for ``r2r=`` / ``rfft=True``: whether ``pa_transpose_r2r`` /
-        ``pa_transpose_rfft`` can (``pa_plan_real_check``, one answer for both)."""
+        ``pa_transpose_rfft`` can (``pa_plan_real_check``, one answer for both); for an
+        ``rfft_first=True`` one: False (see :meth:`fft_first_fusable`)."""
+        if self.rfft_first:
+            return False
         if self.r2r is not None or self.rfft:
             return lib.pa_plan_real_check(self._plan.h, _REAL_FLAGS[self.Ai.dtype]) == _lib.PA_OK
         if self.brfft:
             return lib.pa_plan_brfft_check(self._plan.h, _fft_precision_flag(self.Ai)) == _lib.PA_OK
         return lib.pa_plan_fft_check_ex(self._plan.h, _fft_precision_flag(self.Ai)) == _lib.PA_OK
+
+
+    def fft_first_fusable(self) -> bool:
+        """Whether the send-side fused kernel can run on this transposition: for a complex one
+        ``transpose_(self, fft_first=...)`` (``pa_plan_fft_put_check``), for an ``rfft_first=True``
+        one ``transpose_(self)`` (``pa_plan_rfft_put_check``).  Needs ``PeerPut`` when the
+        transposition exchanges data; the answer is the same on every rank of the grid line."""
+        if self.rfft_first:
+            flag = _BRFFT_PAIRS[(self.Ai.dtype, self.Ao.dtype)]
+            return lib.pa_plan_rfft_put_check(self._plan.h, flag) == _lib.PA_OK
+        if self.brfft or self.rfft or self.r2r is not None:
+            return False
+        return lib.pa_plan_fft_put_check(self._plan.h, _fft_precision_flag(self.Ai)) == _lib.PA_OK
 
 
 def _fft_precision_flag(u: PencilArray) -> int:
@@ -390,7 +428,8 @@ def Waitall(t: Transposition):
     return None
 
 
-def transpose_(*args, method=None, waitall=True, overlap=True, stage_self=False, fft=None):
+def transpose_(*args, method=None, waitall=True, overlap=True, stage_self=False, fft=None,
+               fft_first=None):
     """``transpose!(dest, src; method)`` or ``transpose!(t; waitall)`` (:160-179).
 
     ``fft="forward"`` / ``"backward"`` (GPU extension, SURVEY 8 f2): the unpack and the
@@ -401,8 +440,16 @@ def transpose_(*args, method=None, waitall=True, overlap=True, stage_self=False,
     out of the peers' ``src`` arrays (one kernel per rank, no staging; ``waitall=False`` defers
     only the fence that guards the reuse of ``src``).  ``PeerPut`` is refused.
 
-    A ``Transposition(..., brfft=True)`` (``r2r=``, ``rfft=True``) runs the fused transpose +
-    complex-to-real (real-to-real, real-to-complex) transform; ``fft=`` does not apply to it."""
+    ``fft_first="forward"`` / ``"backward"`` (GPU extension, send side): ``dest`` receives the
+    transposition of the 1-d FFT of ``src`` along ``src``'s first memory dimension, in one kernel
+    per rank that loads the source lines, transforms them and stores every bin into the rank
+    that owns it (``pa_fft_put``): ``PeerPut``, or a local transposition with any method.  Byte
+    for byte ``fft_`` on a copy of ``src`` followed by the plain transposition; ``fft=`` and
+    ``fft_first=`` exclude each other.
+
+    A ``Transposition(..., brfft=True)`` (``r2r=``, ``rfft=True``, ``rfft_first=True``) runs the
+    fused transpose + complex-to-real (real-to-real, real-to-complex) transform; ``fft=`` and
+    ``fft_first=`` do not apply to it."""
     if len(args) == 1 and isinstance(args[0], Transposition):
         t = args[0]
     elif len(args) == 2:
@@ -415,6 +462,16 @@ def transpose_(*args, method=None, waitall=True, overlap=True, stage_self=False,
         raise TypeError("transpose_(dest, src; method) or transpose_(t; waitall)")
     flags = (_lib.PA_WAITALL if waitall else 0) | (0 if overlap else _lib.PA_NO_OVERLAP) | (
         _lib.PA_STAGE_SELF if stage_self else 0)
+    if t.rfft_first:
+        if fft is not None or fft_first is not None:
+            raise ArgumentError(_lib.PA_EINVAL, "an rfft_first transposition implies its transform: "
+                                "transpose_(t) without fft= / fft_first=")
+        check(lib.pa_rfft_put(t.plan.h, t.Pi.topology.comm.handle, t.Ai.pencil._h,
+                              C.c_void_p(t.Ai.data_ptr() or None), C.c_void_p(t.Ao.data_ptr() or None),
+                              flags | _BRFFT_PAIRS[(t.Ai.dtype, t.Ao.dtype)], _stream_ptr()))
+        return t if len(args) == 1 else args[0]
+    if fft_first is not None and (t.brfft or t.rfft or t.r2r is not None):
+        raise ArgumentError(_lib.PA_EINVAL, "fft_first= applies to complex transpositions only")
     if t.brfft:
         if fft is not None:
             raise ArgumentError(_lib.PA_EINVAL, "a brfft transposition implies its transform: "
@@ -437,6 +494,19 @@ def transpose_(*args, method=None, waitall=True, overlap=True, stage_self=False,
         else:
             check(lib.pa_transpose_r2r(t.plan.h, comm, _R2R_KINDS[t.r2r], src, dst, flags,
                                        _stream_ptr()))
+        return t if len(args) == 1 else args[0]
+    if fft_first is not None:
+        if fft is not None:
+            raise ArgumentError(_lib.PA_EINVAL, "fft= and fft_first= exclude each other")
+        if fft_first in ("forward", -1):
+            flags |= _lib.PA_FFT_FORWARD
+        elif fft_first in ("backward", 1):
+            flags |= _lib.PA_FFT_BACKWARD
+        else:
+            raise ArgumentError(_lib.PA_EINVAL, "fft_first must be 'forward' or 'backward'")
+        check(lib.pa_fft_put(t.plan.h, t.Pi.topology.comm.handle, C.c_void_p(t.Ai.data_ptr() or None),
+                             C.c_void_p(t.Ao.data_ptr() or None), flags | _fft_precision_flag(t.Ai),
+                             _stream_ptr()))
         return t if len(args) == 1 else args[0]
     if fft is not None:
         if fft in ("forward", -1):
