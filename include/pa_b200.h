@@ -521,6 +521,33 @@ pa_status pa_put_all_rfft(pa_plan* plan, const pa_pencil* real, const void* src,
  * `flags` matters.  Cached per plan and precision, apart from every other verdict.  Host-only.  */
 pa_status pa_plan_fft_put_check(const pa_plan* plan, unsigned flags);
 pa_status pa_plan_rfft_put_check(const pa_plan* plan, unsigned flags);
+/* The wall-bounded legs of the same send-side fusion (DESIGN §3j).  `plan` is a REAL plan (Float64,
+ * elsize 8; Float32, elsize 4 with PA_FFT_F32) that moves N reals per line along the first memory
+ * dim of its input pencil, N a power of two in 16..2048; the blocks may split a line at any real.
+ * pa_r2r_put: T is pa_r2r's transform of `kind` (PA_REDFT10, PA_REDFT01, PA_RODFT10 or PA_RODFT01)
+ *   on the real src; dst equals pa_r2r on a copy of src followed by pa_transpose.
+ * pa_brfft_put: T is the c2r transform of pa_brfft; src is the ComplexF64 (ComplexF32) array on
+ *   `cplx`, the N/2+1-bin counterpart of the plan's input pencil (related to it as `cplx` to `real`
+ *   in pa_rfft); dst equals pa_brfft followed by pa_transpose of the real array.
+ * flags: any of PA_FFT_F32 and PA_WAITALL (the direction is implied); every other bit, PA_STAGE_SELF
+ * included, is PA_EINVAL, as is any other kind.  src (aligned to 2 reals) and dst (aligned to the
+ * real) must not overlap, NULL only when empty.  Schedule, protocol, events, refusals on the host
+ * (a `cplx` not related to the plan's input pencil: PA_EINCOMPAT) and PA_ENOGPU as for pa_fft_put. */
+pa_status pa_r2r_put(pa_plan* plan, pa_comm* comm, int kind, const void* src, void* dst, unsigned flags,
+                     void* stream);
+pa_status pa_brfft_put(pa_plan* plan, pa_comm* comm, const pa_pencil* cplx, const void* src, void* dst,
+                       unsigned flags, void* stream);
+/* Their kernels without the window protocol, as pa_put_all_fft: the self block into `dst`, the
+ * block of peer n into `peers[n-1]`.  flags: 0 or PA_FFT_F32.  The plan must exchange data.      */
+pa_status pa_put_all_r2r(pa_plan* plan, int kind, const void* src, void* const* peers, void* dst,
+                         unsigned flags, void* stream);
+pa_status pa_put_all_brfft(pa_plan* plan, const pa_pencil* cplx, const void* src, void* const* peers,
+                           void* dst, unsigned flags, void* stream);
+/* Can pa_r2r_put and pa_brfft_put run on this real plan?  One verdict for both, with the rules of
+ * pa_plan_fft_put_check (line length N, at most 8 blocks, PA_PEER_PUT when the plan exchanges data,
+ * the same answer on every rank of the grid line).  Only PA_FFT_F32 of `flags` matters.  Cached per
+ * plan and precision, apart from every other verdict.  Host-only.                                 */
+pa_status pa_plan_real_put_check(const pa_plan* plan, unsigned flags);
 
 /* ---- host chains -----------------------------------------------------------
  * A sequence of transpositions applied to HOST arrays (plan i+1 consumes what

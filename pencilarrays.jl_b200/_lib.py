@@ -144,6 +144,11 @@ SIGNATURES = {
     "pa_put_all_rfft": (C.c_int, [_P, _P, _P, C.POINTER(_P), _P, C.c_uint, _P]),
     "pa_plan_fft_put_check": (C.c_int, [_P, C.c_uint]),
     "pa_plan_rfft_put_check": (C.c_int, [_P, C.c_uint]),
+    "pa_r2r_put": (C.c_int, [_P, _P, C.c_int, _P, _P, C.c_uint, _P]),
+    "pa_brfft_put": (C.c_int, [_P, _P, _P, _P, _P, C.c_uint, _P]),
+    "pa_put_all_r2r": (C.c_int, [_P, C.c_int, _P, C.POINTER(_P), _P, C.c_uint, _P]),
+    "pa_put_all_brfft": (C.c_int, [_P, _P, _P, C.POINTER(_P), _P, C.c_uint, _P]),
+    "pa_plan_real_put_check": (C.c_int, [_P, C.c_uint]),
     "pa_host_chain_create": (C.c_int, [C.c_int, C.POINTER(_P), _P, C.POINTER(_P)]),
     "pa_host_chain_destroy": (None, [_P]),
     "pa_host_chain_submit": (C.c_int, [_P, _P, _P, _I64P]),

@@ -1090,24 +1090,28 @@ pa_status pa_plan_real_check(const pa_plan* plan, unsigned flags) {
   })
 }
 
-// ---- send-side fused transform + put (pa_fft_put, pa_rfft_put, pa_put_all_fft / _rfft) ----------
-// The checks they share, all on the host: the plan's verdict, then (rfft) `real` against the plan's
-// INPUT pencil as pa_rfft relates them, then src / dst (NULL only when empty, not overlapping,
-// aligned to the complex element).
-static pa_status put_args(const char* who, Plan& P, const pa_pencil* real, const void* src,
-                          const void* dst, bool rfft, bool f32) {
-  pa_status s = rfft ? plan_rfft_put_check(&P, f32) : plan_fft_put_check(&P, f32);
+// ---- send-side fused transform + put (pa_fft_put, pa_rfft_put, pa_r2r_put, pa_brfft_put and
+//      their pa_put_all_*) ------------------------------------------------------------------------
+// The checks they share, all on the host: the plan's verdict, then (rfft, brfft) `pen` against the
+// plan's INPUT pencil as pa_rfft relates them (rfft: `pen` is the real pencil of src; brfft: the
+// complex one), then src / dst (NULL only when empty, not overlapping, aligned: fft / rfft to the
+// complex element; r2r / brfft src to a pair of reals or a complex element, dst to the real).
+static pa_status put_args(const char* who, Plan& P, const pa_pencil* pen, const void* src,
+                          const void* dst, PutMode mode, bool f32) {
+  const bool rfft = mode == PutMode::rfft, real = mode == PutMode::r2r || mode == PutMode::brfft;
+  pa_status s = real ? plan_real_put_check(&P, f32) : rfft ? plan_rfft_put_check(&P, f32)
+                                                           : plan_fft_put_check(&P, f32);
   if (s != PA_OK) return s;
   const i64 es = P.elsize;
   i64 src_bytes = P.length_in * es;
-  if (rfft) {
+  if (rfft || mode == PutMode::brfft) {
     const pa_pencil in{P.pin};
     int N = 0;
     i64 nlines = 0;
-    s = rfft_checks(who, real, &in, P.n_extra, P.extra, PA_FFT_FORWARD | (f32 ? PA_FFT_F32 : 0u), nullptr,
-                    nullptr, false, &N, &nlines);
+    s = rfft_checks(who, rfft ? pen : &in, rfft ? &in : pen, P.n_extra, P.extra,
+                    PA_FFT_FORWARD | (f32 ? PA_FFT_F32 : 0u), nullptr, nullptr, false, &N, &nlines);
     if (s != PA_OK) return s;
-    src_bytes = nlines * N * (es / 2);
+    src_bytes = rfft ? nlines * N * (es / 2) : nlines * (N / 2 + 1) * 2 * es;
   }
   const i64 dst_bytes = P.length_out * es;
   if ((!src && src_bytes > 0) || (!dst && dst_bytes > 0)) {
@@ -1117,8 +1121,18 @@ static pa_status put_args(const char* who, Plan& P, const pa_pencil* real, const
   const uintptr_t a = (uintptr_t)src, b = (uintptr_t)dst;
   if (src_bytes > 0 && dst_bytes > 0 && a < b + (uintptr_t)dst_bytes && b < a + (uintptr_t)src_bytes) {
     set_error("%s: src and dst overlap (the send-side fusion has no staged schedule: transform in "
-              "place with %s, then transpose)", who, rfft ? "rfft_" : "fft_");
+              "place with %s, then transpose)", who,
+              mode == PutMode::fft ? "fft_" : rfft ? "rfft_" : mode == PutMode::r2r ? "r2r_" : "brfft_");
     return PA_EINVAL;
+  }
+  if (real) {
+    // (the load reads pairs of reals / complex elements; every real is stored alone)
+    if ((src_bytes > 0 && a % (2 * es)) || (dst_bytes > 0 && b % es)) {
+      set_error("%s: src must be aligned to %lld bytes and dst to the %lld-byte real", who,
+                (long long)(2 * es), (long long)es);
+      return PA_EINVAL;
+    }
+    return PA_OK;
   }
   if ((src_bytes > 0 && a % es) || (dst_bytes > 0 && b % es)) {
     set_error("%s: src and dst must be aligned to the %lld-byte complex element", who, (long long)es);
@@ -1127,17 +1141,18 @@ static pa_status put_args(const char* who, Plan& P, const pa_pencil* real, const
   return PA_OK;
 }
 
-// flags: exactly one of PA_FFT_FORWARD / PA_FFT_BACKWARD (rfft: none, the direction is implied),
-// with any of `extra`
-static pa_status put_flags(const char* who, unsigned flags, bool rfft, unsigned extra) {
+// flags: exactly one of PA_FFT_FORWARD / PA_FFT_BACKWARD (fft), or none (rfft, r2r, brfft: the
+// direction is implied), with any of `extra`
+static pa_status put_flags(const char* who, unsigned flags, PutMode mode, unsigned extra) {
   if (flags & PA_STAGE_SELF) {
     set_error("%s: PA_STAGE_SELF does not apply: the send-side fusion stores the self block "
               "straight into dst", who);
     return PA_EINVAL;
   }
+  const bool implied = mode != PutMode::fft;
   const unsigned dir = flags & ~extra;
-  if (rfft ? dir != 0 : (dir != PA_FFT_FORWARD && dir != PA_FFT_BACKWARD)) {
-    if (rfft)
+  if (implied ? dir != 0 : (dir != PA_FFT_FORWARD && dir != PA_FFT_BACKWARD)) {
+    if (implied)
       set_error("%s: flags may combine %s only (the direction is implied)", who,
                 (extra & PA_WAITALL) ? "PA_WAITALL and PA_FFT_F32" : "PA_FFT_F32");
     else
@@ -1148,39 +1163,68 @@ static pa_status put_flags(const char* who, unsigned flags, bool rfft, unsigned 
   return PA_OK;
 }
 
-static pa_status fft_put(pa_plan* plan, pa_comm* comm, const pa_pencil* real, const void* src, void* dst,
-                         unsigned flags, void* stream, bool rfft) {
-  const char* who = rfft ? "pa_rfft_put" : "pa_fft_put";
+static pa_status r2r_kind_check(const char* who, int kind) {
+  if (kind != PA_REDFT10 && kind != PA_REDFT01 && kind != PA_RODFT10 && kind != PA_RODFT01) {
+    set_error("%s: kind %d is not PA_REDFT10, PA_REDFT01, PA_RODFT10 or PA_RODFT01", who, kind);
+    return PA_EINVAL;
+  }
+  return PA_OK;
+}
+
+static const char* put_name(PutMode mode, bool all) {
+  switch (mode) {
+    case PutMode::fft: return all ? "pa_put_all_fft" : "pa_fft_put";
+    case PutMode::rfft: return all ? "pa_put_all_rfft" : "pa_rfft_put";
+    case PutMode::r2r: return all ? "pa_put_all_r2r" : "pa_r2r_put";
+    case PutMode::brfft: break;
+  }
+  return all ? "pa_put_all_brfft" : "pa_brfft_put";
+}
+
+static pa_status fft_put(pa_plan* plan, pa_comm* comm, const pa_pencil* pen, const void* src, void* dst,
+                         unsigned flags, void* stream, PutMode mode, int r2r_kind = 0) {
+  const char* who = put_name(mode, false);
   if (!plan) {
     set_error("%s: null plan", who);
     return PA_EINVAL;
   }
-  pa_status s = put_flags(who, flags, rfft, PA_FFT_F32 | PA_WAITALL);
+  pa_status s = put_flags(who, flags, mode, PA_FFT_F32 | PA_WAITALL);
   if (s != PA_OK) return s;
+  if (mode == PutMode::r2r && (s = r2r_kind_check(who, r2r_kind)) != PA_OK) return s;
   Plan& P = *plan->p;
   const bool f32 = (flags & PA_FFT_F32) != 0;
-  s = put_args(who, P, real, src, dst, rfft, f32);
+  s = put_args(who, P, pen, src, dst, mode, f32);
   if (s != PA_OK) return s;
   s = need_gpu();
   if (s != PA_OK) return s;
-  return transpose_put_fft(&P, comm ? comm->p : nullptr, src, dst, flags, rfft, stream);
+  return transpose_put_fft(&P, comm ? comm->p : nullptr, src, dst, flags, mode, r2r_kind, stream);
 }
 
 pa_status pa_fft_put(pa_plan* plan, pa_comm* comm, const void* src, void* dst, unsigned flags,
                      void* stream) {
-  GUARD({ return fft_put(plan, comm, nullptr, src, dst, flags, stream, false); })
+  GUARD({ return fft_put(plan, comm, nullptr, src, dst, flags, stream, PutMode::fft); })
 }
 
 pa_status pa_rfft_put(pa_plan* plan, pa_comm* comm, const pa_pencil* real, const void* src, void* dst,
                       unsigned flags, void* stream) {
-  GUARD({ return fft_put(plan, comm, real, src, dst, flags, stream, true); })
+  GUARD({ return fft_put(plan, comm, real, src, dst, flags, stream, PutMode::rfft); })
+}
+
+pa_status pa_r2r_put(pa_plan* plan, pa_comm* comm, int kind, const void* src, void* dst, unsigned flags,
+                     void* stream) {
+  GUARD({ return fft_put(plan, comm, nullptr, src, dst, flags, stream, PutMode::r2r, kind); })
+}
+
+pa_status pa_brfft_put(pa_plan* plan, pa_comm* comm, const pa_pencil* cplx, const void* src, void* dst,
+                       unsigned flags, void* stream) {
+  GUARD({ return fft_put(plan, comm, cplx, src, dst, flags, stream, PutMode::brfft); })
 }
 
 // The send-side fused kernel without the window protocol: the self block into `dst`, the put
 // block of peer n into peers[n - 1] (its dst, as mapped here; the self entry is ignored).
-static pa_status put_all_fft(pa_plan* plan, const pa_pencil* real, const void* src, void* const* peers,
-                             void* dst, unsigned flags, void* stream, bool rfft) {
-  const char* who = rfft ? "pa_put_all_rfft" : "pa_put_all_fft";
+static pa_status put_all_fft(pa_plan* plan, const pa_pencil* pen, const void* src, void* const* peers,
+                             void* dst, unsigned flags, void* stream, PutMode mode, int r2r_kind = 0) {
+  const char* who = put_name(mode, true);
   if (!plan) {
     set_error("%s: null plan", who);
     return PA_EINVAL;
@@ -1190,10 +1234,11 @@ static pa_status put_all_fft(pa_plan* plan, const pa_pencil* real, const void* s
     set_error("%s: plan has no exchange", who);
     return PA_EINVAL;
   }
-  pa_status s = put_flags(who, flags, rfft, PA_FFT_F32);
+  pa_status s = put_flags(who, flags, mode, PA_FFT_F32);
   if (s != PA_OK) return s;
+  if (mode == PutMode::r2r && (s = r2r_kind_check(who, r2r_kind)) != PA_OK) return s;
   const bool f32 = (flags & PA_FFT_F32) != 0;
-  s = put_args(who, P, real, src, dst, rfft, f32);
+  s = put_args(who, P, pen, src, dst, mode, f32);
   if (s != PA_OK) return s;
   const i64 es = P.elsize;
   std::vector<const BlockCopy*> blocks;
@@ -1216,18 +1261,38 @@ static pa_status put_all_fft(pa_plan* plan, const pa_pencil* real, const void* s
   s = need_gpu();
   if (s != PA_OK) return s;
   bool launched = false;
-  return put_fft(P.nproc, blocks.data(), src, dsts.data(), (flags & PA_FFT_BACKWARD) ? 1 : -1, rfft, f32,
-                 nullptr, stream, &launched);
+  return put_fft(P.nproc, blocks.data(), src, dsts.data(), (flags & PA_FFT_BACKWARD) ? 1 : -1, mode,
+                 r2r_kind, f32, nullptr, stream, &launched);
 }
 
 pa_status pa_put_all_fft(pa_plan* plan, const void* src, void* const* peers, void* dst, unsigned flags,
                          void* stream) {
-  GUARD({ return put_all_fft(plan, nullptr, src, peers, dst, flags, stream, false); })
+  GUARD({ return put_all_fft(plan, nullptr, src, peers, dst, flags, stream, PutMode::fft); })
 }
 
 pa_status pa_put_all_rfft(pa_plan* plan, const pa_pencil* real, const void* src, void* const* peers,
                           void* dst, unsigned flags, void* stream) {
-  GUARD({ return put_all_fft(plan, real, src, peers, dst, flags, stream, true); })
+  GUARD({ return put_all_fft(plan, real, src, peers, dst, flags, stream, PutMode::rfft); })
+}
+
+pa_status pa_put_all_r2r(pa_plan* plan, int kind, const void* src, void* const* peers, void* dst,
+                         unsigned flags, void* stream) {
+  GUARD({ return put_all_fft(plan, nullptr, src, peers, dst, flags, stream, PutMode::r2r, kind); })
+}
+
+pa_status pa_put_all_brfft(pa_plan* plan, const pa_pencil* cplx, const void* src, void* const* peers,
+                           void* dst, unsigned flags, void* stream) {
+  GUARD({ return put_all_fft(plan, cplx, src, peers, dst, flags, stream, PutMode::brfft); })
+}
+
+pa_status pa_plan_real_put_check(const pa_plan* plan, unsigned flags) {
+  GUARD({
+    if (!plan) {
+      set_error("pa_plan_real_put_check: null plan");
+      return PA_EINVAL;
+    }
+    return plan_real_put_check(plan->p, (flags & PA_FFT_F32) != 0);
+  })
 }
 
 pa_status pa_plan_fft_put_check(const pa_plan* plan, unsigned flags) {

@@ -641,6 +641,40 @@ struct R2rParams {
   const void* tw4;  // W_4N^k: w_k = exp(-i pi k / 2N), k <= N/2
 };
 
+// The DCT-III pre-pass of the 01 kinds in place (r2r_tail, k_r2r_put): a thread owns the slots k
+// and L - k of its pair.  tw = W_N, tw4 = W_4N.
+template <int LOGL, int C, class T>
+__device__ __forceinline__ void r2r_pre(cplx_t<T>* sm, int pitch, int ncol, int t,
+                                        const typename Vec2<T>::type* twp,
+                                        const typename Vec2<T>::type* tw4p) {
+  using cx = cplx_t<T>;
+  using V = typename Vec2<T>::type;
+  constexpr int L = 1 << LOGL;
+  constexpr int P = L / 2 + 1;  // pairs (k, L - k) per line
+  auto twN = [twp](int k) {
+    const V w = __ldg(twp + k);
+    return cx{w.x, w.y};
+  };
+  auto w4 = [tw4p](int k) {  // w_k = W_4N^k
+    const V w = __ldg(tw4p + k);
+    return cx{w.x, w.y};
+  };
+#pragma unroll
+  for (int w0 = 0; w0 < C * P; w0 += FFT_THREADS) {
+    const int w = w0 + t, c = w / P, k = w % P;
+    if (w < C * P && c < ncol) {
+      cx* line = sm + c * pitch;
+      const cx vk = pa_fft::dct3_pre_pair(line[pa_fft::pad_index(k)], w4(k));
+      const cx vl = pa_fft::dct3_pre_pair(line[pa_fft::pad_index(L - k)], w4(L - k));
+      cx zk, zl;
+      pa_fft::brfft_pre_pair(k, vk, vl, twN(k), &zk, &zl);
+      line[pa_fft::pad_index(k)] = zk;
+      if (k > 0) line[pa_fft::pad_index(L - k)] = zl;
+    }
+  }
+  __syncthreads();
+}
+
 // k_r2r after its load (k_unpack_r2r runs it after its gather): the DCT-III pre-pass for the 01
 // kinds, the L-point passes, and the DCT-II post-pass and store (10 kinds) or the store of the N
 // reals (01 kinds) of line c at out(c).  tw = W_N, tw4 = W_4N.
@@ -665,23 +699,7 @@ __device__ __forceinline__ void r2r_tail(cplx_t<T>* sm, int pitch, int ncol, int
     return cx{w.x, w.y};
   };
 
-  if constexpr (!FWD) {
-    // ---- pre-pass in place: a thread owns the slots k and L - k of its pair ----
-#pragma unroll
-    for (int w0 = 0; w0 < C * P; w0 += FFT_THREADS) {
-      const int w = w0 + t, c = w / P, k = w % P;
-      if (w < C * P && c < ncol) {
-        cx* line = sm + c * pitch;
-        const cx vk = pa_fft::dct3_pre_pair(line[pa_fft::pad_index(k)], w4(k));
-        const cx vl = pa_fft::dct3_pre_pair(line[pa_fft::pad_index(L - k)], w4(L - k));
-        cx zk, zl;
-        pa_fft::brfft_pre_pair(k, vk, vl, twN(k), &zk, &zl);
-        line[pa_fft::pad_index(k)] = zk;
-        if (k > 0) line[pa_fft::pad_index(L - k)] = zl;
-      }
-    }
-    __syncthreads();
-  }
+  if constexpr (!FWD) r2r_pre<LOGL, C, T>(sm, pitch, ncol, t, twp, tw4p);
 
   fft_passes<LOGL, LOGL, C>(sm, pitch, ncol, FWD ? -1 : 1, twL);
 
@@ -724,12 +742,52 @@ __device__ __forceinline__ void r2r_tail(cplx_t<T>* sm, int pitch, int ncol, int
   }
 }
 
+// The load of k_r2r (k_r2r_put loads its lines with it too), linear as k_rfft's: the reals
+// (x[2m], x[2m+1]) of a line, one element per load, the RS threads of line c reading it from
+// src(c), reordered on their way into shared memory
+template <int LOGL, int C, bool FWD, class T, class Src>
+__device__ __forceinline__ void r2r_load(cplx_t<T>* sm, int pitch, int ncol, int t, bool sine,
+                                         const Src& src) {
+  using V = typename Vec2<T>::type;
+  constexpr int L = 1 << LOGL, N = 2 * L;
+  constexpr int RS = FFT_THREADS / C;  // threads per line
+  constexpr int U = (L + RS - 1) / RS;
+  const int c = t / RS, r = t % RS;
+  if (c < ncol) {
+    const V* s = src(c);
+    T* line = reinterpret_cast<T*>(sm + c * pitch);
+    V v[U];
+#pragma unroll
+    for (int q = 0; q < U; ++q)
+      if (r + q * RS < L) v[q] = __ldcs(s + r + q * RS);
+#pragma unroll
+    for (int q = 0; q < U; ++q) {
+      const int m = r + q * RS;
+      if (m < L) {
+        if constexpr (FWD) {
+          // DCT-II: v[m] = x[2m], v[N-1-m] = x[2m+1], v[i] the part i & 1 of complex slot i / 2.
+          // DST-II transforms (-1)^n x[n]
+          line[2 * pa_fft::pad_index(m >> 1) + (m & 1)] = v[q].x;
+          line[2 * pa_fft::pad_index((N - 1 - m) >> 1) + ((N - 1 - m) & 1)] = sine ? -v[q].y : v[q].y;
+        } else {
+          // DCT-III: slot j holds (X[j], X[N-j]), j = 0 ... L, as brfft_pre_pair's pairs do.
+          // DST-III transforms X reversed: X[2m] is then entry N-1-2m
+          const int ja = sine ? N - 1 - 2 * m : 2 * m, jb = sine ? N - 2 - 2 * m : 2 * m + 1;
+          if (ja <= L) line[2 * pa_fft::pad_index(ja)] = v[q].x;
+          if (ja >= L) line[2 * pa_fft::pad_index(N - ja) + 1] = v[q].x;
+          if (jb <= L) line[2 * pa_fft::pad_index(jb)] = v[q].y;
+          if (jb >= L) line[2 * pa_fft::pad_index(N - jb) + 1] = v[q].y;
+        }
+      }
+    }
+    if (!FWD && r == 0) line[1] = T(0);  // X[N] := 0 (slot 0)
+  }
+}
+
 template <int LOGL, int C, bool FWD, class T>
 __global__ void __launch_bounds__(FFT_THREADS) k_r2r(const __grid_constant__ R2rParams p) {
   using cx = cplx_t<T>;
   using V = typename Vec2<T>::type;
-  constexpr int L = 1 << LOGL, N = 2 * L;
-  constexpr int RS = FFT_THREADS / C;  // threads per line
   extern __shared__ __align__(16) unsigned char fft_smem[];
   cx* sm = reinterpret_cast<cx*>(fft_smem);
   const int t = threadIdx.x;
@@ -740,41 +798,10 @@ __global__ void __launch_bounds__(FFT_THREADS) k_r2r(const __grid_constant__ R2r
   const V* twp = reinterpret_cast<const V*>(p.tw);
   const V* tw4p = reinterpret_cast<const V*>(p.tw4);
 
-  // ---- load (linear gather, as k_rfft): the reals (x[2m], x[2m+1]) of a line, one element per
-  //      load, reordered on their way into shared memory ----
-  {
-    constexpr int U = (L + RS - 1) / RS;
-    const int c = t / RS, r = t % RS;
-    if (c < ncol) {
-      const V* s = reinterpret_cast<const V*>(p.src + (l0 + c) * p.line);
-      T* line = reinterpret_cast<T*>(sm + c * pitch);
-      V v[U];
-#pragma unroll
-      for (int q = 0; q < U; ++q)
-        if (r + q * RS < L) v[q] = __ldcs(s + r + q * RS);
-#pragma unroll
-      for (int q = 0; q < U; ++q) {
-        const int m = r + q * RS;
-        if (m < L) {
-          if constexpr (FWD) {
-            // DCT-II: v[m] = x[2m], v[N-1-m] = x[2m+1], v[i] the part i & 1 of complex slot i / 2.
-            // DST-II transforms (-1)^n x[n]
-            line[2 * pa_fft::pad_index(m >> 1) + (m & 1)] = v[q].x;
-            line[2 * pa_fft::pad_index((N - 1 - m) >> 1) + ((N - 1 - m) & 1)] = sine ? -v[q].y : v[q].y;
-          } else {
-            // DCT-III: slot j holds (X[j], X[N-j]), j = 0 ... L, as brfft_pre_pair's pairs do.
-            // DST-III transforms X reversed: X[2m] is then entry N-1-2m
-            const int ja = sine ? N - 1 - 2 * m : 2 * m, jb = sine ? N - 2 - 2 * m : 2 * m + 1;
-            if (ja <= L) line[2 * pa_fft::pad_index(ja)] = v[q].x;
-            if (ja >= L) line[2 * pa_fft::pad_index(N - ja) + 1] = v[q].x;
-            if (jb <= L) line[2 * pa_fft::pad_index(jb)] = v[q].y;
-            if (jb >= L) line[2 * pa_fft::pad_index(N - jb) + 1] = v[q].y;
-          }
-        }
-      }
-      if (!FWD && r == 0) line[1] = T(0);  // X[N] := 0 (slot 0)
-    }
-  }
+  // ---- load (linear gather, as k_rfft), reordered on its way into shared memory ----
+  r2r_load<LOGL, C, FWD, T>(sm, pitch, ncol, t, sine, [&p, l0](int c) {
+    return reinterpret_cast<const V*>(p.src + (l0 + c) * p.line);
+  });
   __syncthreads();
 
   r2r_tail<LOGL, C, FWD, T>(sm, pitch, ncol, t, sine, twp, tw4p,
@@ -909,17 +936,22 @@ __device__ __forceinline__ void put_done(const MultiFlags& mf) {
   }
 }
 
-// The destination of bin k of the CTA's lines: the block that owns it, at its CTA origin `base`
-// (every block is tried with a compile-time index, so `base` stays in registers)
-template <class T>
-__device__ __forceinline__ typename Vec2<T>::type* put_target(const FftPutParams& pp, char* const* base,
-                                                              int c, int k) {
+// The destination of element k (a bin; k_r2r_put / k_brfft_put: a real) of the CTA's line c: the
+// block that owns it, at its CTA origin `base` (every block is tried with a compile-time index, so
+// `base` stays in registers)
+template <class E>
+__device__ __forceinline__ E* put_at(const FftPutParams& pp, char* const* base, int c, int k) {
   char* o = nullptr;
 #pragma unroll
   for (int b = 0; b < FFT_MAXB; ++b)
     if (b < pp.nb && k >= pp.blk[b].y0 && k < pp.blk[b].y0 + pp.blk[b].ey)
       o = base[b] + (long long)(k - pp.blk[b].y0) * pp.blk[b].dsy + c * pp.blk[b].dsx;
-  return reinterpret_cast<typename Vec2<T>::type*>(o);
+  return reinterpret_cast<E*>(o);
+}
+template <class T>
+__device__ __forceinline__ typename Vec2<T>::type* put_target(const FftPutParams& pp, char* const* base,
+                                                              int c, int k) {
+  return put_at<typename Vec2<T>::type>(pp, base, c, k);
 }
 
 // Every block's origin for this CTA's first line: its outer offsets (from the CTA index, as
@@ -1021,6 +1053,159 @@ __global__ void __maxnreg__(128) k_rfft_put(const __grid_constant__ FftPutParams
                              &xk, &xl);
       __stcs(put_target<T>(pp, base, c, k), vec2(xk.x, xk.y));
       if (k != L - k) __stcs(put_target<T>(pp, base, c, L - k), vec2(xl.x, xl.y));
+    }
+  }
+  put_done(pp.mf);
+}
+
+// ---- send-side fused real line transforms + put (pa_r2r_put / pa_brfft_put, DESIGN §3j) ----
+// The plan moves REAL elements: N reals per line, the blocks tiling [0, N) at any boundary (32
+// reals over 3 ranks: 11 / 11 / 10), so every real is stored alone -- a pair (x[2m], x[2m+1]) may
+// straddle two blocks, and a block that starts at an odd real is only element-aligned.  The
+// across-lines pattern stores one real of C consecutive lines from C consecutive threads; the
+// along-the-line pattern one real per thread, consecutive threads on consecutive reals.
+
+// r2r: k_r2r's load (r2r_load), the DCT-III pre-pass (01 kinds), the L-point passes, then the
+// DCT-II post-pass (10 kinds) or the read-out of the N reals, every real stored into the block
+// that owns it.  p.L = N / 2, p.tw = W_N, p.tw4 = W_4N, p.sine.  Same lines per CTA and pitch as
+// k_r2r for that N and direction.
+template <int LOGL, int C, bool FWD, class T>
+__global__ void __maxnreg__(128) k_r2r_put(const __grid_constant__ FftPutParams pp) {
+  using cx = cplx_t<T>;
+  using V = typename Vec2<T>::type;
+  constexpr int L = 1 << LOGL, N = 2 * L;
+  constexpr int P = L / 2 + 1;  // pairs (k, L - k) per line
+  extern __shared__ __align__(16) unsigned char fft_smem[];
+  cx* sm = reinterpret_cast<cx*>(fft_smem);
+  const FftParams& p = pp.p;
+  const int t = threadIdx.x;
+  put_ready_signal(pp.mf);
+  long long so_off[FFT_MAXB], d_off;
+  const long long x0 = cta_offsets(p, C, so_off, &d_off);
+  const int ncol = (int)((p.ex - x0) < C ? (p.ex - x0) : C);
+  const int pitch = p.pitch;
+  const bool sine = p.sine != 0;
+  const V* twp = reinterpret_cast<const V*>(p.tw);
+  const V* tw4p = reinterpret_cast<const V*>(p.tw4);
+  r2r_load<LOGL, C, FWD, T>(sm, pitch, ncol, t, sine, [&p, &so_off, x0](int c) {
+    return reinterpret_cast<const V*>(p.blk[0].src + so_off[0] + (x0 + c) * p.blk[0].ssx);
+  });
+  __syncthreads();
+  auto twL = [twp](int i) {  // W_L^i = W_N^(2i)
+    const V w = __ldg(twp + 2 * i);
+    return cx{w.x, w.y};
+  };
+  if constexpr (!FWD) r2r_pre<LOGL, C, T>(sm, pitch, ncol, t, twp, tw4p);
+  fft_passes<LOGL, LOGL, C>(sm, pitch, ncol, FWD ? -1 : 1, twL);
+  put_ready_wait(pp.mf);
+
+  char* base[FFT_MAXB];
+  put_bases(pp, x0, base);
+  const bool across = pp.across != 0;
+  if constexpr (FWD) {
+    // ---- post-pass + store: the pair k yields Y[k], Y[N-k], Y[L-k] and Y[L+k] (r2r_tail's);
+    //      DST-II stores Y[j] at N-1-j ----
+    auto twN = [twp](int k) {
+      const V w = __ldg(twp + k);
+      return cx{w.x, w.y};
+    };
+    auto w4 = [tw4p](int k) {  // w_k = W_4N^k
+      const V w = __ldg(tw4p + k);
+      return cx{w.x, w.y};
+    };
+    for (int w0 = 0; w0 < C * P; w0 += FFT_THREADS) {
+      const int w = w0 + t;
+      const int c = across ? (w & (C - 1)) : (w / P), k = across ? (w / C) : (w % P);
+      if (w < C * P && c < ncol) {
+        const cx* line = sm + c * pitch;
+        cx vk, vl;
+        pa_fft::rfft_post_pair(line[pa_fft::pad_index(fft_pos<LOGL, LOGL>(k & (L - 1)))],
+                               line[pa_fft::pad_index(fft_pos<LOGL, LOGL>((L - k) & (L - 1)))], twN(k),
+                               &vk, &vl);
+        T yk, ynk, yl, ynl;
+        pa_fft::dct2_post_pair(vk, w4(k), &yk, &ynk);      // Y[k], Y[N-k]
+        pa_fft::dct2_post_pair(vl, w4(L - k), &yl, &ynl);  // Y[L-k], Y[L+k]
+        auto put = [&](int j, T y) { __stcs(put_at<T>(pp, base, c, sine ? N - 1 - j : j), y); };
+        put(k, yk);
+        if (k > 0 && k < L / 2) put(N - k, ynk);
+        if (k < L / 2) put(L - k, yl);
+        if (k > 0) put(L + k, ynl);
+      }
+    }
+  } else {
+    // ---- store: x[2m] = v[m], x[2m+1] = v[N-1-m]; DST-III: times (-1)^n ----
+    for (int w0 = 0; w0 < C * N; w0 += FFT_THREADS) {
+      const int w = w0 + t;
+      const int c = across ? (w & (C - 1)) : (w >> (LOGL + 1)), n = across ? (w / C) : (w & (N - 1));
+      if (w < C * N && c < ncol) {
+        const T* line = reinterpret_cast<const T*>(sm + c * pitch);
+        const int i = (n & 1) ? N - 1 - (n >> 1) : (n >> 1);
+        const T v = line[2 * pa_fft::pad_index(fft_pos<LOGL, LOGL>(i >> 1)) + (i & 1)];
+        __stcs(put_at<T>(pp, base, c, n), (sine && (n & 1)) ? -v : v);
+      }
+    }
+  }
+  put_done(pp.mf);
+}
+
+// c2r: k_rfft's backward load (rfft_load, the N/2 + 1 bins), its pre-pass and its L-point passes,
+// then the N reals z[n] = x[2n] + i x[2n+1] of a line stored into the blocks that own them.  The
+// source is the complex counterpart of the plan's real one; p.L = N / 2, p.tw = W_N.
+template <int LOGL, int C, class T>
+__global__ void __maxnreg__(128) k_brfft_put(const __grid_constant__ FftPutParams pp) {
+  using cx = cplx_t<T>;
+  using V = typename Vec2<T>::type;
+  constexpr int L = 1 << LOGL, N = 2 * L;
+  constexpr int P = L / 2 + 1;  // pairs (k, L - k) per line
+  extern __shared__ __align__(16) unsigned char fft_smem[];
+  cx* sm = reinterpret_cast<cx*>(fft_smem);
+  const FftParams& p = pp.p;
+  const int t = threadIdx.x;
+  put_ready_signal(pp.mf);
+  long long so_off[FFT_MAXB], d_off;
+  const long long x0 = cta_offsets(p, C, so_off, &d_off);
+  const int ncol = (int)((p.ex - x0) < C ? (p.ex - x0) : C);
+  const int pitch = p.pitch;
+  rfft_load<LOGL, C, false, T>(sm, pitch, ncol, t, [&p, &so_off, x0](int c) {
+    return reinterpret_cast<const V*>(p.blk[0].src + so_off[0] + (x0 + c) * p.blk[0].ssx);
+  });
+  __syncthreads();
+  const V* twp = reinterpret_cast<const V*>(p.tw);
+  auto twN = [twp](int k) {
+    const V w = __ldg(twp + k);
+    return cx{w.x, w.y};
+  };
+  auto twL = [twp](int i) {  // W_L^i = W_N^(2i)
+    const V w = __ldg(twp + 2 * i);
+    return cx{w.x, w.y};
+  };
+  // ---- pre-pass in place (k_rfft<..., false>): a thread owns the slots k and L - k ----
+#pragma unroll
+  for (int w0 = 0; w0 < C * P; w0 += FFT_THREADS) {
+    const int w = w0 + t, c = w / P, k = w % P;
+    if (w < C * P && c < ncol) {
+      cx* line = sm + c * pitch;
+      cx zk, zl;
+      pa_fft::brfft_pre_pair(k, line[pa_fft::pad_index(k)], line[pa_fft::pad_index(L - k)], twN(k),
+                             &zk, &zl);
+      line[pa_fft::pad_index(k)] = zk;
+      if (k > 0) line[pa_fft::pad_index(L - k)] = zl;
+    }
+  }
+  __syncthreads();
+  fft_passes<LOGL, LOGL, C>(sm, pitch, ncol, 1, twL);
+  put_ready_wait(pp.mf);
+
+  // ---- store: real n of line c is part n & 1 of complex slot n / 2 ----
+  char* base[FFT_MAXB];
+  put_bases(pp, x0, base);
+  const bool across = pp.across != 0;
+  for (int w0 = 0; w0 < C * N; w0 += FFT_THREADS) {
+    const int w = w0 + t;
+    const int c = across ? (w & (C - 1)) : (w >> (LOGL + 1)), n = across ? (w / C) : (w & (N - 1));
+    if (w < C * N && c < ncol) {
+      const T* line = reinterpret_cast<const T*>(sm + c * pitch);
+      __stcs(put_at<T>(pp, base, c, n), line[2 * pa_fft::pad_index(fft_pos<LOGL, LOGL>(n >> 1)) + (n & 1)]);
     }
   }
   put_done(pp.mf);
@@ -1427,11 +1612,17 @@ pa_status get_fft(int nb, const BlockCopy* const* blocks, const void* const* src
 // rfft: the plan is the COMPLEX plan of M bins per line, and `src` the REAL array of N reals per
 // line that replaces its source (same layout otherwise): the source offsets and strides, multiples
 // of M, are rescaled to N reals -- brfft's destination rescale, mirrored.
+// r2r / brfft: the plan is the REAL plan of M = N reals per line (the blocks may split it at any
+// real).  r2r: `src` is its source.  brfft: `src` is the COMPLEX array of N/2 + 1 bins per line
+// that replaces it, the source offsets and strides rescaled from N reals to N/2 + 1 bins.  Both
+// require those offsets and strides to be multiples of N, so one verdict serves both.
 static pa_status put_fft_geometry(int nb, const BlockCopy* const* blocks, const void* src,
-                                  void* const* dsts, bool f32, bool rfft, FftPutParams& pp, int* C_out,
+                                  void* const* dsts, bool f32, PutMode mode, FftPutParams& pp, int* C_out,
                                   unsigned long long* grid_out) {
-  const char* what = rfft ? "fused rfft + put" : "fused FFT + put";
-  const i64 es = f32 ? 8 : 16;  // complex element bytes (the plan's elements)
+  const bool rfft = mode == PutMode::rfft;
+  const bool real = mode == PutMode::r2r || mode == PutMode::brfft;  // the plan moves reals
+  const char* what = real ? "fused real transform + put" : rfft ? "fused rfft + put" : "fused FFT + put";
+  const i64 es = real ? (f32 ? 4 : 8) : (f32 ? 8 : 16);  // the plan's element bytes
   memset(&pp, 0, sizeof pp);
   *grid_out = 0;
   const BlockCopy* ref = nullptr;
@@ -1440,8 +1631,12 @@ static pa_status put_fft_geometry(int nb, const BlockCopy* const* blocks, const 
     const BlockCopy& B = *blocks[b];
     if (B.count == 0) continue;
     if (B.elsize != es) {
-      set_error(f32 ? "%s: PA_FFT_F32 takes ComplexF32 (8-byte) elements only"
-                    : "%s: ComplexF64 (16-byte) elements only", what);
+      if (real)
+        set_error(f32 ? "%s: PA_FFT_F32 takes Float32 (4-byte) elements only"
+                      : "%s: Float64 (8-byte) elements only", what);
+      else
+        set_error(f32 ? "%s: PA_FFT_F32 takes ComplexF32 (8-byte) elements only"
+                      : "%s: ComplexF64 (16-byte) elements only", what);
       return PA_EINVAL;
     }
     if (B.raw[0].ss != 1) {
@@ -1476,13 +1671,16 @@ static pa_status put_fft_geometry(int nb, const BlockCopy* const* blocks, const 
     F.dsy = B.raw[0].ds * es;
     M += B.raw[0].e;
   }
-  const i64 L = rfft ? M - 1 : M;  // rfft: the N/2-point complex FFT of a real line of N = 2 (M - 1)
+  // rfft: the N/2-point complex FFT of a real line of N = 2 (M - 1); r2r / brfft: of N = M reals
+  const i64 L = rfft ? M - 1 : real ? M / 2 : M;
   int logL = 0;
   while ((1LL << logL) < L) ++logL;
-  if ((1LL << logL) != L || L < 8 || L > 1024) {
+  if ((1LL << logL) != L || L < 8 || L > 1024 || (real && 2 * L != M)) {
     if (rfft)
       set_error("%s: %lld bins per line are not N/2+1 with N a power of two in 16..2048", what,
                 (long long)M);
+    else if (real)
+      set_error("%s: line length N = %lld is not a power of two in 16..2048", what, (long long)M);
     else
       set_error("%s: line length %lld is not a power of two in 8..1024", what, (long long)L);
     return PA_EINVAL;
@@ -1515,19 +1713,24 @@ static pa_status put_fft_geometry(int nb, const BlockCopy* const* blocks, const 
   for (int i = 1; i < ref->nd_raw && jx < 0; ++i)
     if (ref->raw[i].e > 1) jx = i;
   // source offsets and strides: complex elements, or (rfft) multiples of M bins that become
-  // multiples of N reals
-  const i64 N = 2 * L, rs = es / 2;
+  // multiples of N reals, or (r2r / brfft) multiples of N reals that stay reals (r2r) or become
+  // multiples of N/2 + 1 bins (brfft)
+  const i64 N = 2 * L, rs = real ? es : es / 2, Mc = L + 1;
   auto src_bytes = [&](long long off, long long* out) {
-    if (!rfft) {
+    if (!rfft && !real) {
       *out = off * es;
       return true;
     }
     if (off % M != 0) {
-      set_error("%s: a source stride or offset is not a multiple of the %lld bins of a line", what,
-                (long long)M);
+      if (rfft)
+        set_error("%s: a source stride or offset is not a multiple of the %lld bins of a line", what,
+                  (long long)M);
+      else
+        set_error("%s: a source stride or offset is not a multiple of the %lld reals of a line", what,
+                  (long long)M);
       return false;
     }
-    *out = off / M * N * rs;
+    *out = rfft ? off / M * N * rs : mode == PutMode::brfft ? off / M * Mc * 2 * rs : off * rs;
     return true;
   };
   FftParams& p = pp.p;
@@ -1538,8 +1741,8 @@ static pa_status put_fft_geometry(int nb, const BlockCopy* const* blocks, const 
   S.src = src ? (const char*)src + v : nullptr;
   S.y0 = 0;
   S.ey = (int)L;
-  S.ssy = rfft ? 2 * rs : es;
-  S.ssx = rfft ? N * rs : L * es;
+  S.ssy = (rfft || real) ? 2 * rs : es;
+  S.ssx = mode == PutMode::brfft ? Mc * 2 * rs : (rfft || real) ? N * rs : L * es;
   if (jx >= 0 && !src_bytes(ref->raw[jx].ss, &S.ssx)) return PA_EINVAL;
   for (int i = 1; i < ref->nd_raw; ++i)
     if (i != jx && ref->raw[i].e > 1) {
@@ -1564,10 +1767,12 @@ static pa_status put_fft_geometry(int nb, const BlockCopy* const* blocks, const 
   p.ex = jx >= 0 ? ref->raw[jx].e : 1;
   p.L = (int)L;
   p.logL = logL;
-  p.pitch = pa_fft::padded_pitch((int)L);  // fft_ / k_rfft (forward): L points per shared line
-  // the lines per CTA of fft_ (tunable fft_lines included) / of k_rfft
+  // fft_ / k_rfft (forward) / k_r2r (10 kinds): L points per shared line; k_rfft (backward) and
+  // k_r2r (01 kinds) stage the L + 1 slots, which put_fft sets
+  p.pitch = pa_fft::padded_pitch((int)L);
+  // the lines per CTA of fft_ (tunable fft_lines included) / of k_rfft and k_r2r
   const int C = f32 ? fft_lines_f32(logL)
-                    : ((!rfft && g_tun.fft_lines == 4 && logL >= 8) ? 4 : fft_lines(logL));
+                    : ((mode == PutMode::fft && g_tun.fft_lines == 4 && logL >= 8) ? 4 : fft_lines(logL));
   p.tiles_x = (unsigned)((p.ex + C - 1) / C);
   unsigned long long grid = p.tiles_x;
   for (int i = 0; i < p.no; ++i) grid *= (unsigned long long)p.oe[i];
@@ -1581,20 +1786,30 @@ static pa_status put_fft_geometry(int nb, const BlockCopy* const* blocks, const 
 }
 
 pa_status put_fft(int nb, const BlockCopy* const* blocks, const void* src, void* const* dsts, int sign,
-                  bool rfft, bool f32, const MultiFlags* mf, void* stream, bool* launched) {
-  // (the entry points have already asked plan_fft_put_check / plan_rfft_put_check)
+                  PutMode mode, int r2r_kind, bool f32, const MultiFlags* mf, void* stream, bool* launched) {
+  // (the entry points have already asked plan_fft_put_check / plan_rfft_put_check /
+  //  plan_real_put_check)
   *launched = false;
   FftPutParams pp;
   int C = 0;
   unsigned long long grid = 0;
-  pa_status s = put_fft_geometry(nb, blocks, src, dsts, f32, rfft, pp, &C, &grid);
+  pa_status s = put_fft_geometry(nb, blocks, src, dsts, f32, mode, pp, &C, &grid);
   if (s != PA_OK || grid == 0) return s;
   if (mf) pp.mf = *mf;
   FftParams& p = pp.p;
   const int logL = p.logL;
+  const bool rfft = mode == PutMode::rfft;
+  // r2r: the 10 kinds run k_r2r's forward path, the 01 kinds its backward one
+  const bool r2r_fwd = r2r_kind == PA_REDFT10 || r2r_kind == PA_RODFT10;
   p.sign = rfft ? -1 : (sign < 0 ? -1 : 1);
-  p.tw = twiddles(rfft ? 2 * p.L : p.L, f32);
-  if (!p.tw) {
+  p.tw = twiddles(mode == PutMode::fft ? p.L : 2 * p.L, f32);
+  if (mode == PutMode::r2r) {
+    p.sine = (r2r_kind == PA_RODFT10 || r2r_kind == PA_RODFT01) ? 1 : 0;
+    p.tw4 = twiddles(8 * p.L, f32);
+  }
+  // k_rfft (backward) and k_r2r (01 kinds) stage the pairs of slots 0..L
+  if (mode == PutMode::brfft || (mode == PutMode::r2r && !r2r_fwd)) p.pitch = pa_fft::padded_pitch(p.L + 1);
+  if (!p.tw || (mode == PutMode::r2r && !p.tw4)) {
     set_error("fused put: twiddle table allocation failed");
     cudaGetLastError();
     return PA_ENOMEM;
@@ -1609,36 +1824,46 @@ pa_status put_fft(int nb, const BlockCopy* const* blocks, const void* src, void*
     kern<<<(unsigned)grid, FFT_THREADS, smem, (cudaStream_t)stream>>>(pp);
     e = cudaGetLastError();
   };
-  auto launch_mode = [&](auto fft_kern, auto rfft_kern) { rfft ? launch(rfft_kern) : launch(fft_kern); };
+  // the kernels of one line length and lines per CTA, by mode (and r2r direction)
+#define PUT_KERNELS(LG, CC, T)                                                                   \
+  switch (mode) {                                                                                \
+    case PutMode::fft: launch(k_fft_put<LG, CC, T>); break;                                      \
+    case PutMode::rfft: launch(k_rfft_put<LG, CC, T>); break;                                    \
+    case PutMode::r2r:                                                                           \
+      r2r_fwd ? launch(k_r2r_put<LG, CC, true, T>) : launch(k_r2r_put<LG, CC, false, T>);        \
+      break;                                                                                     \
+    case PutMode::brfft: launch(k_brfft_put<LG, CC, T>); break;                                  \
+  }
   if (f32) {
     switch (logL) {
-      case 3: launch_mode(k_fft_put<3, 16, float>, k_rfft_put<3, 16, float>); break;
-      case 4: launch_mode(k_fft_put<4, 16, float>, k_rfft_put<4, 16, float>); break;
-      case 5: launch_mode(k_fft_put<5, 16, float>, k_rfft_put<5, 16, float>); break;
-      case 6: launch_mode(k_fft_put<6, 16, float>, k_rfft_put<6, 16, float>); break;
-      case 7: launch_mode(k_fft_put<7, 16, float>, k_rfft_put<7, 16, float>); break;
-      case 8: launch_mode(k_fft_put<8, 16, float>, k_rfft_put<8, 16, float>); break;
-      case 9: launch_mode(k_fft_put<9, 16, float>, k_rfft_put<9, 16, float>); break;
-      default: launch_mode(k_fft_put<10, 8, float>, k_rfft_put<10, 8, float>); break;
+      case 3: PUT_KERNELS(3, 16, float) break;
+      case 4: PUT_KERNELS(4, 16, float) break;
+      case 5: PUT_KERNELS(5, 16, float) break;
+      case 6: PUT_KERNELS(6, 16, float) break;
+      case 7: PUT_KERNELS(7, 16, float) break;
+      case 8: PUT_KERNELS(8, 16, float) break;
+      case 9: PUT_KERNELS(9, 16, float) break;
+      default: PUT_KERNELS(10, 8, float) break;
     }
   } else {
     switch (logL) {
-      case 3: launch_mode(k_fft_put<3, 8, double>, k_rfft_put<3, 8, double>); break;
-      case 4: launch_mode(k_fft_put<4, 8, double>, k_rfft_put<4, 8, double>); break;
-      case 5: launch_mode(k_fft_put<5, 8, double>, k_rfft_put<5, 8, double>); break;
-      case 6: launch_mode(k_fft_put<6, 8, double>, k_rfft_put<6, 8, double>); break;
-      case 7: launch_mode(k_fft_put<7, 8, double>, k_rfft_put<7, 8, double>); break;
+      case 3: PUT_KERNELS(3, 8, double) break;
+      case 4: PUT_KERNELS(4, 8, double) break;
+      case 5: PUT_KERNELS(5, 8, double) break;
+      case 6: PUT_KERNELS(6, 8, double) break;
+      case 7: PUT_KERNELS(7, 8, double) break;
       case 8:
-        if (C == 4) launch(k_fft_put<8, 4, double>);
-        else launch_mode(k_fft_put<8, 8, double>, k_rfft_put<8, 8, double>);
+        if (C == 4) launch(k_fft_put<8, 4, double>);  // (tunable fft_lines = 4: the complex FFT only)
+        else PUT_KERNELS(8, 8, double)
         break;
       case 9:
         if (C == 4) launch(k_fft_put<9, 4, double>);
-        else launch_mode(k_fft_put<9, 8, double>, k_rfft_put<9, 8, double>);
+        else PUT_KERNELS(9, 8, double)
         break;
-      default: launch_mode(k_fft_put<10, 4, double>, k_rfft_put<10, 4, double>); break;
+      default: PUT_KERNELS(10, 4, double) break;
     }
   }
+#undef PUT_KERNELS
   if (e != cudaSuccess) {
     set_error("fused put kernel launch failed: %s", cudaGetErrorString(e));
     return PA_ECUDA;
@@ -1957,13 +2182,20 @@ pa_status plan_real_check(Plan* P, bool f32) {
   return P->real_check[q];
 }
 
-// Can pa_fft_put (rfft: pa_rfft_put) run on this plan?  The send-side kernel runs on PeerPut plans
-// and on local transposes (no exchange, or a line of one rank) of any method.  As fused_check,
-// every rank of the grid line gets the same answer: its plan is rebuilt and its blocks -- the
-// self block and the put blocks -- checked.
-static pa_status put_check(Plan* P, bool f32, bool rfft) {
-  const char* what = rfft ? "fused rfft + put" : "fused FFT + put";
-  if (P->elsize != (f32 ? 8 : 16)) {
+// Can pa_fft_put (rfft: pa_rfft_put; brfft: pa_r2r_put and pa_brfft_put) run on this plan?  The
+// send-side kernel runs on PeerPut plans and on local transposes (no exchange, or a line of one
+// rank) of any method.  As fused_check, every rank of the grid line gets the same answer: its plan
+// is rebuilt and its blocks -- the self block and the put blocks -- checked.
+static pa_status put_check(Plan* P, bool f32, PutMode mode) {
+  const bool real = mode == PutMode::r2r || mode == PutMode::brfft;
+  const char* what = real ? "fused real transform + put"
+                          : mode == PutMode::rfft ? "fused rfft + put" : "fused FFT + put";
+  if (real && P->elsize != (f32 ? 4 : 8)) {
+    set_error(f32 ? "%s: PA_FFT_F32 takes a Float32 (elsize 4) plan"
+                  : "%s: a Float64 (elsize 8) plan, or PA_FFT_F32 for Float32", what);
+    return PA_EINVAL;
+  }
+  if (!real && P->elsize != (f32 ? 8 : 16)) {
     set_error(f32 ? "%s: PA_FFT_F32 takes a ComplexF32 (elsize 8) plan"
                   : "%s: a ComplexF64 (elsize 16) plan, or PA_FFT_F32 for ComplexF32", what);
     return PA_EINVAL;
@@ -1980,12 +2212,17 @@ static pa_status put_check(Plan* P, bool f32, bool rfft) {
   unsigned long long grid = 0;
   if (P->dim < 0 || P->nproc == 1) {
     const BlockCopy* b = &P->self_fused;
-    return put_fft_geometry(1, &b, nullptr, nullptr, f32, rfft, pp, &C, &grid);
+    return put_fft_geometry(1, &b, nullptr, nullptr, f32, mode, pp, &C, &grid);
   }
   if (P->method != PA_PEER_PUT) {
-    set_error("%s: the send-side fusion needs PeerPut (or a local transposition); with "
-              "PointToPoint, Alltoallv or PeerGet transform src first and fuse the next transform "
-              "into the receive side (pa_transpose with PA_FFT_FORWARD / PA_FFT_BACKWARD)", what);
+    if (real)
+      set_error("%s: the send-side fusion needs PeerPut (or a local transposition); with "
+                "PointToPoint, Alltoallv or PeerGet transform src first and fuse the next transform "
+                "into the receive side (pa_transpose_r2r, pa_transpose_rfft, pa_transpose_brfft)", what);
+    else
+      set_error("%s: the send-side fusion needs PeerPut (or a local transposition); with "
+                "PointToPoint, Alltoallv or PeerGet transform src first and fuse the next transform "
+                "into the receive side (pa_transpose with PA_FFT_FORWARD / PA_FFT_BACKWARD)", what);
     return PA_EINVAL;
   }
   for (int n = 0; n < P->nproc; ++n) {
@@ -1996,7 +2233,7 @@ static pa_status put_check(Plan* P, bool f32, bool rfft) {
     std::vector<const BlockCopy*> bl;
     for (int k = 0; k < Q->nproc; ++k)
       bl.push_back(k == Q->self_index ? &Q->self_fused : &Q->peers[k].put);
-    s = put_fft_geometry(Q->nproc, bl.data(), nullptr, nullptr, f32, rfft, pp, &C, &grid);
+    s = put_fft_geometry(Q->nproc, bl.data(), nullptr, nullptr, f32, mode, pp, &C, &grid);
     if (s != PA_OK) {
       if (n != P->self_index) {
         const std::string why = last_error();
@@ -2013,7 +2250,7 @@ static pa_status put_check(Plan* P, bool f32, bool rfft) {
 pa_status plan_fft_put_check(Plan* P, bool f32) {
   const int q = f32 ? 1 : 0;
   if (P->fft_put_check_lines[q] != g_tun.fft_lines) {
-    P->fft_put_check[q] = put_check(P, f32, false);
+    P->fft_put_check[q] = put_check(P, f32, PutMode::fft);
     P->fft_put_check_err[q] = P->fft_put_check[q] == PA_OK ? std::string() : std::string(last_error());
     P->fft_put_check_lines[q] = g_tun.fft_lines;
   } else if (P->fft_put_check[q] != PA_OK) {
@@ -2026,13 +2263,27 @@ pa_status plan_fft_put_check(Plan* P, bool f32) {
 pa_status plan_rfft_put_check(Plan* P, bool f32) {
   const int q = f32 ? 1 : 0;
   if (!P->rfft_put_checked[q]) {
-    P->rfft_put_check[q] = put_check(P, f32, true);
+    P->rfft_put_check[q] = put_check(P, f32, PutMode::rfft);
     P->rfft_put_check_err[q] = P->rfft_put_check[q] == PA_OK ? std::string() : std::string(last_error());
     P->rfft_put_checked[q] = true;
   } else if (P->rfft_put_check[q] != PA_OK) {
     set_error("%s", P->rfft_put_check_err[q].c_str());
   }
   return P->rfft_put_check[q];
+}
+
+// One verdict for pa_r2r_put and pa_brfft_put (the brfft geometry checks all that r2r's does, and
+// its rescale); cached per plan and per precision, apart from every other verdict.
+pa_status plan_real_put_check(Plan* P, bool f32) {
+  const int q = f32 ? 1 : 0;
+  if (!P->real_put_checked[q]) {
+    P->real_put_check[q] = put_check(P, f32, PutMode::brfft);
+    P->real_put_check_err[q] = P->real_put_check[q] == PA_OK ? std::string() : std::string(last_error());
+    P->real_put_checked[q] = true;
+  } else if (P->real_put_check[q] != PA_OK) {
+    set_error("%s", P->real_put_check_err[q].c_str());
+  }
+  return P->real_put_check[q];
 }
 
 pa_status rfft_lines(int N, bool forward, bool f32, i64 nlines, const void* src, void* dst,

@@ -242,6 +242,10 @@ struct Plan {
   bool rfft_put_checked[2] = {false, false};
   pa_status rfft_put_check[2] = {PA_OK, PA_OK};
   std::string rfft_put_check_err[2];
+  // cached answers of plan_real_put_check, [0] Float64 and [1] Float32 (PA_FFT_F32)
+  bool real_put_checked[2] = {false, false};
+  pa_status real_put_check[2] = {PA_OK, PA_OK};
+  std::string real_put_check_err[2];
   ~Plan();
 };
 
@@ -327,24 +331,36 @@ pa_status unpack_rfft(int nb, const BlockCopy* const* blocks, const void* const*
 // plan_fft_check's question for unpack_r2r and unpack_rfft (one verdict for both); its own
 // cache, the same uniformity over the line
 pa_status plan_real_check(Plan* plan, bool f32);
-// send-side fused transform + put (fft.cu, k_fft_put / k_rfft_put): the transform along the
-// first memory dim of the local `src`, every output bin stored into the block that owns it.
-// blocks[i] / dsts[i]: the self block (self_fused) into the local dst, the put block of every
-// other rank into that rank's dst as mapped here.  rfft: the plan is the complex plan of N/2 + 1
-// bins per line and `src` the real array of N reals per line; else sign -1 forward, +1 backward.
-// `mf` (NULL: none): the window protocol spoken inside the launch.  *launched = false: this rank
-// has no source lines and nothing was launched -- the caller then speaks the protocol with flag
-// kernels
+// What the send-side fused put of a transposition computes from the source lines.  The plan moves
+// dst's elements; src is the counterpart of the plan's source with the other element type
+enum class PutMode {
+  fft,    // the complex FFT (pa_fft_put): a complex plan, src complex
+  rfft,   // N reals -> N/2 + 1 bins (pa_rfft_put): a complex plan, src the real counterpart
+  r2r,    // N reals -> N reals, a DCT / DST (pa_r2r_put): a real plan, src real
+  brfft,  // N/2 + 1 bins -> N reals (pa_brfft_put): a real plan, src the complex counterpart
+};
+
+// send-side fused transform + put (fft.cu, k_fft_put / k_rfft_put / k_r2r_put / k_brfft_put): the
+// transform along the first memory dim of the local `src`, every output element stored into the
+// block that owns it.  blocks[i] / dsts[i]: the self block (self_fused) into the local dst, the put
+// block of every other rank into that rank's dst as mapped here.  fft: sign -1 forward, +1
+// backward; r2r: r2r_kind one of PA_REDFT10 / PA_REDFT01 / PA_RODFT10 / PA_RODFT01.  `mf` (NULL:
+// none): the window protocol spoken inside the launch.  *launched = false: this rank has no source
+// lines and nothing was launched -- the caller then speaks the protocol with flag kernels
 pa_status put_fft(int nb, const BlockCopy* const* blocks, const void* src, void* const* dsts, int sign,
-                  bool rfft, bool f32, const MultiFlags* mf, void* stream, bool* launched);
-// can put_fft run the complex FFT (rfft: the r2c transform) on this plan?  PeerPut plans and local
-// transposes only; the same answer on every rank of the grid line; own caches.  No device call.
+                  PutMode mode, int r2r_kind, bool f32, const MultiFlags* mf, void* stream,
+                  bool* launched);
+// can put_fft run the complex FFT (rfft: the r2c transform; real: r2r and brfft, one verdict) on
+// this plan?  PeerPut plans and local transposes only; the same answer on every rank of the grid
+// line; own caches.  No device call.
 pa_status plan_fft_put_check(Plan* plan, bool f32);
 pa_status plan_rfft_put_check(Plan* plan, bool f32);
-// dst = transpose(fft_(src)) (rfft: transpose(rfft_(src)), src the real array) on the caller's
-// stream (local plans) or PeerPut's one-sided schedule; every argument has been checked
+pa_status plan_real_put_check(Plan* plan, bool f32);
+// dst = transpose(T(src)), T the transform of `mode` (fft: its direction from flags; r2r: kind
+// r2r_kind), on the caller's stream (local plans) or PeerPut's one-sided schedule; every argument
+// has been checked
 pa_status transpose_put_fft(Plan* plan, Comm* comm, const void* src, void* dst, unsigned flags,
-                            bool rfft, void* stream);
+                            PutMode mode, int r2r_kind, void* stream);
 // real-line transforms (fft.cu): `nlines` dense, consecutive lines of N reals (src when forward,
 // dst when backward) <-> N/2 + 1 complex bins; N a power of two in 16..2048.  f32: Float32 <->
 // ComplexF32, else Float64 <-> ComplexF64

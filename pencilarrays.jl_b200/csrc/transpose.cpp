@@ -669,8 +669,6 @@ static BlockCopy contiguous_block(i64 bytes, const void* src, const void* dst) {
 }
 
 // ---- the one-sided methods --------------------------------------------------------
-// the send-side fused transform a PeerPut schedule runs in place of its put kernels
-enum class SendFft { none, fft, rfft };
 
 // PeerPut: each remote block is read from `src` and stored, already permuted,
 // into the destination rank's `dest` through its peer mapping.  PeerGet is the
@@ -681,15 +679,16 @@ enum class SendFft { none, fft, rfft };
 // fft_sign != 0 (PeerGet only): the fused gather + FFT (k_get_fft) replaces the get kernel and
 // the self block -- ONE kernel reads every line from the peers' src and the local src,
 // transforms and stores it; the protocol around it is the same.
-// send != none (PeerPut only): the send-side fused transform (k_fft_put / k_rfft_put) replaces
-// the put kernel and the self block -- ONE kernel loads every local source line, transforms it
-// and stores its bins into the local dst and the peers' dst (fft_sign: the FFT's direction).
+// send != NULL (PeerPut only): the send-side fused transform of mode *send (k_fft_put,
+// k_rfft_put, k_r2r_put, k_brfft_put) replaces the put kernel and the self block -- ONE kernel
+// loads every local source line, transforms it and stores its outputs into the local dst and the
+// peers' dst (fft_sign: the FFT's direction; r2r_kind: the DCT / DST).
 static pa_status one_sided(Plan* P, Comm* comm, const void* src, void* dst, unsigned flags,
-                           int fft_sign, SendFft send, cudaStream_t user) {
+                           int fft_sign, const PutMode* send, int r2r_kind, cudaStream_t user) {
   TransposeState& S = *P->st;
   const int nproc = P->nproc, me = P->self_index;
   const bool get = P->method == PA_PEER_GET;
-  const bool fft = fft_sign != 0 || send != SendFft::none;  // one fused kernel replaces the blocks
+  const bool fft = fft_sign != 0 || send;  // one fused kernel replaces the blocks
   const bool timing = S.timing;
   // (a rank none of whose peers owns anything has no window to register: nothing will be
   //  put / got, but it still speaks the protocol)
@@ -748,8 +747,8 @@ static pa_status one_sided(Plan* P, Comm* comm, const void* src, void* dst, unsi
   }
   auto fused = [&](const MultiFlags* mf, bool* launched) {
     const bool f32 = (flags & PA_FFT_F32) != 0;
-    if (send != SendFft::none)
-      return put_fft(nproc, fb.data(), src, fd.data(), fft_sign, send == SendFft::rfft, f32, mf, S.comm_s,
+    if (send)
+      return put_fft(nproc, fb.data(), src, fd.data(), fft_sign, *send, r2r_kind, f32, mf, S.comm_s,
                      launched);
     return get_fft(nproc, fb.data(), fs.data(), dst, fft_sign, f32, mf, S.comm_s, launched);
   };
@@ -1289,26 +1288,26 @@ pa_status transpose(Plan* P, Comm* comm, const void* src, void* dst, unsigned fl
     CU(cudaStreamWaitEvent(s, buf_ev, 0));
     CU(cudaStreamWaitEvent(s, buf_unpack_ev, 0));
   }
-  if (one) return one_sided(P, comm, src, dst, flags, fft_sign, SendFft::none, user);
+  if (one) return one_sided(P, comm, src, dst, flags, fft_sign, nullptr, 0, user);
   return staged(P, comm, src, dst, flags, mode, r2r_kind, stage_self, user, buf_ev, buf_unpack_ev);
 }
 
-pa_status transpose_put_fft(Plan* P, Comm* comm, const void* src, void* dst, unsigned flags, bool rfft,
-                            void* stream) {
-  // (pa_fft_put / pa_rfft_put have checked the flags, the arrays and the plan's verdict, which
-  //  admits PeerPut plans and local transposes only)
+pa_status transpose_put_fft(Plan* P, Comm* comm, const void* src, void* dst, unsigned flags, PutMode mode,
+                            int r2r_kind, void* stream) {
+  // (pa_fft_put / pa_rfft_put / pa_r2r_put / pa_brfft_put have checked the flags, the arrays and
+  //  the plan's verdict, which admits PeerPut plans and local transposes only)
   RC(ensure_state(P));
   TransposeState& S = *P->st;
   cudaStream_t user = (cudaStream_t)stream;
   const bool timing = S.timing;
-  const int sign = rfft || (flags & PA_FFT_FORWARD) ? -1 : 1;
+  const int sign = mode != PutMode::fft || (flags & PA_FFT_FORWARD) ? -1 : 1;
   const bool f32 = (flags & PA_FFT_F32) != 0;
   if (timing) CU(cudaEventRecord(S.t[0], user));
   if (P->dim < 0 || P->nproc == 1) {
     // one block, the whole local array: one kernel on the caller's stream
     const BlockCopy* b = &P->self_fused;
     bool launched = false;
-    RC(put_fft(1, &b, src, &dst, sign, rfft, f32, nullptr, user, &launched));
+    RC(put_fft(1, &b, src, &dst, sign, mode, r2r_kind, f32, nullptr, user, &launched));
     if (timing) {
       CU(cudaEventRecord(S.t[6], user));
       S.timed_once = true;
@@ -1330,7 +1329,7 @@ pa_status transpose_put_fft(Plan* P, Comm* comm, const void* src, void* dst, uns
     CU(cudaStreamWaitEvent(s, buf_ev, 0));
     CU(cudaStreamWaitEvent(s, buf_unpack_ev, 0));
   }
-  return one_sided(P, comm, src, dst, flags, sign, rfft ? SendFft::rfft : SendFft::fft, user);
+  return one_sided(P, comm, src, dst, flags, sign, &mode, r2r_kind, user);
 }
 
 // MPI.Waitall(t::Transposition) (Transpositions.jl:127-130)

@@ -535,4 +535,72 @@ rfft_first_fusable(dest::PencilArray{Complex{R}}, pc::Pencil; method = PeerPut()
     ccall((:pa_plan_rfft_put_check, libpa), Cint, (Ptr{Cvoid}, Cuint), first(rfft_put_plan(pc, dest, method)),
           R === Float32 ? Cuint(32) : Cuint(0)) == 0
 
+# The wall-bounded legs of the send-side fusion (pa_r2r_put / pa_brfft_put, DESIGN §3j), on REAL
+# plans: N reals per line along the first memory dimension of the plan's input pencil.  PeerPut, or
+# a local transposition with any method; byte for byte the unfused pair.  Under PeerPut they
+# register dest's window themselves (collective), after the verdict -- refused on every rank of the
+# line alike before any window setup.
+#   r2r_transpose!(dest, src, kind): dest = transpose(r2r(src, kind)), `src` and `dest` R on two real
+#     pencils, `kind` one of REDFT10 / REDFT01 / RODFT10 / RODFT01.
+#   brfft_transpose!(dest, src, pr): dest = transpose(brfft(src)), `src` Complex{R} on the complex
+#     y-pencil, `dest` R on the real x-pencil; `pr`: the real y-pencil the plan transposes from,
+#     `Pencil(pencil(src); size_global = (..., N, ...))` -- passed explicitly, as in
+#     rfft_transpose!.
+function real_put_plan(pr::Pencil, dest::PencilArray{R}, method) where {R<:Union{Float64,Float32}}
+    H = handles(pr.topology)
+    ex = Int64[extra_dims(dest)...]
+    key = (objectid(pr), objectid(pencil(dest)), Tuple(ex), sizeof(R), method_code(method))
+    plan = get!(H.plans, key) do
+        h = Ref{Ptr{Cvoid}}()
+        check(ccall((:pa_plan_create, libpa), Cint,
+            (Ptr{Cvoid}, Ptr{Cvoid}, Cint, Ptr{Int64}, Cint, Cint, Ptr{Ptr{Cvoid}}),
+            pencil_handle(H, pr), pencil_handle(H, pencil(dest)), length(ex), ex, sizeof(R),
+            method_code(method), h))
+        h[]
+    end
+    plan, H
+end
+
+function real_put_window!(plan, pr::Pencil, dest::PencilArray, method, flag)
+    check(ccall((:pa_plan_real_put_check, libpa), Cint, (Ptr{Cvoid}, Cuint), plan, flag))
+    if method isa PeerPut
+        R_dim = findfirst(i -> decomposition(pr)[i] != decomposition(pencil(dest))[i],
+                          1:length(decomposition(pr)))
+        R_dim === nothing || register_window!(plan, parent(dest), pr.topology, R_dim)
+    end
+end
+
+function r2r_transpose!(dest::PencilArray{R,N,<:CuArray}, src::PencilArray{R,N,<:CuArray}, kind::Integer;
+                        method = PeerPut(), waitall = true) where {R<:Union{Float64,Float32},N}
+    plan, H = real_put_plan(pencil(src), dest, method)
+    flag = R === Float32 ? Cuint(32) : Cuint(0)   # PA_FFT_F32
+    real_put_window!(plan, pencil(src), dest, method, flag)
+    flags = (waitall ? Cuint(1) : Cuint(0)) | flag   # PA_WAITALL
+    ptr_or_null(A) = isempty(A) ? C_NULL : devptr(A)
+    check(ccall((:pa_r2r_put, libpa), Cint,
+        (Ptr{Cvoid}, Ptr{Cvoid}, Cint, Ptr{Cvoid}, Ptr{Cvoid}, Cuint, Ptr{Cvoid}),
+        plan, H.comm, Cint(kind), ptr_or_null(parent(src)), ptr_or_null(parent(dest)), flags, stream_ptr()))
+    dest
+end
+
+function brfft_transpose!(dest::PencilArray{R,N,<:CuArray}, src::PencilArray{Complex{R},N,<:CuArray},
+                          pr::Pencil; method = PeerPut(), waitall = true) where {R<:Union{Float64,Float32},N}
+    plan, H = real_put_plan(pr, dest, method)
+    flag = R === Float32 ? Cuint(32) : Cuint(0)   # PA_FFT_F32
+    real_put_window!(plan, pr, dest, method, flag)
+    flags = (waitall ? Cuint(1) : Cuint(0)) | flag   # PA_WAITALL
+    ptr_or_null(A) = isempty(A) ? C_NULL : devptr(A)
+    check(ccall((:pa_brfft_put, libpa), Cint,
+        (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Cuint, Ptr{Cvoid}),
+        plan, H.comm, pencil_handle(H, pencil(src)), ptr_or_null(parent(src)), ptr_or_null(parent(dest)),
+        flags, stream_ptr()))
+    dest
+end
+
+# Whether r2r_transpose! / brfft_transpose! can run (pa_plan_real_put_check, one answer for both):
+# the same answer on every rank of the grid line.
+real_first_fusable(dest::PencilArray{R}, pr::Pencil; method = PeerPut()) where {R<:Union{Float64,Float32}} =
+    ccall((:pa_plan_real_put_check, libpa), Cint, (Ptr{Cvoid}, Cuint), first(real_put_plan(pr, dest, method)),
+          R === Float32 ? Cuint(32) : Cuint(0)) == 0
+
 end # module

@@ -10,6 +10,8 @@
     t = Transposition(cplx_y, real_x; rfft=True)          # GPU extension: cplx = rfft(transpose)
     transpose_(t; fft_first="forward")                    # GPU extension: dest = transpose(fft(src))
     t = Transposition(cplx_y, real_x; rfft_first=True)    # GPU extension: cplx = transpose(rfft(src))
+    t = Transposition(real_y, real_x; r2r_first="REDFT10")  # GPU extension: real = transpose(r2r(src))
+    t = Transposition(real_x, cplx_y; brfft_first=True)   # GPU extension: real = transpose(brfft(src))
 
 Python has no ``!`` in identifiers: ``transpose_`` (torch's in-place naming)
 stands for ``transpose!``; ``transpose_bang`` is an alias.  Errors follow the
@@ -60,9 +62,10 @@ class PeerPut(AbstractTransposeMethod):
     is COLLECTIVE over the communicator (like ``MPI_Win_create``): it exchanges
     CUDA IPC handles of ``dest``.  Falls back to the staged PointToPoint
     schedule when ``src`` and ``dest`` alias (in-place transposes).
-    ``transpose_(t, fft_first=...)`` and ``Transposition(..., rfft_first=True)`` fuse the
-    transform along ``src``'s first memory dimension into the put kernel: one kernel per rank
-    loads every local source line, transforms it and stores the bins into the peers' ``dest``.
+    ``transpose_(t, fft_first=...)`` and ``Transposition(..., rfft_first=True)`` (``r2r_first=``,
+    ``brfft_first=True``) fuse the transform along ``src``'s first memory dimension into the put
+    kernel: one kernel per rank loads every local source line, transforms it and stores the
+    outputs into the peers' ``dest``.
     """
     code = _lib.PA_PEER_PUT
 
@@ -250,6 +253,21 @@ def _register_arenas(plan: _Plan, Po: Pencil, comm):
                           lambda n, mapped, pl=pl: lib.pa_plan_set_recv_window(pl.h, n, mapped))
 
 
+def _real_pencil_of(cplx: Pencil, n: int) -> Pencil:
+    """The real counterpart of a complex pencil with ``n`` points along its first memory dim:
+    :func:`_rfft_pencil` when ``n`` is even, else derived once per (pencil, ``n``) in the same
+    family.  (An odd ``n`` is refused later, by the C verdict, as any other line length.)"""
+    pr = _rfft_pencil(cplx)
+    ax = as_tuple(cplx.perm, cplx.ndims)[0] - 1
+    if pr.size_global[ax] == n:
+        return pr
+    odd = cplx.__dict__.setdefault("_rfft_real_n", {})
+    if n not in odd:
+        odd[n] = Pencil(cplx, size_global=tuple(n if d == ax else m
+                                                for d, m in enumerate(cplx.size_global)))
+    return odd[n]
+
+
 def _brfft_pencil(real: Pencil) -> Pencil:
     """The complex counterpart of a real pencil -- N//2+1 points along its first memory dim --
     derived once per real pencil.  It is in the same family (shares the staging arenas), so
@@ -303,18 +321,35 @@ class Transposition:
     plan from ``Ai``'s N//2+1 counterpart to ``Ao``'s pencil, and ``transpose_(t)`` writes ``Ao =
     transpose(rfft_(Ai))`` in one kernel per rank (``pa_rfft_put``): ``PeerPut``, or a local
     transposition with any method.  Byte for byte ``rfft_`` followed by the plain transposition.
-    ``brfft``, ``r2r``, ``rfft`` and ``rfft_first`` exclude each other."""
+    ``brfft``, ``r2r``, ``rfft`` and ``rfft_first`` exclude each other.
+
+    ``r2r_first="REDFT10"`` (``"REDFT01"``, ``"RODFT10"``, ``"RODFT01"``; GPU extension, send side):
+    ``Ai`` and ``Ao`` are float64 (float32) arrays on two real pencils, and ``transpose_(t)`` writes
+    ``Ao = transpose(r2r_(Ai, kind))`` along ``Ai``'s first memory dim in one kernel per rank
+    (``pa_r2r_put``).  ``brfft_first=True``: ``Ai`` is complex128 (complex64) on a complex pencil
+    and ``Ao`` float64 (float32); N comes from ``Ao``'s pencil, the plan is the real plan from
+    ``Ai``'s N-point counterpart to ``Ao``'s pencil, and ``transpose_(t)`` writes ``Ao =
+    transpose(brfft(Ai))`` (``pa_brfft_put``).  Both need ``PeerPut`` when the transposition
+    exchanges data (any method when it is local) and are byte for byte the unfused pair.  Every
+    one of ``brfft``, ``r2r``, ``rfft``, ``rfft_first``, ``r2r_first`` and ``brfft_first`` excludes
+    the others."""
 
     def __init__(self, Ao: PencilArray, Ai: PencilArray, *, method=None, brfft=False, r2r=None,
-                 rfft=False, rfft_first=False):
+                 rfft=False, rfft_first=False, r2r_first=None, brfft_first=False):
         method = PointToPoint() if method is None else method
         Pi, Po = Ai.pencil, Ao.pencil
         self.brfft = bool(brfft)
         self.r2r = r2r
         self.rfft = bool(rfft)
         self.rfft_first = bool(rfft_first)
+        self.r2r_first = r2r_first
+        self.brfft_first = bool(brfft_first)
         if self.brfft + (r2r is not None) + self.rfft + self.rfft_first > 1:
             raise ArgumentError(_lib.PA_EINVAL, "brfft=, r2r=, rfft= and rfft_first= exclude each other")
+        if (self.brfft + (r2r is not None) + self.rfft + self.rfft_first + (r2r_first is not None)
+                + self.brfft_first > 1):
+            raise ArgumentError(_lib.PA_EINVAL, "brfft=, r2r=, rfft=, rfft_first=, r2r_first= and "
+                                "brfft_first= exclude each other")
         if Ai.extra_dims != Ao.extra_dims:  # :99-103
             raise ArgumentError(_lib.PA_EINVAL,
                                 "incompatible number of extra dimensions of PencilArrays: "
@@ -338,6 +373,21 @@ class Transposition:
                                     "complex128, or float32 and complex64: got "
                                     f"{Ai.dtype} and {Ao.dtype}")
             Pi = _brfft_pencil(Ai.pencil)  # the plan's input: the complex counterpart of src
+        elif r2r_first is not None:
+            if r2r_first not in _R2R_KINDS:
+                raise ArgumentError(_lib.PA_EINVAL,
+                                    f"r2r_first must be one of {sorted(_R2R_KINDS)}: got {r2r_first!r}")
+            if Ai.dtype != Ao.dtype or Ai.dtype not in _REAL_FLAGS:
+                raise ArgumentError(_lib.PA_EINVAL, "r2r_first: dest and src must be two float64 or "
+                                    f"two float32 arrays: got {Ao.dtype} and {Ai.dtype}")
+        elif self.brfft_first:
+            if (Ao.dtype, Ai.dtype) not in _BRFFT_PAIRS:
+                raise ArgumentError(_lib.PA_EINVAL, "brfft_first: dest and src must be float64 and "
+                                    "complex128, or float32 and complex64: got "
+                                    f"{Ao.dtype} and {Ai.dtype}")
+            ax = as_tuple(Ai.pencil.perm, Ai.pencil.ndims)[0] - 1
+            # the plan's input: the real counterpart of src, N points as in dest
+            Pi = _real_pencil_of(Ai.pencil, Ao.pencil.size_global[ax])
         elif self.brfft:
             if (Ao.dtype, Ai.dtype) not in _BRFFT_PAIRS:
                 raise ArgumentError(_lib.PA_EINVAL, "brfft: dest and src must be float64 and "
@@ -350,13 +400,17 @@ class Transposition:
             raise ArgumentError(_lib.PA_EINCOMPAT, "pencil topologies must be the same.")
         self.Pi, self.Po, self.Ai, self.Ao = Pi, Po, Ai, Ao
         self.method = method
-        elsize = Ao.elsize if self.rfft_first else Ai.elsize  # (rfft_first: the complex plan)
+        # (rfft_first: the complex plan; brfft_first: the real plan)
+        elsize = Ao.elsize if (self.rfft_first or self.brfft_first) else Ai.elsize
         self._plan = _get_plan(Pi, Po, Ai.extra_dims, elsize, method)  # remaining checks in C
         d = self._plan.info.dim
         self.dim = None if d == 0 else d  # :110
         if self.rfft_first:
             # (the same verdict on every rank of the line: refused before the collective window setup)
             check(lib.pa_plan_rfft_put_check(self._plan.h, _BRFFT_PAIRS[(Ai.dtype, Ao.dtype)]))
+        if r2r_first is not None or self.brfft_first:
+            # (likewise: one verdict for both, the same on every rank of the line)
+            check(lib.pa_plan_real_put_check(self._plan.h, _REAL_FLAGS[Ao.dtype]))
         fused = "brfft" if self.brfft else "rfft" if self.rfft else "r2r" if r2r is not None else None
         if fused and d != 0 and self._plan.info.nproc > 1 and isinstance(method, (PeerPut, PeerGet)):
             # (the same on every rank of the line: refused before the collective window setup)
@@ -393,8 +447,9 @@ class Transposition:
         For a ``brfft=True`` transposition: whether ``pa_transpose_brfft`` can run
         (``pa_plan_brfft_check``); for ``r2r=`` / ``rfft=True``: whether ``pa_transpose_r2r`` /
         ``pa_transpose_rfft`` can (``pa_plan_real_check``, one answer for both); for an
-        ``rfft_first=True`` one: False (see :meth:`fft_first_fusable`)."""
-        if self.rfft_first:
+        ``rfft_first=True`` (``r2r_first=``, ``brfft_first=True``) one: False (see
+        :meth:`fft_first_fusable`)."""
+        if self.rfft_first or self.r2r_first is not None or self.brfft_first:
             return False
         if self.r2r is not None or self.rfft:
             return lib.pa_plan_real_check(self._plan.h, _REAL_FLAGS[self.Ai.dtype]) == _lib.PA_OK
@@ -406,8 +461,12 @@ class Transposition:
     def fft_first_fusable(self) -> bool:
         """Whether the send-side fused kernel can run on this transposition: for a complex one
         ``transpose_(self, fft_first=...)`` (``pa_plan_fft_put_check``), for an ``rfft_first=True``
-        one ``transpose_(self)`` (``pa_plan_rfft_put_check``).  Needs ``PeerPut`` when the
-        transposition exchanges data; the answer is the same on every rank of the grid line."""
+        one ``transpose_(self)`` (``pa_plan_rfft_put_check``), for an ``r2r_first=`` or
+        ``brfft_first=True`` one ``transpose_(self)`` (``pa_plan_real_put_check``).  Needs ``PeerPut``
+        when the transposition exchanges data; the answer is the same on every rank of the grid
+        line."""
+        if self.r2r_first is not None or self.brfft_first:
+            return lib.pa_plan_real_put_check(self._plan.h, _REAL_FLAGS[self.Ao.dtype]) == _lib.PA_OK
         if self.rfft_first:
             flag = _BRFFT_PAIRS[(self.Ai.dtype, self.Ao.dtype)]
             return lib.pa_plan_rfft_put_check(self._plan.h, flag) == _lib.PA_OK
@@ -447,9 +506,9 @@ def transpose_(*args, method=None, waitall=True, overlap=True, stage_self=False,
     for byte ``fft_`` on a copy of ``src`` followed by the plain transposition; ``fft=`` and
     ``fft_first=`` exclude each other.
 
-    A ``Transposition(..., brfft=True)`` (``r2r=``, ``rfft=True``, ``rfft_first=True``) runs the
-    fused transpose + complex-to-real (real-to-real, real-to-complex) transform; ``fft=`` and
-    ``fft_first=`` do not apply to it."""
+    A ``Transposition(..., brfft=True)`` (``r2r=``, ``rfft=True``, ``rfft_first=True``,
+    ``r2r_first=``, ``brfft_first=True``) runs the fused transpose + complex-to-real (real-to-real,
+    real-to-complex) transform; ``fft=`` and ``fft_first=`` do not apply to it."""
     if len(args) == 1 and isinstance(args[0], Transposition):
         t = args[0]
     elif len(args) == 2:
@@ -469,6 +528,19 @@ def transpose_(*args, method=None, waitall=True, overlap=True, stage_self=False,
         check(lib.pa_rfft_put(t.plan.h, t.Pi.topology.comm.handle, t.Ai.pencil._h,
                               C.c_void_p(t.Ai.data_ptr() or None), C.c_void_p(t.Ao.data_ptr() or None),
                               flags | _BRFFT_PAIRS[(t.Ai.dtype, t.Ao.dtype)], _stream_ptr()))
+        return t if len(args) == 1 else args[0]
+    if t.r2r_first is not None or t.brfft_first:
+        what = "an r2r_first" if t.r2r_first is not None else "a brfft_first"
+        if fft is not None or fft_first is not None:
+            raise ArgumentError(_lib.PA_EINVAL, f"{what} transposition implies its transform: "
+                                "transpose_(t) without fft= / fft_first=")
+        comm = t.Pi.topology.comm.handle
+        src, dst = C.c_void_p(t.Ai.data_ptr() or None), C.c_void_p(t.Ao.data_ptr() or None)
+        flags |= _REAL_FLAGS[t.Ao.dtype]
+        if t.brfft_first:
+            check(lib.pa_brfft_put(t.plan.h, comm, t.Ai.pencil._h, src, dst, flags, _stream_ptr()))
+        else:
+            check(lib.pa_r2r_put(t.plan.h, comm, _R2R_KINDS[t.r2r_first], src, dst, flags, _stream_ptr()))
         return t if len(args) == 1 else args[0]
     if fft_first is not None and (t.brfft or t.rfft or t.r2r is not None):
         raise ArgumentError(_lib.PA_EINVAL, "fft_first= applies to complex transpositions only")
