@@ -496,8 +496,24 @@ pa_status pa_get_all(pa_plan* plan, void* const* peers, void* dst, int max_ctas,
   GUARD({ return all_blocks(plan, true, dst, peers, max_ctas, stream); })
 }
 
+// src / dst of the local arrays: NULL only when empty, not overlapping, dst 16-byte aligned
 static pa_status fused_pointers(const char* who, const void* src, i64 src_bytes, const void* dst,
-                                i64 dst_bytes);
+                                i64 dst_bytes) {
+  if ((!src && src_bytes > 0) || (!dst && dst_bytes > 0)) {
+    set_error("%s: null array pointer for a non-empty local array", who);
+    return PA_EINVAL;
+  }
+  const uintptr_t a = (uintptr_t)src, b = (uintptr_t)dst;
+  if (src_bytes > 0 && dst_bytes > 0 && a < b + (uintptr_t)dst_bytes && b < a + (uintptr_t)src_bytes) {
+    set_error("%s: src and dst overlap", who);
+    return PA_EINVAL;
+  }
+  if (dst_bytes > 0 && (b & 15)) {
+    set_error("%s: dst must be 16-byte aligned", who);
+    return PA_EINVAL;
+  }
+  return PA_OK;
+}
 
 // The one-sided fused gather + FFT without the window protocol.  Every check runs on the host
 // before any device call.
@@ -521,7 +537,7 @@ static pa_status get_all_fft(pa_plan* plan, const void* src, void* const* peers,
   }
   const bool f32 = (flags & PA_FFT_F32) != 0;
   // the verdict pa_transpose asks (for a PeerGet plan it covers this gather)
-  pa_status s = plan_fft_check(&P, f32);
+  pa_status s = plan_check(&P, Side::unpack, FusedMode::fft, f32);
   if (s != PA_OK) return s;
   const i64 es = P.elsize;
   const i64 src_bytes = P.length_in * es, dst_bytes = P.length_out * es;
@@ -700,24 +716,23 @@ pa_status pa_transpose(pa_plan* plan, pa_comm* comm, const void* src, void* dst,
   })
 }
 
-pa_status pa_plan_fft_check(const pa_plan* plan) {
+// pa_plan_*check*: plan_check's answer for the fused kernel of `mode` on `side`
+static pa_status plan_verdict(const char* who, const pa_plan* plan, Side side, FusedMode mode, bool f32) {
   GUARD({
     if (!plan) {
-      set_error("pa_plan_fft_check: null plan");
+      set_error("%s: null plan", who);
       return PA_EINVAL;
     }
-    return plan_fft_check(plan->p, false);
+    return plan_check(plan->p, side, mode, f32);
   })
 }
 
+pa_status pa_plan_fft_check(const pa_plan* plan) {
+  return plan_verdict("pa_plan_fft_check", plan, Side::unpack, FusedMode::fft, false);
+}
+
 pa_status pa_plan_fft_check_ex(const pa_plan* plan, unsigned flags) {
-  GUARD({
-    if (!plan) {
-      set_error("pa_plan_fft_check_ex: null plan");
-      return PA_EINVAL;
-    }
-    return plan_fft_check(plan->p, (flags & PA_FFT_F32) != 0);
-  })
+  return plan_verdict("pa_plan_fft_check_ex", plan, Side::unpack, FusedMode::fft, (flags & PA_FFT_F32) != 0);
 }
 
 pa_status pa_wait(pa_plan* plan, void* stream) {
@@ -876,6 +891,15 @@ pa_status pa_rfft(const pa_pencil* real, const pa_pencil* cplx, int n_extra,
 }
 
 // ---- real-to-real line transforms (DCT-II/III, DST-II/III) ----------------------------
+// kind: FFTW's REDFT10 (DCT-II), REDFT01 (DCT-III), RODFT10 (DST-II) or RODFT01 (DST-III)
+static pa_status r2r_kind_check(const char* who, int kind) {
+  if (kind != PA_REDFT10 && kind != PA_REDFT01 && kind != PA_RODFT10 && kind != PA_RODFT01) {
+    set_error("%s: kind %d is not PA_REDFT10, PA_REDFT01, PA_RODFT10 or PA_RODFT01", who, kind);
+    return PA_EINVAL;
+  }
+  return PA_OK;
+}
+
 // The checks in pa_rfft's order, all on the host before any device call.
 static pa_status r2r(const pa_pencil* pencil, int n_extra, const int64_t* extra_dims, int kind,
                      unsigned flags, const void* src, void* dst, void* stream) {
@@ -888,10 +912,8 @@ static pa_status r2r(const pa_pencil* pencil, int n_extra, const int64_t* extra_
   int ax = 0;
   pa_status s = line_axis(who, R, &ax);
   if (s != PA_OK) return s;
-  if (kind != PA_REDFT10 && kind != PA_REDFT01 && kind != PA_RODFT10 && kind != PA_RODFT01) {
-    set_error("%s: kind %d is not PA_REDFT10, PA_REDFT01, PA_RODFT10 or PA_RODFT01", who, kind);
-    return PA_EINVAL;
-  }
+  s = r2r_kind_check(who, kind);
+  if (s != PA_OK) return s;
   if (flags & ~PA_FFT_F32) {
     set_error("%s: flags must be 0 or PA_FFT_F32", who);
     return PA_EINVAL;
@@ -912,8 +934,7 @@ static pa_status r2r(const pa_pencil* pencil, int n_extra, const int64_t* extra_
   }
   s = need_gpu();
   if (s != PA_OK) return s;
-  return r2r_lines((int)N, kind == PA_REDFT10 || kind == PA_RODFT10,
-                   kind == PA_RODFT10 || kind == PA_RODFT01, f32, nlines, src, dst, stream);
+  return r2r_lines((int)N, r2r_forward(kind), r2r_sine(kind), f32, nlines, src, dst, stream);
 }
 
 pa_status pa_r2r(const pa_pencil* pencil, int n_extra, const int64_t* extra_dims, int kind,
@@ -927,25 +948,6 @@ static pa_status fused_flags(const char* who, unsigned flags) {
   if (flags & ~(PA_WAITALL | PA_NO_OVERLAP | PA_STAGE_SELF | PA_FFT_F32)) {
     set_error("%s: flags may combine PA_WAITALL, PA_NO_OVERLAP, PA_STAGE_SELF and PA_FFT_F32 only "
               "(the direction is implied)", who);
-    return PA_EINVAL;
-  }
-  return PA_OK;
-}
-
-// src / dst of the local arrays: NULL only when empty, not overlapping, dst 16-byte aligned
-static pa_status fused_pointers(const char* who, const void* src, i64 src_bytes, const void* dst,
-                                i64 dst_bytes) {
-  if ((!src && src_bytes > 0) || (!dst && dst_bytes > 0)) {
-    set_error("%s: null array pointer for a non-empty local array", who);
-    return PA_EINVAL;
-  }
-  const uintptr_t a = (uintptr_t)src, b = (uintptr_t)dst;
-  if (src_bytes > 0 && dst_bytes > 0 && a < b + (uintptr_t)dst_bytes && b < a + (uintptr_t)src_bytes) {
-    set_error("%s: src and dst overlap", who);
-    return PA_EINVAL;
-  }
-  if (dst_bytes > 0 && (b & 15)) {
-    set_error("%s: dst must be 16-byte aligned", who);
     return PA_EINVAL;
   }
   return PA_OK;
@@ -977,7 +979,7 @@ static pa_status transpose_brfft(pa_plan* plan, pa_comm* comm, const pa_pencil* 
   s = fused_pointers("pa_transpose_brfft", src, src_bytes, dst, dst_bytes);
   if (s != PA_OK) return s;
   // the same verdict on every rank of the grid line: a refusal launches nothing anywhere
-  s = plan_brfft_check(&P, f32);
+  s = plan_check(&P, Side::unpack, FusedMode::brfft, f32);
   if (s != PA_OK) return s;
   s = need_gpu();
   if (s != PA_OK) return s;
@@ -990,13 +992,7 @@ pa_status pa_transpose_brfft(pa_plan* plan, pa_comm* comm, const pa_pencil* real
 }
 
 pa_status pa_plan_brfft_check(const pa_plan* plan, unsigned flags) {
-  GUARD({
-    if (!plan) {
-      set_error("pa_plan_brfft_check: null plan");
-      return PA_EINVAL;
-    }
-    return plan_brfft_check(plan->p, (flags & PA_FFT_F32) != 0);
-  })
+  return plan_verdict("pa_plan_brfft_check", plan, Side::unpack, FusedMode::brfft, (flags & PA_FFT_F32) != 0);
 }
 
 // A real plan (Float64, elsize 8; Float32, elsize 4 with PA_FFT_F32) for pa_transpose_r2r /
@@ -1019,10 +1015,8 @@ static pa_status transpose_r2r(pa_plan* plan, pa_comm* comm, int kind, const voi
   }
   pa_status s = fused_flags(who, flags);
   if (s != PA_OK) return s;
-  if (kind != PA_REDFT10 && kind != PA_REDFT01 && kind != PA_RODFT10 && kind != PA_RODFT01) {
-    set_error("%s: kind %d is not PA_REDFT10, PA_REDFT01, PA_RODFT10 or PA_RODFT01", who, kind);
-    return PA_EINVAL;
-  }
+  s = r2r_kind_check(who, kind);
+  if (s != PA_OK) return s;
   Plan& P = *plan->p;
   const bool f32 = (flags & PA_FFT_F32) != 0;
   s = real_plan(who, P, f32);
@@ -1033,7 +1027,7 @@ static pa_status transpose_r2r(pa_plan* plan, pa_comm* comm, int kind, const voi
   s = fused_pointers(who, src, P.length_in * P.elsize, dst, P.length_out * P.elsize);
   if (s != PA_OK) return s;
   // the same verdict on every rank of the grid line: a refusal launches nothing anywhere
-  s = plan_real_check(&P, f32);
+  s = plan_check(&P, Side::unpack, FusedMode::r2r, f32);
   if (s != PA_OK) return s;
   s = need_gpu();
   if (s != PA_OK) return s;
@@ -1068,7 +1062,7 @@ static pa_status transpose_rfft(pa_plan* plan, pa_comm* comm, const pa_pencil* c
   const i64 dst_bytes = nlines * (N / 2 + 1) * 2 * P.elsize;
   s = fused_pointers(who, src, P.length_in * P.elsize, dst, dst_bytes);
   if (s != PA_OK) return s;
-  s = plan_real_check(&P, f32);
+  s = plan_check(&P, Side::unpack, FusedMode::rfft, f32);
   if (s != PA_OK) return s;
   s = need_gpu();
   if (s != PA_OK) return s;
@@ -1081,13 +1075,7 @@ pa_status pa_transpose_rfft(pa_plan* plan, pa_comm* comm, const pa_pencil* cplx,
 }
 
 pa_status pa_plan_real_check(const pa_plan* plan, unsigned flags) {
-  GUARD({
-    if (!plan) {
-      set_error("pa_plan_real_check: null plan");
-      return PA_EINVAL;
-    }
-    return plan_real_check(plan->p, (flags & PA_FFT_F32) != 0);
-  })
+  return plan_verdict("pa_plan_real_check", plan, Side::unpack, FusedMode::r2r, (flags & PA_FFT_F32) != 0);
 }
 
 // ---- send-side fused transform + put (pa_fft_put, pa_rfft_put, pa_r2r_put, pa_brfft_put and
@@ -1097,14 +1085,13 @@ pa_status pa_plan_real_check(const pa_plan* plan, unsigned flags) {
 // complex one), then src / dst (NULL only when empty, not overlapping, aligned: fft / rfft to the
 // complex element; r2r / brfft src to a pair of reals or a complex element, dst to the real).
 static pa_status put_args(const char* who, Plan& P, const pa_pencil* pen, const void* src,
-                          const void* dst, PutMode mode, bool f32) {
-  const bool rfft = mode == PutMode::rfft, real = mode == PutMode::r2r || mode == PutMode::brfft;
-  pa_status s = real ? plan_real_put_check(&P, f32) : rfft ? plan_rfft_put_check(&P, f32)
-                                                           : plan_fft_put_check(&P, f32);
+                          const void* dst, FusedMode mode, bool f32) {
+  const bool rfft = mode == FusedMode::rfft, real = put_moves_reals(mode);
+  pa_status s = plan_check(&P, Side::put, mode, f32);
   if (s != PA_OK) return s;
   const i64 es = P.elsize;
   i64 src_bytes = P.length_in * es;
-  if (rfft || mode == PutMode::brfft) {
+  if (rfft || mode == FusedMode::brfft) {
     const pa_pencil in{P.pin};
     int N = 0;
     i64 nlines = 0;
@@ -1122,7 +1109,7 @@ static pa_status put_args(const char* who, Plan& P, const pa_pencil* pen, const 
   if (src_bytes > 0 && dst_bytes > 0 && a < b + (uintptr_t)dst_bytes && b < a + (uintptr_t)src_bytes) {
     set_error("%s: src and dst overlap (the send-side fusion has no staged schedule: transform in "
               "place with %s, then transpose)", who,
-              mode == PutMode::fft ? "fft_" : rfft ? "rfft_" : mode == PutMode::r2r ? "r2r_" : "brfft_");
+              mode == FusedMode::fft ? "fft_" : rfft ? "rfft_" : mode == FusedMode::r2r ? "r2r_" : "brfft_");
     return PA_EINVAL;
   }
   if (real) {
@@ -1143,13 +1130,13 @@ static pa_status put_args(const char* who, Plan& P, const pa_pencil* pen, const 
 
 // flags: exactly one of PA_FFT_FORWARD / PA_FFT_BACKWARD (fft), or none (rfft, r2r, brfft: the
 // direction is implied), with any of `extra`
-static pa_status put_flags(const char* who, unsigned flags, PutMode mode, unsigned extra) {
+static pa_status put_flags(const char* who, unsigned flags, FusedMode mode, unsigned extra) {
   if (flags & PA_STAGE_SELF) {
     set_error("%s: PA_STAGE_SELF does not apply: the send-side fusion stores the self block "
               "straight into dst", who);
     return PA_EINVAL;
   }
-  const bool implied = mode != PutMode::fft;
+  const bool implied = mode != FusedMode::fft;
   const unsigned dir = flags & ~extra;
   if (implied ? dir != 0 : (dir != PA_FFT_FORWARD && dir != PA_FFT_BACKWARD)) {
     if (implied)
@@ -1163,26 +1150,18 @@ static pa_status put_flags(const char* who, unsigned flags, PutMode mode, unsign
   return PA_OK;
 }
 
-static pa_status r2r_kind_check(const char* who, int kind) {
-  if (kind != PA_REDFT10 && kind != PA_REDFT01 && kind != PA_RODFT10 && kind != PA_RODFT01) {
-    set_error("%s: kind %d is not PA_REDFT10, PA_REDFT01, PA_RODFT10 or PA_RODFT01", who, kind);
-    return PA_EINVAL;
-  }
-  return PA_OK;
-}
-
-static const char* put_name(PutMode mode, bool all) {
+static const char* put_name(FusedMode mode, bool all) {
   switch (mode) {
-    case PutMode::fft: return all ? "pa_put_all_fft" : "pa_fft_put";
-    case PutMode::rfft: return all ? "pa_put_all_rfft" : "pa_rfft_put";
-    case PutMode::r2r: return all ? "pa_put_all_r2r" : "pa_r2r_put";
-    case PutMode::brfft: break;
+    case FusedMode::fft: return all ? "pa_put_all_fft" : "pa_fft_put";
+    case FusedMode::rfft: return all ? "pa_put_all_rfft" : "pa_rfft_put";
+    case FusedMode::r2r: return all ? "pa_put_all_r2r" : "pa_r2r_put";
+    case FusedMode::brfft: break;
   }
   return all ? "pa_put_all_brfft" : "pa_brfft_put";
 }
 
 static pa_status fft_put(pa_plan* plan, pa_comm* comm, const pa_pencil* pen, const void* src, void* dst,
-                         unsigned flags, void* stream, PutMode mode, int r2r_kind = 0) {
+                         unsigned flags, void* stream, FusedMode mode, int r2r_kind = 0) {
   const char* who = put_name(mode, false);
   if (!plan) {
     set_error("%s: null plan", who);
@@ -1190,7 +1169,7 @@ static pa_status fft_put(pa_plan* plan, pa_comm* comm, const pa_pencil* pen, con
   }
   pa_status s = put_flags(who, flags, mode, PA_FFT_F32 | PA_WAITALL);
   if (s != PA_OK) return s;
-  if (mode == PutMode::r2r && (s = r2r_kind_check(who, r2r_kind)) != PA_OK) return s;
+  if (mode == FusedMode::r2r && (s = r2r_kind_check(who, r2r_kind)) != PA_OK) return s;
   Plan& P = *plan->p;
   const bool f32 = (flags & PA_FFT_F32) != 0;
   s = put_args(who, P, pen, src, dst, mode, f32);
@@ -1202,28 +1181,28 @@ static pa_status fft_put(pa_plan* plan, pa_comm* comm, const pa_pencil* pen, con
 
 pa_status pa_fft_put(pa_plan* plan, pa_comm* comm, const void* src, void* dst, unsigned flags,
                      void* stream) {
-  GUARD({ return fft_put(plan, comm, nullptr, src, dst, flags, stream, PutMode::fft); })
+  GUARD({ return fft_put(plan, comm, nullptr, src, dst, flags, stream, FusedMode::fft); })
 }
 
 pa_status pa_rfft_put(pa_plan* plan, pa_comm* comm, const pa_pencil* real, const void* src, void* dst,
                       unsigned flags, void* stream) {
-  GUARD({ return fft_put(plan, comm, real, src, dst, flags, stream, PutMode::rfft); })
+  GUARD({ return fft_put(plan, comm, real, src, dst, flags, stream, FusedMode::rfft); })
 }
 
 pa_status pa_r2r_put(pa_plan* plan, pa_comm* comm, int kind, const void* src, void* dst, unsigned flags,
                      void* stream) {
-  GUARD({ return fft_put(plan, comm, nullptr, src, dst, flags, stream, PutMode::r2r, kind); })
+  GUARD({ return fft_put(plan, comm, nullptr, src, dst, flags, stream, FusedMode::r2r, kind); })
 }
 
 pa_status pa_brfft_put(pa_plan* plan, pa_comm* comm, const pa_pencil* cplx, const void* src, void* dst,
                        unsigned flags, void* stream) {
-  GUARD({ return fft_put(plan, comm, cplx, src, dst, flags, stream, PutMode::brfft); })
+  GUARD({ return fft_put(plan, comm, cplx, src, dst, flags, stream, FusedMode::brfft); })
 }
 
 // The send-side fused kernel without the window protocol: the self block into `dst`, the put
 // block of peer n into peers[n - 1] (its dst, as mapped here; the self entry is ignored).
 static pa_status put_all_fft(pa_plan* plan, const pa_pencil* pen, const void* src, void* const* peers,
-                             void* dst, unsigned flags, void* stream, PutMode mode, int r2r_kind = 0) {
+                             void* dst, unsigned flags, void* stream, FusedMode mode, int r2r_kind = 0) {
   const char* who = put_name(mode, true);
   if (!plan) {
     set_error("%s: null plan", who);
@@ -1236,7 +1215,7 @@ static pa_status put_all_fft(pa_plan* plan, const pa_pencil* pen, const void* sr
   }
   pa_status s = put_flags(who, flags, mode, PA_FFT_F32);
   if (s != PA_OK) return s;
-  if (mode == PutMode::r2r && (s = r2r_kind_check(who, r2r_kind)) != PA_OK) return s;
+  if (mode == FusedMode::r2r && (s = r2r_kind_check(who, r2r_kind)) != PA_OK) return s;
   const bool f32 = (flags & PA_FFT_F32) != 0;
   s = put_args(who, P, pen, src, dst, mode, f32);
   if (s != PA_OK) return s;
@@ -1267,52 +1246,34 @@ static pa_status put_all_fft(pa_plan* plan, const pa_pencil* pen, const void* sr
 
 pa_status pa_put_all_fft(pa_plan* plan, const void* src, void* const* peers, void* dst, unsigned flags,
                          void* stream) {
-  GUARD({ return put_all_fft(plan, nullptr, src, peers, dst, flags, stream, PutMode::fft); })
+  GUARD({ return put_all_fft(plan, nullptr, src, peers, dst, flags, stream, FusedMode::fft); })
 }
 
 pa_status pa_put_all_rfft(pa_plan* plan, const pa_pencil* real, const void* src, void* const* peers,
                           void* dst, unsigned flags, void* stream) {
-  GUARD({ return put_all_fft(plan, real, src, peers, dst, flags, stream, PutMode::rfft); })
+  GUARD({ return put_all_fft(plan, real, src, peers, dst, flags, stream, FusedMode::rfft); })
 }
 
 pa_status pa_put_all_r2r(pa_plan* plan, int kind, const void* src, void* const* peers, void* dst,
                          unsigned flags, void* stream) {
-  GUARD({ return put_all_fft(plan, nullptr, src, peers, dst, flags, stream, PutMode::r2r, kind); })
+  GUARD({ return put_all_fft(plan, nullptr, src, peers, dst, flags, stream, FusedMode::r2r, kind); })
 }
 
 pa_status pa_put_all_brfft(pa_plan* plan, const pa_pencil* cplx, const void* src, void* const* peers,
                            void* dst, unsigned flags, void* stream) {
-  GUARD({ return put_all_fft(plan, cplx, src, peers, dst, flags, stream, PutMode::brfft); })
+  GUARD({ return put_all_fft(plan, cplx, src, peers, dst, flags, stream, FusedMode::brfft); })
 }
 
 pa_status pa_plan_real_put_check(const pa_plan* plan, unsigned flags) {
-  GUARD({
-    if (!plan) {
-      set_error("pa_plan_real_put_check: null plan");
-      return PA_EINVAL;
-    }
-    return plan_real_put_check(plan->p, (flags & PA_FFT_F32) != 0);
-  })
+  return plan_verdict("pa_plan_real_put_check", plan, Side::put, FusedMode::r2r, (flags & PA_FFT_F32) != 0);
 }
 
 pa_status pa_plan_fft_put_check(const pa_plan* plan, unsigned flags) {
-  GUARD({
-    if (!plan) {
-      set_error("pa_plan_fft_put_check: null plan");
-      return PA_EINVAL;
-    }
-    return plan_fft_put_check(plan->p, (flags & PA_FFT_F32) != 0);
-  })
+  return plan_verdict("pa_plan_fft_put_check", plan, Side::put, FusedMode::fft, (flags & PA_FFT_F32) != 0);
 }
 
 pa_status pa_plan_rfft_put_check(const pa_plan* plan, unsigned flags) {
-  GUARD({
-    if (!plan) {
-      set_error("pa_plan_rfft_put_check: null plan");
-      return PA_EINVAL;
-    }
-    return plan_rfft_put_check(plan->p, (flags & PA_FFT_F32) != 0);
-  })
+  return plan_verdict("pa_plan_rfft_put_check", plan, Side::put, FusedMode::rfft, (flags & PA_FFT_F32) != 0);
 }
 
 pa_status pa_host_chain_create(int n, pa_plan* const* plans, pa_comm* comm, pa_host_chain** out) {

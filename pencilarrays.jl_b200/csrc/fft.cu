@@ -33,6 +33,7 @@
 #include <map>
 #include <mutex>
 #include <tuple>
+#include <type_traits>
 #include <vector>
 
 // twiddles: one table lookup per butterfly, the other powers by squaring / products (the
@@ -1250,10 +1251,79 @@ static const void* twiddles(int L, bool f32) {
   return d;
 }
 
+// the twiddle tables of a launch: W_n into *tw and, with n4 > 0, W_n4 into *tw4
+static pa_status line_twiddles(const char* what, bool f32, int n, const void** tw, int n4 = 0,
+                               const void** tw4 = nullptr) {
+  *tw = twiddles(n, f32);
+  if (n4 > 0) *tw4 = twiddles(n4, f32);
+  if (!*tw || (n4 > 0 && !*tw4)) {
+    set_error("%s: twiddle table allocation failed", what);
+    cudaGetLastError();
+    return PA_ENOMEM;
+  }
+  return PA_OK;
+}
+
+// Lines per CTA of the line kernels: fft_lines / fft_lines_f32, except that tunable fft_lines = 4
+// gives the complex FFT 4 lines per CTA also for 256- / 512-point lines in double precision
+// (64-byte gathers, first pass of radix 4 / 8 in registers, half the shared memory per CTA)
+static int lines_per_cta(bool f32, int logL, bool complex_fft) {
+  if (f32) return fft_lines_f32(logL);
+  return (complex_fft && g_tun.fft_lines == 4 && logL >= 8) ? 4 : fft_lines(logL);
+}
+
+template <int V>
+using Int = std::integral_constant<int, V>;
+
+// Returns f(Int<LOGL>, Int<C>, T{}) for lines of 2^logL points (3..10) and the C lines per CTA that
+// lines_per_cta gave: one kernel instantiation of a family.  Only the complex-FFT families
+// (LINES4) instantiate the C = 4 variants at 256 and 512 points in double precision.
+template <bool LINES4 = false, class F>
+static auto dispatch(bool f32, int logL, int C, F&& f) {
+  auto at = [&](auto lg) {
+    constexpr int LG = decltype(lg)::value;
+    if (f32) return f(lg, Int<fft_lines_f32(LG)>{}, float{});
+    if constexpr (LINES4 && (LG == 8 || LG == 9))
+      if (C == 4) return f(lg, Int<4>{}, double{});
+    return f(lg, Int<fft_lines(LG)>{}, double{});
+  };
+  switch (logL) {
+    case 3: return at(Int<3>{});
+    case 4: return at(Int<4>{});
+    case 5: return at(Int<5>{});
+    case 6: return at(Int<6>{});
+    case 7: return at(Int<7>{});
+    case 8: return at(Int<8>{});
+    case 9: return at(Int<9>{});
+    default: return at(Int<10>{});
+  }
+}
+
+// Launches a line kernel of C lines per CTA, each staged in `pitch` complex slots of shared
+// memory, and counts it.  Shared memory is the scarce resource: ask for the largest carve-out so
+// that several CTAs (gather of one, butterflies of another) overlap on an SM.
+template <class Params>
+static pa_status launch_lines(const char* what, void (*kern)(Params), const Params& p,
+                              unsigned long long grid, int C, int pitch, bool f32, void* stream) {
+  const size_t smem = (f32 ? sizeof(pa_fft::cplxf) : sizeof(cplx)) * (size_t)C * pitch;
+  cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout,
+                       cudaSharedmemCarveoutMaxShared);
+  cudaGetLastError();
+  kern<<<(unsigned)grid, FFT_THREADS, smem, (cudaStream_t)stream>>>(p);
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) {
+    set_error("%s kernel launch failed: %s", what, cudaGetErrorString(e));
+    return PA_ECUDA;
+  }
+  count_launch();
+  return PA_OK;
+}
+
 // Launch geometry of the fused kernel from the blocks of one rank (`blocks[i]` moves block i
 // from `srcs[i]` -- recv_buf, or the src parent for the fused self block -- into `dst`;
 // together they must tile the destination box), and every check of it.  srcs / dst may be
-// NULL: plan_fft_check runs this on the blocks a peer would see, without arrays.  *grid = 0:
+// NULL: fused_check runs this on the blocks a peer would see, without arrays.  *grid = 0:
 // nothing to do on this rank.  f32: ComplexF32 elements (PA_FFT_F32), else ComplexF64.
 // brfft (k_unpack_brfft): the lines are M = N/2 + 1 bins, and `dst` is the REAL array of N
 // reals per line in place of the complex one the blocks describe (DESIGN §3e).
@@ -1264,7 +1334,7 @@ static pa_status fft_geometry(int nb, const BlockCopy* const* blocks, const void
                               void* dst, bool f32, FusedMode mode, FftParams& p, int* C_out,
                               unsigned long long* grid_out) {
   const bool brfft = mode == FusedMode::brfft;
-  const bool real = mode == FusedMode::r2r || mode == FusedMode::rfft;  // real source elements
+  const bool real = unpack_moves_reals(mode);  // real source elements
   const i64 es = real ? (f32 ? 4 : 8) : (f32 ? 8 : 16);  // element bytes
   memset(&p, 0, sizeof p);
   *grid_out = 0;
@@ -1459,12 +1529,8 @@ static pa_status fft_geometry(int nb, const BlockCopy* const* blocks, const void
     for (int o = 0; o < p.no; ++o)
       if (!to_cplx(p.dso[o] / es, &p.dso[o])) return PA_EINVAL;
   }
-  // tunable "fft_lines" = 4: 4 lines per CTA also for 256- / 512-point lines (64-byte gathers,
-  // first pass of radix 4 / 8 in registers, half the shared memory per CTA); double precision
-  // only -- single precision always takes fft_lines_f32.  brfft, r2r, rfft: the lines per CTA of
-  // k_rfft
-  const int C = f32 ? fft_lines_f32(logL)
-                    : ((mode == FusedMode::fft && g_tun.fft_lines == 4 && logL >= 8) ? 4 : fft_lines(logL));
+  // (brfft, r2r, rfft: the lines per CTA of k_rfft)
+  const int C = lines_per_cta(f32, logL, mode == FusedMode::fft);
   p.tiles_x = (unsigned)((p.ex + C - 1) / C);
   unsigned long long grid = p.tiles_x;
   for (int i = 0; i < p.no; ++i) grid *= (unsigned long long)p.oe[i];
@@ -1477,71 +1543,53 @@ static pa_status fft_geometry(int nb, const BlockCopy* const* blocks, const void
   return PA_OK;
 }
 
-pa_status unpack_fft(int nb, const BlockCopy* const* blocks, const void* const* srcs, void* dst,
-                     int sign, bool f32, void* stream) {
-  // (pa_transpose has already asked plan_fft_check, for every rank of the line, before it
+pa_status unpack_fused(int nb, const BlockCopy* const* blocks, const void* const* srcs, void* dst, int sign,
+                       FusedMode mode, int r2r_kind, bool f32, void* stream) {
+  // (the entry points have already asked plan_check, for every rank of the line, before they
   //  enqueued anything: these checks only guard direct callers)
   FftParams p;
   int C = 0;
   unsigned long long grid = 0;
-  pa_status s = fft_geometry(nb, blocks, srcs, dst, f32, FusedMode::fft, p, &C, &grid);
+  pa_status s = fft_geometry(nb, blocks, srcs, dst, f32, mode, p, &C, &grid);
   if (s != PA_OK || grid == 0) return s;
   const int logL = p.logL;
-  p.sign = sign < 0 ? -1 : 1;
-  p.tw = twiddles(p.L, f32);
-  if (!p.tw) {
-    set_error("fused FFT: twiddle table allocation failed");
-    cudaGetLastError();
-    return PA_ENOMEM;
+  const bool forward = r2r_forward(r2r_kind);
+  const char* what = "fused FFT";
+  void (*kern)(FftParams) = nullptr;
+  switch (mode) {
+    case FusedMode::fft:
+      p.sign = sign < 0 ? -1 : 1;
+      kern = dispatch<true>(f32, logL, C, [](auto lg, auto c, auto t) { return k_unpack_fft<lg, c, decltype(t)>; });
+      break;
+    case FusedMode::rfft:
+      what = "fused rfft";
+      p.pitch = pa_fft::padded_pitch(p.L);  // as rfft_lines, forward
+      kern = dispatch(f32, logL, C, [](auto lg, auto c, auto t) { return k_unpack_rfft<lg, c, decltype(t)>; });
+      break;
+    case FusedMode::r2r:
+      what = "fused r2r";
+      p.pitch = pa_fft::padded_pitch(forward ? p.L : p.L + 1);  // as r2r_lines
+      p.sine = r2r_sine(r2r_kind) ? 1 : 0;
+      kern = dispatch(f32, logL, C, [forward](auto lg, auto c, auto t) {
+        return forward ? k_unpack_r2r<lg, c, true, decltype(t)> : k_unpack_r2r<lg, c, false, decltype(t)>;
+      });
+      break;
+    case FusedMode::brfft:
+      what = "fused brfft";
+      p.sign = 1;
+      kern = dispatch(f32, logL, C, [](auto lg, auto c, auto t) { return k_unpack_brfft<lg, c, decltype(t)>; });
+      break;
   }
-  const size_t smem = (f32 ? sizeof(pa_fft::cplxf) : sizeof(cplx)) * (size_t)C * p.pitch;
-  cudaError_t e = cudaSuccess;
-  auto launch = [&](auto kern) {
-    // shared memory is the scarce resource: ask for the largest carve-out so that
-    // several CTAs (gather of one, butterflies of another) overlap on an SM
-    static bool configured = false;  // one static per instantiation of this lambda's closure type
-    (void)configured;
-    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout,
-                         cudaSharedmemCarveoutMaxShared);
-    cudaGetLastError();
-    kern<<<(unsigned)grid, FFT_THREADS, smem, (cudaStream_t)stream>>>(p);
-    e = cudaGetLastError();
-  };
-  if (f32) {
-    switch (logL) {
-      case 3: launch(k_unpack_fft<3, 16, float>); break;
-      case 4: launch(k_unpack_fft<4, 16, float>); break;
-      case 5: launch(k_unpack_fft<5, 16, float>); break;
-      case 6: launch(k_unpack_fft<6, 16, float>); break;
-      case 7: launch(k_unpack_fft<7, 16, float>); break;
-      case 8: launch(k_unpack_fft<8, 16, float>); break;
-      case 9: launch(k_unpack_fft<9, 16, float>); break;
-      default: launch(k_unpack_fft<10, 8, float>); break;
-    }
-  } else {
-    switch (logL) {
-      case 3: launch(k_unpack_fft<3, 8, double>); break;
-      case 4: launch(k_unpack_fft<4, 8, double>); break;
-      case 5: launch(k_unpack_fft<5, 8, double>); break;
-      case 6: launch(k_unpack_fft<6, 8, double>); break;
-      case 7: launch(k_unpack_fft<7, 8, double>); break;
-      case 8: if (C == 4) launch(k_unpack_fft<8, 4, double>); else launch(k_unpack_fft<8, 8, double>); break;
-      case 9: if (C == 4) launch(k_unpack_fft<9, 4, double>); else launch(k_unpack_fft<9, 8, double>); break;
-      default: launch(k_unpack_fft<10, 4, double>); break;
-    }
-  }
-  if (e != cudaSuccess) {
-    set_error("fused FFT kernel launch failed: %s", cudaGetErrorString(e));
-    return PA_ECUDA;
-  }
-  count_launch();
-  return PA_OK;
+  // W_L for the complex FFT, W_N (N = 2L reals) for the real-line kernels; r2r also W_4N
+  s = line_twiddles(what, f32, mode == FusedMode::fft ? p.L : 2 * p.L, &p.tw,
+                    mode == FusedMode::r2r ? 8 * p.L : 0, &p.tw4);
+  if (s != PA_OK) return s;
+  return launch_lines(what, kern, p, grid, C, p.pitch, f32, stream);
 }
 
 pa_status get_fft(int nb, const BlockCopy* const* blocks, const void* const* srcs, void* dst, int sign,
                   bool f32, const MultiFlags* mf, void* stream, bool* launched) {
-  // (pa_transpose and pa_get_all_fft have already asked plan_fft_check)
+  // (pa_transpose and pa_get_all_fft have already asked plan_check)
   *launched = false;
   FftGetParams gp;
   int C = 0;
@@ -1551,54 +1599,13 @@ pa_status get_fft(int nb, const BlockCopy* const* blocks, const void* const* src
   FftParams& p = gp.p;
   memset(&gp.mf, 0, sizeof gp.mf);
   if (mf) gp.mf = *mf;
-  const int logL = p.logL;
   p.sign = sign < 0 ? -1 : 1;
-  p.tw = twiddles(p.L, f32);
-  if (!p.tw) {
-    set_error("fused FFT: twiddle table allocation failed");
-    cudaGetLastError();
-    return PA_ENOMEM;
-  }
-  const size_t smem = (f32 ? sizeof(pa_fft::cplxf) : sizeof(cplx)) * (size_t)C * p.pitch;
-  cudaError_t e = cudaSuccess;
-  auto launch = [&](auto kern) {
-    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout,
-                         cudaSharedmemCarveoutMaxShared);
-    cudaGetLastError();
-    kern<<<(unsigned)grid, FFT_THREADS, smem, (cudaStream_t)stream>>>(gp);
-    e = cudaGetLastError();
-  };
-  if (f32) {
-    switch (logL) {
-      case 3: launch(k_get_fft<3, 16, float>); break;
-      case 4: launch(k_get_fft<4, 16, float>); break;
-      case 5: launch(k_get_fft<5, 16, float>); break;
-      case 6: launch(k_get_fft<6, 16, float>); break;
-      case 7: launch(k_get_fft<7, 16, float>); break;
-      case 8: launch(k_get_fft<8, 16, float>); break;
-      case 9: launch(k_get_fft<9, 16, float>); break;
-      default: launch(k_get_fft<10, 8, float>); break;
-    }
-  } else {
-    switch (logL) {
-      case 3: launch(k_get_fft<3, 8, double>); break;
-      case 4: launch(k_get_fft<4, 8, double>); break;
-      case 5: launch(k_get_fft<5, 8, double>); break;
-      case 6: launch(k_get_fft<6, 8, double>); break;
-      case 7: launch(k_get_fft<7, 8, double>); break;
-      case 8: if (C == 4) launch(k_get_fft<8, 4, double>); else launch(k_get_fft<8, 8, double>); break;
-      case 9: if (C == 4) launch(k_get_fft<9, 4, double>); else launch(k_get_fft<9, 8, double>); break;
-      default: launch(k_get_fft<10, 4, double>); break;
-    }
-  }
-  if (e != cudaSuccess) {
-    set_error("one-sided fused FFT kernel launch failed: %s", cudaGetErrorString(e));
-    return PA_ECUDA;
-  }
-  count_launch();
-  *launched = true;
-  return PA_OK;
+  s = line_twiddles("fused FFT", f32, p.L, &p.tw);
+  if (s != PA_OK) return s;
+  auto kern = dispatch<true>(f32, p.logL, C, [](auto lg, auto c, auto t) { return k_get_fft<lg, c, decltype(t)>; });
+  s = launch_lines("one-sided fused FFT", kern, gp, grid, C, p.pitch, f32, stream);
+  *launched = s == PA_OK;
+  return s;
 }
 
 // Launch geometry of k_fft_put / k_rfft_put from the blocks of one rank -- the mirror of
@@ -1608,7 +1615,7 @@ pa_status get_fft(int nb, const BlockCopy* const* blocks, const void* const* src
 // must tile [0, M) along it (M = L points; rfft: M = N/2 + 1 bins) and share every other dim,
 // whose destination strides may differ (the peers' arrays have their own layouts).  The column
 // dim is the destination's stride-1 dim when that is not the line dim.  src / dsts may be NULL:
-// plan_fft_put_check runs this without arrays.  *grid = 0: this rank has no source lines.
+// put_check runs this without arrays.  *grid = 0: this rank has no source lines.
 // rfft: the plan is the COMPLEX plan of M bins per line, and `src` the REAL array of N reals per
 // line that replaces its source (same layout otherwise): the source offsets and strides, multiples
 // of M, are rescaled to N reals -- brfft's destination rescale, mirrored.
@@ -1617,10 +1624,10 @@ pa_status get_fft(int nb, const BlockCopy* const* blocks, const void* const* src
 // that replaces it, the source offsets and strides rescaled from N reals to N/2 + 1 bins.  Both
 // require those offsets and strides to be multiples of N, so one verdict serves both.
 static pa_status put_fft_geometry(int nb, const BlockCopy* const* blocks, const void* src,
-                                  void* const* dsts, bool f32, PutMode mode, FftPutParams& pp, int* C_out,
+                                  void* const* dsts, bool f32, FusedMode mode, FftPutParams& pp, int* C_out,
                                   unsigned long long* grid_out) {
-  const bool rfft = mode == PutMode::rfft;
-  const bool real = mode == PutMode::r2r || mode == PutMode::brfft;  // the plan moves reals
+  const bool rfft = mode == FusedMode::rfft;
+  const bool real = put_moves_reals(mode);  // the plan moves reals
   const char* what = real ? "fused real transform + put" : rfft ? "fused rfft + put" : "fused FFT + put";
   const i64 es = real ? (f32 ? 4 : 8) : (f32 ? 8 : 16);  // the plan's element bytes
   memset(&pp, 0, sizeof pp);
@@ -1730,7 +1737,7 @@ static pa_status put_fft_geometry(int nb, const BlockCopy* const* blocks, const 
                   (long long)M);
       return false;
     }
-    *out = rfft ? off / M * N * rs : mode == PutMode::brfft ? off / M * Mc * 2 * rs : off * rs;
+    *out = rfft ? off / M * N * rs : mode == FusedMode::brfft ? off / M * Mc * 2 * rs : off * rs;
     return true;
   };
   FftParams& p = pp.p;
@@ -1742,7 +1749,7 @@ static pa_status put_fft_geometry(int nb, const BlockCopy* const* blocks, const 
   S.y0 = 0;
   S.ey = (int)L;
   S.ssy = (rfft || real) ? 2 * rs : es;
-  S.ssx = mode == PutMode::brfft ? Mc * 2 * rs : (rfft || real) ? N * rs : L * es;
+  S.ssx = mode == FusedMode::brfft ? Mc * 2 * rs : (rfft || real) ? N * rs : L * es;
   if (jx >= 0 && !src_bytes(ref->raw[jx].ss, &S.ssx)) return PA_EINVAL;
   for (int i = 1; i < ref->nd_raw; ++i)
     if (i != jx && ref->raw[i].e > 1) {
@@ -1771,8 +1778,7 @@ static pa_status put_fft_geometry(int nb, const BlockCopy* const* blocks, const 
   // k_r2r (01 kinds) stage the L + 1 slots, which put_fft sets
   p.pitch = pa_fft::padded_pitch((int)L);
   // the lines per CTA of fft_ (tunable fft_lines included) / of k_rfft and k_r2r
-  const int C = f32 ? fft_lines_f32(logL)
-                    : ((mode == PutMode::fft && g_tun.fft_lines == 4 && logL >= 8) ? 4 : fft_lines(logL));
+  const int C = lines_per_cta(f32, logL, mode == FusedMode::fft);
   p.tiles_x = (unsigned)((p.ex + C - 1) / C);
   unsigned long long grid = p.tiles_x;
   for (int i = 0; i < p.no; ++i) grid *= (unsigned long long)p.oe[i];
@@ -1786,9 +1792,8 @@ static pa_status put_fft_geometry(int nb, const BlockCopy* const* blocks, const 
 }
 
 pa_status put_fft(int nb, const BlockCopy* const* blocks, const void* src, void* const* dsts, int sign,
-                  PutMode mode, int r2r_kind, bool f32, const MultiFlags* mf, void* stream, bool* launched) {
-  // (the entry points have already asked plan_fft_put_check / plan_rfft_put_check /
-  //  plan_real_put_check)
+                  FusedMode mode, int r2r_kind, bool f32, const MultiFlags* mf, void* stream, bool* launched) {
+  // (the entry points have already asked plan_check)
   *launched = false;
   FftPutParams pp;
   int C = 0;
@@ -1798,265 +1803,42 @@ pa_status put_fft(int nb, const BlockCopy* const* blocks, const void* src, void*
   if (mf) pp.mf = *mf;
   FftParams& p = pp.p;
   const int logL = p.logL;
-  const bool rfft = mode == PutMode::rfft;
   // r2r: the 10 kinds run k_r2r's forward path, the 01 kinds its backward one
-  const bool r2r_fwd = r2r_kind == PA_REDFT10 || r2r_kind == PA_RODFT10;
-  p.sign = rfft ? -1 : (sign < 0 ? -1 : 1);
-  p.tw = twiddles(mode == PutMode::fft ? p.L : 2 * p.L, f32);
-  if (mode == PutMode::r2r) {
-    p.sine = (r2r_kind == PA_RODFT10 || r2r_kind == PA_RODFT01) ? 1 : 0;
-    p.tw4 = twiddles(8 * p.L, f32);
+  const bool r2r_fwd = r2r_forward(r2r_kind);
+  p.sign = mode == FusedMode::rfft ? -1 : (sign < 0 ? -1 : 1);
+  void (*kern)(FftPutParams) = nullptr;
+  switch (mode) {
+    case FusedMode::fft:
+      kern = dispatch<true>(f32, logL, C, [](auto lg, auto c, auto t) { return k_fft_put<lg, c, decltype(t)>; });
+      break;
+    case FusedMode::rfft:
+      kern = dispatch(f32, logL, C, [](auto lg, auto c, auto t) { return k_rfft_put<lg, c, decltype(t)>; });
+      break;
+    case FusedMode::r2r:
+      p.sine = r2r_sine(r2r_kind) ? 1 : 0;
+      kern = dispatch(f32, logL, C, [r2r_fwd](auto lg, auto c, auto t) {
+        return r2r_fwd ? k_r2r_put<lg, c, true, decltype(t)> : k_r2r_put<lg, c, false, decltype(t)>;
+      });
+      break;
+    case FusedMode::brfft:
+      kern = dispatch(f32, logL, C, [](auto lg, auto c, auto t) { return k_brfft_put<lg, c, decltype(t)>; });
+      break;
   }
   // k_rfft (backward) and k_r2r (01 kinds) stage the pairs of slots 0..L
-  if (mode == PutMode::brfft || (mode == PutMode::r2r && !r2r_fwd)) p.pitch = pa_fft::padded_pitch(p.L + 1);
-  if (!p.tw || (mode == PutMode::r2r && !p.tw4)) {
-    set_error("fused put: twiddle table allocation failed");
-    cudaGetLastError();
-    return PA_ENOMEM;
-  }
-  const size_t smem = (f32 ? sizeof(pa_fft::cplxf) : sizeof(cplx)) * (size_t)C * p.pitch;
-  cudaError_t e = cudaSuccess;
-  auto launch = [&](auto kern) {
-    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout,
-                         cudaSharedmemCarveoutMaxShared);
-    cudaGetLastError();
-    kern<<<(unsigned)grid, FFT_THREADS, smem, (cudaStream_t)stream>>>(pp);
-    e = cudaGetLastError();
-  };
-  // the kernels of one line length and lines per CTA, by mode (and r2r direction)
-#define PUT_KERNELS(LG, CC, T)                                                                   \
-  switch (mode) {                                                                                \
-    case PutMode::fft: launch(k_fft_put<LG, CC, T>); break;                                      \
-    case PutMode::rfft: launch(k_rfft_put<LG, CC, T>); break;                                    \
-    case PutMode::r2r:                                                                           \
-      r2r_fwd ? launch(k_r2r_put<LG, CC, true, T>) : launch(k_r2r_put<LG, CC, false, T>);        \
-      break;                                                                                     \
-    case PutMode::brfft: launch(k_brfft_put<LG, CC, T>); break;                                  \
-  }
-  if (f32) {
-    switch (logL) {
-      case 3: PUT_KERNELS(3, 16, float) break;
-      case 4: PUT_KERNELS(4, 16, float) break;
-      case 5: PUT_KERNELS(5, 16, float) break;
-      case 6: PUT_KERNELS(6, 16, float) break;
-      case 7: PUT_KERNELS(7, 16, float) break;
-      case 8: PUT_KERNELS(8, 16, float) break;
-      case 9: PUT_KERNELS(9, 16, float) break;
-      default: PUT_KERNELS(10, 8, float) break;
-    }
-  } else {
-    switch (logL) {
-      case 3: PUT_KERNELS(3, 8, double) break;
-      case 4: PUT_KERNELS(4, 8, double) break;
-      case 5: PUT_KERNELS(5, 8, double) break;
-      case 6: PUT_KERNELS(6, 8, double) break;
-      case 7: PUT_KERNELS(7, 8, double) break;
-      case 8:
-        if (C == 4) launch(k_fft_put<8, 4, double>);  // (tunable fft_lines = 4: the complex FFT only)
-        else PUT_KERNELS(8, 8, double)
-        break;
-      case 9:
-        if (C == 4) launch(k_fft_put<9, 4, double>);
-        else PUT_KERNELS(9, 8, double)
-        break;
-      default: PUT_KERNELS(10, 4, double) break;
-    }
-  }
-#undef PUT_KERNELS
-  if (e != cudaSuccess) {
-    set_error("fused put kernel launch failed: %s", cudaGetErrorString(e));
-    return PA_ECUDA;
-  }
-  count_launch();
-  *launched = true;
-  return PA_OK;
+  if (mode == FusedMode::brfft || (mode == FusedMode::r2r && !r2r_fwd)) p.pitch = pa_fft::padded_pitch(p.L + 1);
+  s = line_twiddles("fused put", f32, mode == FusedMode::fft ? p.L : 2 * p.L, &p.tw,
+                    mode == FusedMode::r2r ? 8 * p.L : 0, &p.tw4);
+  if (s != PA_OK) return s;
+  s = launch_lines("fused put", kern, pp, grid, C, p.pitch, f32, stream);
+  *launched = s == PA_OK;
+  return s;
 }
 
-pa_status unpack_brfft(int nb, const BlockCopy* const* blocks, const void* const* srcs, void* dst,
-                       bool f32, void* stream) {
-  // (pa_transpose_brfft has already asked plan_brfft_check for every rank of the line)
-  FftParams p;
-  int C = 0;
-  unsigned long long grid = 0;
-  pa_status s = fft_geometry(nb, blocks, srcs, dst, f32, FusedMode::brfft, p, &C, &grid);
-  if (s != PA_OK || grid == 0) return s;
-  const int logL = p.logL;
-  p.sign = 1;
-  p.tw = twiddles(2 * p.L, f32);
-  if (!p.tw) {
-    set_error("fused brfft: twiddle table allocation failed");
-    cudaGetLastError();
-    return PA_ENOMEM;
-  }
-  const size_t smem = (f32 ? sizeof(pa_fft::cplxf) : sizeof(cplx)) * (size_t)C * p.pitch;
-  cudaError_t e = cudaSuccess;
-  auto launch = [&](auto kern) {
-    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout,
-                         cudaSharedmemCarveoutMaxShared);
-    cudaGetLastError();
-    kern<<<(unsigned)grid, FFT_THREADS, smem, (cudaStream_t)stream>>>(p);
-    e = cudaGetLastError();
-  };
-  if (f32) {
-    switch (logL) {
-      case 3: launch(k_unpack_brfft<3, 16, float>); break;
-      case 4: launch(k_unpack_brfft<4, 16, float>); break;
-      case 5: launch(k_unpack_brfft<5, 16, float>); break;
-      case 6: launch(k_unpack_brfft<6, 16, float>); break;
-      case 7: launch(k_unpack_brfft<7, 16, float>); break;
-      case 8: launch(k_unpack_brfft<8, 16, float>); break;
-      case 9: launch(k_unpack_brfft<9, 16, float>); break;
-      default: launch(k_unpack_brfft<10, 8, float>); break;
-    }
-  } else {
-    switch (logL) {
-      case 3: launch(k_unpack_brfft<3, 8, double>); break;
-      case 4: launch(k_unpack_brfft<4, 8, double>); break;
-      case 5: launch(k_unpack_brfft<5, 8, double>); break;
-      case 6: launch(k_unpack_brfft<6, 8, double>); break;
-      case 7: launch(k_unpack_brfft<7, 8, double>); break;
-      case 8: launch(k_unpack_brfft<8, 8, double>); break;
-      case 9: launch(k_unpack_brfft<9, 8, double>); break;
-      default: launch(k_unpack_brfft<10, 4, double>); break;
-    }
-  }
-  if (e != cudaSuccess) {
-    set_error("fused brfft kernel launch failed: %s", cudaGetErrorString(e));
-    return PA_ECUDA;
-  }
-  count_launch();
-  return PA_OK;
-}
-
-// kind: FFTW's REDFT10 (DCT-II), REDFT01 (DCT-III), RODFT10 (DST-II) or RODFT01 (DST-III)
-pa_status unpack_r2r(int nb, const BlockCopy* const* blocks, const void* const* srcs, void* dst,
-                     int kind, bool f32, void* stream) {
-  // (pa_transpose_r2r has already asked plan_real_check for every rank of the line)
-  const bool forward = kind == PA_REDFT10 || kind == PA_RODFT10;
-  FftParams p;
-  int C = 0;
-  unsigned long long grid = 0;
-  pa_status s = fft_geometry(nb, blocks, srcs, dst, f32, FusedMode::r2r, p, &C, &grid);
-  if (s != PA_OK || grid == 0) return s;
-  const int logL = p.logL, N = 2 * p.L;
-  p.pitch = pa_fft::padded_pitch(forward ? p.L : p.L + 1);  // as r2r_lines
-  p.sine = (kind == PA_RODFT10 || kind == PA_RODFT01) ? 1 : 0;
-  p.tw = twiddles(N, f32);
-  p.tw4 = twiddles(4 * N, f32);
-  if (!p.tw || !p.tw4) {
-    set_error("fused r2r: twiddle table allocation failed");
-    cudaGetLastError();
-    return PA_ENOMEM;
-  }
-  const size_t smem = (f32 ? sizeof(pa_fft::cplxf) : sizeof(cplx)) * (size_t)C * p.pitch;
-  cudaError_t e = cudaSuccess;
-  auto launch = [&](auto kern) {
-    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout,
-                         cudaSharedmemCarveoutMaxShared);
-    cudaGetLastError();
-    kern<<<(unsigned)grid, FFT_THREADS, smem, (cudaStream_t)stream>>>(p);
-    e = cudaGetLastError();
-  };
-  auto launch_dir = [&](auto fwd_kern, auto bwd_kern) { forward ? launch(fwd_kern) : launch(bwd_kern); };
-  if (f32) {
-    switch (logL) {
-      case 3: launch_dir(k_unpack_r2r<3, 16, true, float>, k_unpack_r2r<3, 16, false, float>); break;
-      case 4: launch_dir(k_unpack_r2r<4, 16, true, float>, k_unpack_r2r<4, 16, false, float>); break;
-      case 5: launch_dir(k_unpack_r2r<5, 16, true, float>, k_unpack_r2r<5, 16, false, float>); break;
-      case 6: launch_dir(k_unpack_r2r<6, 16, true, float>, k_unpack_r2r<6, 16, false, float>); break;
-      case 7: launch_dir(k_unpack_r2r<7, 16, true, float>, k_unpack_r2r<7, 16, false, float>); break;
-      case 8: launch_dir(k_unpack_r2r<8, 16, true, float>, k_unpack_r2r<8, 16, false, float>); break;
-      case 9: launch_dir(k_unpack_r2r<9, 16, true, float>, k_unpack_r2r<9, 16, false, float>); break;
-      default: launch_dir(k_unpack_r2r<10, 8, true, float>, k_unpack_r2r<10, 8, false, float>); break;
-    }
-  } else {
-    switch (logL) {
-      case 3: launch_dir(k_unpack_r2r<3, 8, true, double>, k_unpack_r2r<3, 8, false, double>); break;
-      case 4: launch_dir(k_unpack_r2r<4, 8, true, double>, k_unpack_r2r<4, 8, false, double>); break;
-      case 5: launch_dir(k_unpack_r2r<5, 8, true, double>, k_unpack_r2r<5, 8, false, double>); break;
-      case 6: launch_dir(k_unpack_r2r<6, 8, true, double>, k_unpack_r2r<6, 8, false, double>); break;
-      case 7: launch_dir(k_unpack_r2r<7, 8, true, double>, k_unpack_r2r<7, 8, false, double>); break;
-      case 8: launch_dir(k_unpack_r2r<8, 8, true, double>, k_unpack_r2r<8, 8, false, double>); break;
-      case 9: launch_dir(k_unpack_r2r<9, 8, true, double>, k_unpack_r2r<9, 8, false, double>); break;
-      default: launch_dir(k_unpack_r2r<10, 4, true, double>, k_unpack_r2r<10, 4, false, double>); break;
-    }
-  }
-  if (e != cudaSuccess) {
-    set_error("fused r2r kernel launch failed: %s", cudaGetErrorString(e));
-    return PA_ECUDA;
-  }
-  count_launch();
-  return PA_OK;
-}
-
-pa_status unpack_rfft(int nb, const BlockCopy* const* blocks, const void* const* srcs, void* dst,
-                      bool f32, void* stream) {
-  // (pa_transpose_rfft has already asked plan_real_check for every rank of the line)
-  FftParams p;
-  int C = 0;
-  unsigned long long grid = 0;
-  pa_status s = fft_geometry(nb, blocks, srcs, dst, f32, FusedMode::rfft, p, &C, &grid);
-  if (s != PA_OK || grid == 0) return s;
-  const int logL = p.logL;
-  p.pitch = pa_fft::padded_pitch(p.L);  // as rfft_lines, forward
-  p.tw = twiddles(2 * p.L, f32);
-  if (!p.tw) {
-    set_error("fused rfft: twiddle table allocation failed");
-    cudaGetLastError();
-    return PA_ENOMEM;
-  }
-  const size_t smem = (f32 ? sizeof(pa_fft::cplxf) : sizeof(cplx)) * (size_t)C * p.pitch;
-  cudaError_t e = cudaSuccess;
-  auto launch = [&](auto kern) {
-    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout,
-                         cudaSharedmemCarveoutMaxShared);
-    cudaGetLastError();
-    kern<<<(unsigned)grid, FFT_THREADS, smem, (cudaStream_t)stream>>>(p);
-    e = cudaGetLastError();
-  };
-  if (f32) {
-    switch (logL) {
-      case 3: launch(k_unpack_rfft<3, 16, float>); break;
-      case 4: launch(k_unpack_rfft<4, 16, float>); break;
-      case 5: launch(k_unpack_rfft<5, 16, float>); break;
-      case 6: launch(k_unpack_rfft<6, 16, float>); break;
-      case 7: launch(k_unpack_rfft<7, 16, float>); break;
-      case 8: launch(k_unpack_rfft<8, 16, float>); break;
-      case 9: launch(k_unpack_rfft<9, 16, float>); break;
-      default: launch(k_unpack_rfft<10, 8, float>); break;
-    }
-  } else {
-    switch (logL) {
-      case 3: launch(k_unpack_rfft<3, 8, double>); break;
-      case 4: launch(k_unpack_rfft<4, 8, double>); break;
-      case 5: launch(k_unpack_rfft<5, 8, double>); break;
-      case 6: launch(k_unpack_rfft<6, 8, double>); break;
-      case 7: launch(k_unpack_rfft<7, 8, double>); break;
-      case 8: launch(k_unpack_rfft<8, 8, double>); break;
-      case 9: launch(k_unpack_rfft<9, 8, double>); break;
-      default: launch(k_unpack_rfft<10, 4, double>); break;
-    }
-  }
-  if (e != cudaSuccess) {
-    set_error("fused rfft kernel launch failed: %s", cudaGetErrorString(e));
-    return PA_ECUDA;
-  }
-  count_launch();
-  return PA_OK;
-}
-
-// Can pa_transpose fuse the FFT (brfft: pa_transpose_brfft the complex-to-real transform) into
-// this plan's unpack?  Every rank of a grid line must get the same answer: a rank that refused
-// before the exchange while its peers went ahead would leave them waiting on flags it never
-// sets.  So the answer depends on the global geometry only: the blocks that EVERY rank of the
-// line would gather -- each rank's plan rebuilt from the pencils with that rank's coordinates --
-// with the self block read from src and staged through recv_buf alike.  A PeerGet plan may also
-// run the complex FFT one-sided (k_get_fft): its blocks are then the peers' get blocks, read from
-// their src arrays, and the self block from src, so that configuration is checked as well.
+// Every rank of a grid line must get the same verdict from plan_check: a rank that refused before
+// the exchange while its peers went ahead would leave them waiting on flags it never sets.  So the
+// answer depends on the global geometry only: the blocks that EVERY rank of the line would gather
+// (receive side) or store (send side) -- each rank's plan rebuilt from the pencils with that rank's
+// coordinates.
 // The plan rank n of P's grid line holds: P itself for this rank, else rebuilt from the pencils
 // with that rank's coordinates (owned by `hold`).
 static pa_status line_plan(Plan* P, int n, std::unique_ptr<Plan>& hold, const Plan** Q) {
@@ -2077,8 +1859,40 @@ static pa_status line_plan(Plan* P, int n, std::unique_ptr<Plan>& hold, const Pl
   return PA_OK;
 }
 
+// geometry(Q) for the plan Q of every rank of P's grid line; a refusal for another rank names it
+template <class F>
+static pa_status every_line_rank(Plan* P, F&& geometry) {
+  for (int n = 0; n < P->nproc; ++n) {
+    std::unique_ptr<Plan> hold;
+    const Plan* Q = nullptr;
+    pa_status s = line_plan(P, n, hold, &Q);
+    if (s != PA_OK) return s;
+    s = geometry(*Q);
+    if (s != PA_OK) {
+      if (n != P->self_index) {
+        const std::string why = last_error();
+        set_error("%s (on rank %d of the grid line)", why.c_str(), n + 1);
+      }
+      return s;
+    }
+  }
+  return PA_OK;
+}
+
+// Can the receive side (unpack_fused; for the complex FFT on a PeerGet plan also get_fft) run
+// `mode` on this plan?  The blocks of every rank are checked with the self block read from src and
+// staged through recv_buf alike; a PeerGet plan may also run the complex FFT one-sided (k_get_fft):
+// its blocks are then the peers' get blocks, read from their src arrays, and the self block from
+// src, so that configuration is checked as well.
 static pa_status fused_check(Plan* P, bool f32, FusedMode mode) {
-  if (mode == FusedMode::r2r || mode == FusedMode::rfft) {
+  const bool exchange = P->dim >= 0 && P->nproc > 1;
+  if (mode != FusedMode::fft && exchange && (P->method == PA_PEER_PUT || P->method == PA_PEER_GET)) {
+    // (src and dst never alias, so these methods never fall back to a staged schedule)
+    set_error("%s: the one-sided methods have no unpack pass to fuse with; use PointToPoint / Alltoallv",
+              mode == FusedMode::brfft ? "fused brfft" : "fused real transform");
+    return PA_EINVAL;
+  }
+  if (unpack_moves_reals(mode)) {
     if (P->elsize != (f32 ? 4 : 8)) {
       set_error(f32 ? "fused real transform: PA_FFT_F32 takes Float32 (4-byte) elements only"
                     : "fused real transform: Float64 (8-byte) elements only");
@@ -2094,102 +1908,32 @@ static pa_status fused_check(Plan* P, bool f32, FusedMode mode) {
   FftParams p;
   int C = 0;
   unsigned long long grid = 0;
-  if (P->dim < 0 || P->nproc == 1) {
+  if (!exchange) {
     const BlockCopy* b = &P->self_fused;
     return fft_geometry(1, &b, nullptr, nullptr, f32, mode, p, &C, &grid);
   }
-  for (int n = 0; n < P->nproc; ++n) {
-    std::unique_ptr<Plan> hold;
-    const Plan* Q = nullptr;
-    {
-      pa_status s = line_plan(P, n, hold, &Q);
-      if (s != PA_OK) return s;
-    }
-    // 0: self block from src, 1: self block staged through recv_buf, 2: one-sided get
-    const int configs = (mode == FusedMode::fft && P->method == PA_PEER_GET) ? 3 : 2;
+  // 0: self block from src, 1: self block staged through recv_buf, 2: one-sided get
+  const int configs = (mode == FusedMode::fft && P->method == PA_PEER_GET) ? 3 : 2;
+  return every_line_rank(P, [&](const Plan& Q) {
     for (int cfg = 0; cfg < configs; ++cfg) {
       std::vector<const BlockCopy*> bl;
-      for (int k = 0; k < Q->nproc; ++k)
-        bl.push_back(k == Q->self_index && cfg != 1 ? &Q->self_fused
-                                                    : cfg == 2 ? &Q->peers[k].get : &Q->peers[k].unpack);
-      pa_status s = fft_geometry(Q->nproc, bl.data(), nullptr, nullptr, f32, mode, p, &C, &grid);
-      if (s != PA_OK) {
-        if (n != P->self_index) {
-          const std::string why = last_error();
-          set_error("%s (on rank %d of the grid line)", why.c_str(), n + 1);
-        }
-        return s;
-      }
+      for (int k = 0; k < Q.nproc; ++k)
+        bl.push_back(k == Q.self_index && cfg != 1 ? &Q.self_fused
+                                                   : cfg == 2 ? &Q.peers[k].get : &Q.peers[k].unpack);
+      pa_status s = fft_geometry(Q.nproc, bl.data(), nullptr, nullptr, f32, mode, p, &C, &grid);
+      if (s != PA_OK) return s;
     }
-  }
-  return PA_OK;
+    return PA_OK;
+  });
 }
 
-// Cached per plan, per precision (f32: ComplexF32) and per value of tunable fft_lines.
-pa_status plan_fft_check(Plan* P, bool f32) {
-  const int q = f32 ? 1 : 0;
-  if (P->fft_check_lines[q] != g_tun.fft_lines) {
-    P->fft_check[q] = fused_check(P, f32, FusedMode::fft);
-    P->fft_check_err[q] = P->fft_check[q] == PA_OK ? std::string() : std::string(last_error());
-    P->fft_check_lines[q] = g_tun.fft_lines;
-  } else if (P->fft_check[q] != PA_OK) {
-    set_error("%s", P->fft_check_err[q].c_str());
-  }
-  return P->fft_check[q];
-}
-
-// Cached per plan and per precision, apart from plan_fft_check's verdicts (the lines per CTA of
-// the brfft kernel do not depend on tunable fft_lines).
-pa_status plan_brfft_check(Plan* P, bool f32) {
-  const int q = f32 ? 1 : 0;
-  if (!P->brfft_checked[q]) {
-    if (P->dim >= 0 && P->nproc > 1 && (P->method == PA_PEER_PUT || P->method == PA_PEER_GET)) {
-      // (src and the real dst never alias, so these methods never fall back to a staged schedule)
-      set_error("fused brfft: the one-sided methods have no unpack pass to fuse with; use "
-                "PointToPoint / Alltoallv");
-      P->brfft_check[q] = PA_EINVAL;
-    } else {
-      P->brfft_check[q] = fused_check(P, f32, FusedMode::brfft);
-    }
-    P->brfft_check_err[q] = P->brfft_check[q] == PA_OK ? std::string() : std::string(last_error());
-    P->brfft_checked[q] = true;
-  } else if (P->brfft_check[q] != PA_OK) {
-    set_error("%s", P->brfft_check_err[q].c_str());
-  }
-  return P->brfft_check[q];
-}
-
-// Can pa_transpose_r2r / pa_transpose_rfft run on this real plan?  Both kernels gather the same
-// blocks (N reals per line), so one verdict answers for both: the rfft geometry, which checks
-// everything the r2r geometry does plus the rescale of the destination to N/2 + 1 bins per line.
-// Cached per plan and per precision, apart from the fft and brfft verdicts.
-pa_status plan_real_check(Plan* P, bool f32) {
-  const int q = f32 ? 1 : 0;
-  if (!P->real_checked[q]) {
-    if (P->dim >= 0 && P->nproc > 1 && (P->method == PA_PEER_PUT || P->method == PA_PEER_GET)) {
-      // (src and dst never overlap, so these methods never fall back to a staged schedule)
-      set_error("fused real transform: the one-sided methods have no unpack pass to fuse with; "
-                "use PointToPoint / Alltoallv");
-      P->real_check[q] = PA_EINVAL;
-    } else {
-      P->real_check[q] = fused_check(P, f32, FusedMode::rfft);
-    }
-    P->real_check_err[q] = P->real_check[q] == PA_OK ? std::string() : std::string(last_error());
-    P->real_checked[q] = true;
-  } else if (P->real_check[q] != PA_OK) {
-    set_error("%s", P->real_check_err[q].c_str());
-  }
-  return P->real_check[q];
-}
-
-// Can pa_fft_put (rfft: pa_rfft_put; brfft: pa_r2r_put and pa_brfft_put) run on this plan?  The
-// send-side kernel runs on PeerPut plans and on local transposes (no exchange, or a line of one
-// rank) of any method.  As fused_check, every rank of the grid line gets the same answer: its plan
-// is rebuilt and its blocks -- the self block and the put blocks -- checked.
-static pa_status put_check(Plan* P, bool f32, PutMode mode) {
-  const bool real = mode == PutMode::r2r || mode == PutMode::brfft;
+// Can the send side (put_fft) run `mode` on this plan?  The send-side kernel runs on PeerPut plans
+// and on local transposes (no exchange, or a line of one rank) of any method.  The blocks of every
+// rank -- the self block and the put blocks -- are checked.
+static pa_status put_check(Plan* P, bool f32, FusedMode mode) {
+  const bool real = put_moves_reals(mode);
   const char* what = real ? "fused real transform + put"
-                          : mode == PutMode::rfft ? "fused rfft + put" : "fused FFT + put";
+                          : mode == FusedMode::rfft ? "fused rfft + put" : "fused FFT + put";
   if (real && P->elsize != (f32 ? 4 : 8)) {
     set_error(f32 ? "%s: PA_FFT_F32 takes a Float32 (elsize 4) plan"
                   : "%s: a Float64 (elsize 8) plan, or PA_FFT_F32 for Float32", what);
@@ -2225,65 +1969,31 @@ static pa_status put_check(Plan* P, bool f32, PutMode mode) {
                 "into the receive side (pa_transpose with PA_FFT_FORWARD / PA_FFT_BACKWARD)", what);
     return PA_EINVAL;
   }
-  for (int n = 0; n < P->nproc; ++n) {
-    std::unique_ptr<Plan> hold;
-    const Plan* Q = nullptr;
-    pa_status s = line_plan(P, n, hold, &Q);
-    if (s != PA_OK) return s;
+  return every_line_rank(P, [&](const Plan& Q) {
     std::vector<const BlockCopy*> bl;
-    for (int k = 0; k < Q->nproc; ++k)
-      bl.push_back(k == Q->self_index ? &Q->self_fused : &Q->peers[k].put);
-    s = put_fft_geometry(Q->nproc, bl.data(), nullptr, nullptr, f32, mode, pp, &C, &grid);
-    if (s != PA_OK) {
-      if (n != P->self_index) {
-        const std::string why = last_error();
-        set_error("%s (on rank %d of the grid line)", why.c_str(), n + 1);
-      }
-      return s;
-    }
-  }
-  return PA_OK;
+    for (int k = 0; k < Q.nproc; ++k)
+      bl.push_back(k == Q.self_index ? &Q.self_fused : &Q.peers[k].put);
+    return put_fft_geometry(Q.nproc, bl.data(), nullptr, nullptr, f32, mode, pp, &C, &grid);
+  });
 }
 
-// Cached per plan, per precision and (lines per CTA of fft_) per value of tunable fft_lines, apart
-// from every other verdict.
-pa_status plan_fft_put_check(Plan* P, bool f32) {
-  const int q = f32 ? 1 : 0;
-  if (P->fft_put_check_lines[q] != g_tun.fft_lines) {
-    P->fft_put_check[q] = put_check(P, f32, PutMode::fft);
-    P->fft_put_check_err[q] = P->fft_put_check[q] == PA_OK ? std::string() : std::string(last_error());
-    P->fft_put_check_lines[q] = g_tun.fft_lines;
-  } else if (P->fft_put_check[q] != PA_OK) {
-    set_error("%s", P->fft_put_check_err[q].c_str());
+pa_status plan_check(Plan* P, Side side, FusedMode mode, bool f32) {
+  // r2r shares the verdict of its sibling, whose geometry checks all that r2r's does plus the
+  // rescale between N reals and N/2 + 1 bins: rfft on the receive side, brfft on the send side
+  if (mode == FusedMode::r2r) mode = side == Side::unpack ? FusedMode::rfft : FusedMode::brfft;
+  const int question = (side == Side::put ? 3 : 0) +
+                       (mode == FusedMode::fft ? 0 : mode == FusedMode::rfft ? 1 : 2);
+  Verdict& v = P->verdicts[question][f32 ? 1 : 0];
+  // the complex FFT's lines per CTA, and so its geometry, depend on tunable fft_lines
+  const int key = mode == FusedMode::fft ? g_tun.fft_lines : 0;
+  if (v.key != key) {
+    v.status = side == Side::unpack ? fused_check(P, f32, mode) : put_check(P, f32, mode);
+    v.err = v.status == PA_OK ? std::string() : std::string(last_error());
+    v.key = key;
+  } else if (v.status != PA_OK) {
+    set_error("%s", v.err.c_str());
   }
-  return P->fft_put_check[q];
-}
-
-// Cached per plan and per precision, apart from every other verdict.
-pa_status plan_rfft_put_check(Plan* P, bool f32) {
-  const int q = f32 ? 1 : 0;
-  if (!P->rfft_put_checked[q]) {
-    P->rfft_put_check[q] = put_check(P, f32, PutMode::rfft);
-    P->rfft_put_check_err[q] = P->rfft_put_check[q] == PA_OK ? std::string() : std::string(last_error());
-    P->rfft_put_checked[q] = true;
-  } else if (P->rfft_put_check[q] != PA_OK) {
-    set_error("%s", P->rfft_put_check_err[q].c_str());
-  }
-  return P->rfft_put_check[q];
-}
-
-// One verdict for pa_r2r_put and pa_brfft_put (the brfft geometry checks all that r2r's does, and
-// its rescale); cached per plan and per precision, apart from every other verdict.
-pa_status plan_real_put_check(Plan* P, bool f32) {
-  const int q = f32 ? 1 : 0;
-  if (!P->real_put_checked[q]) {
-    P->real_put_check[q] = put_check(P, f32, PutMode::brfft);
-    P->real_put_check_err[q] = P->real_put_check[q] == PA_OK ? std::string() : std::string(last_error());
-    P->real_put_checked[q] = true;
-  } else if (P->real_put_check[q] != PA_OK) {
-    set_error("%s", P->real_put_check_err[q].c_str());
-  }
-  return P->real_put_check[q];
+  return v.status;
 }
 
 pa_status rfft_lines(int N, bool forward, bool f32, i64 nlines, const void* src, void* dst,
@@ -2304,58 +2014,18 @@ pa_status rfft_lines(int N, bool forward, bool f32, i64 nlines, const void* src,
   p.src_line = forward ? rs * N : cs * (L + 1);
   p.dst_line = forward ? cs * (L + 1) : rs * N;
   p.pitch = pa_fft::padded_pitch(forward ? L : L + 1);  // backward stages all N/2 + 1 bins
-  p.tw = twiddles(N, f32);
-  if (!p.tw) {
-    set_error("rfft: twiddle table allocation failed");
-    cudaGetLastError();
-    return PA_ENOMEM;
-  }
-  const int C = f32 ? fft_lines_f32(logL) : fft_lines(logL);
+  pa_status s = line_twiddles("rfft", f32, N, &p.tw);
+  if (s != PA_OK) return s;
+  const int C = lines_per_cta(f32, logL, false);
   const long long grid = (nlines + C - 1) / C;
   if (grid > 0x7fffffffLL) {
     set_error("rfft: too many lines for one launch");
     return PA_EINVAL;
   }
-  const size_t smem = (size_t)cs * C * p.pitch;
-  cudaError_t e = cudaSuccess;
-  auto launch = [&](auto kern) {
-    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout,
-                         cudaSharedmemCarveoutMaxShared);
-    cudaGetLastError();
-    kern<<<(unsigned)grid, FFT_THREADS, smem, (cudaStream_t)stream>>>(p);
-    e = cudaGetLastError();
-  };
-  auto launch_dir = [&](auto fwd_kern, auto bwd_kern) { forward ? launch(fwd_kern) : launch(bwd_kern); };
-  if (f32) {
-    switch (logL) {
-      case 3: launch_dir(k_rfft<3, 16, true, float>, k_rfft<3, 16, false, float>); break;
-      case 4: launch_dir(k_rfft<4, 16, true, float>, k_rfft<4, 16, false, float>); break;
-      case 5: launch_dir(k_rfft<5, 16, true, float>, k_rfft<5, 16, false, float>); break;
-      case 6: launch_dir(k_rfft<6, 16, true, float>, k_rfft<6, 16, false, float>); break;
-      case 7: launch_dir(k_rfft<7, 16, true, float>, k_rfft<7, 16, false, float>); break;
-      case 8: launch_dir(k_rfft<8, 16, true, float>, k_rfft<8, 16, false, float>); break;
-      case 9: launch_dir(k_rfft<9, 16, true, float>, k_rfft<9, 16, false, float>); break;
-      default: launch_dir(k_rfft<10, 8, true, float>, k_rfft<10, 8, false, float>); break;
-    }
-  } else {
-    switch (logL) {
-      case 3: launch_dir(k_rfft<3, 8, true, double>, k_rfft<3, 8, false, double>); break;
-      case 4: launch_dir(k_rfft<4, 8, true, double>, k_rfft<4, 8, false, double>); break;
-      case 5: launch_dir(k_rfft<5, 8, true, double>, k_rfft<5, 8, false, double>); break;
-      case 6: launch_dir(k_rfft<6, 8, true, double>, k_rfft<6, 8, false, double>); break;
-      case 7: launch_dir(k_rfft<7, 8, true, double>, k_rfft<7, 8, false, double>); break;
-      case 8: launch_dir(k_rfft<8, 8, true, double>, k_rfft<8, 8, false, double>); break;
-      case 9: launch_dir(k_rfft<9, 8, true, double>, k_rfft<9, 8, false, double>); break;
-      default: launch_dir(k_rfft<10, 4, true, double>, k_rfft<10, 4, false, double>); break;
-    }
-  }
-  if (e != cudaSuccess) {
-    set_error("rfft kernel launch failed: %s", cudaGetErrorString(e));
-    return PA_ECUDA;
-  }
-  count_launch();
-  return PA_OK;
+  auto kern = dispatch(f32, logL, C, [forward](auto lg, auto c, auto t) {
+    return forward ? k_rfft<lg, c, true, decltype(t)> : k_rfft<lg, c, false, decltype(t)>;
+  });
+  return launch_lines("rfft", kern, p, grid, C, p.pitch, f32, stream);
 }
 
 pa_status r2r_lines(int N, bool forward, bool sine, bool f32, i64 nlines, const void* src, void* dst,
@@ -2372,63 +2042,22 @@ pa_status r2r_lines(int N, bool forward, bool sine, bool f32, i64 nlines, const 
   p.src = (const char*)src;
   p.dst = (char*)dst;
   p.nlines = nlines;
-  const long long rs = f32 ? 4 : 8, cs = 2 * rs;  // bytes of a real / a complex element
+  const long long rs = f32 ? 4 : 8;  // bytes of a real element
   p.line = rs * N;
   p.pitch = pa_fft::padded_pitch(forward ? L : L + 1);  // backward stages the pairs of slots 0..L
   p.sine = sine ? 1 : 0;
-  p.tw = twiddles(N, f32);
-  p.tw4 = twiddles(4 * N, f32);
-  if (!p.tw || !p.tw4) {
-    set_error("r2r: twiddle table allocation failed");
-    cudaGetLastError();
-    return PA_ENOMEM;
-  }
-  const int C = f32 ? fft_lines_f32(logL) : fft_lines(logL);
+  pa_status s = line_twiddles("r2r", f32, N, &p.tw, 4 * N, &p.tw4);
+  if (s != PA_OK) return s;
+  const int C = lines_per_cta(f32, logL, false);
   const long long grid = (nlines + C - 1) / C;
   if (grid > 0x7fffffffLL) {
     set_error("r2r: too many lines for one launch");
     return PA_EINVAL;
   }
-  const size_t smem = (size_t)cs * C * p.pitch;
-  cudaError_t e = cudaSuccess;
-  auto launch = [&](auto kern) {
-    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout,
-                         cudaSharedmemCarveoutMaxShared);
-    cudaGetLastError();
-    kern<<<(unsigned)grid, FFT_THREADS, smem, (cudaStream_t)stream>>>(p);
-    e = cudaGetLastError();
-  };
-  auto launch_dir = [&](auto fwd_kern, auto bwd_kern) { forward ? launch(fwd_kern) : launch(bwd_kern); };
-  if (f32) {
-    switch (logL) {
-      case 3: launch_dir(k_r2r<3, 16, true, float>, k_r2r<3, 16, false, float>); break;
-      case 4: launch_dir(k_r2r<4, 16, true, float>, k_r2r<4, 16, false, float>); break;
-      case 5: launch_dir(k_r2r<5, 16, true, float>, k_r2r<5, 16, false, float>); break;
-      case 6: launch_dir(k_r2r<6, 16, true, float>, k_r2r<6, 16, false, float>); break;
-      case 7: launch_dir(k_r2r<7, 16, true, float>, k_r2r<7, 16, false, float>); break;
-      case 8: launch_dir(k_r2r<8, 16, true, float>, k_r2r<8, 16, false, float>); break;
-      case 9: launch_dir(k_r2r<9, 16, true, float>, k_r2r<9, 16, false, float>); break;
-      default: launch_dir(k_r2r<10, 8, true, float>, k_r2r<10, 8, false, float>); break;
-    }
-  } else {
-    switch (logL) {
-      case 3: launch_dir(k_r2r<3, 8, true, double>, k_r2r<3, 8, false, double>); break;
-      case 4: launch_dir(k_r2r<4, 8, true, double>, k_r2r<4, 8, false, double>); break;
-      case 5: launch_dir(k_r2r<5, 8, true, double>, k_r2r<5, 8, false, double>); break;
-      case 6: launch_dir(k_r2r<6, 8, true, double>, k_r2r<6, 8, false, double>); break;
-      case 7: launch_dir(k_r2r<7, 8, true, double>, k_r2r<7, 8, false, double>); break;
-      case 8: launch_dir(k_r2r<8, 8, true, double>, k_r2r<8, 8, false, double>); break;
-      case 9: launch_dir(k_r2r<9, 8, true, double>, k_r2r<9, 8, false, double>); break;
-      default: launch_dir(k_r2r<10, 4, true, double>, k_r2r<10, 4, false, double>); break;
-    }
-  }
-  if (e != cudaSuccess) {
-    set_error("r2r kernel launch failed: %s", cudaGetErrorString(e));
-    return PA_ECUDA;
-  }
-  count_launch();
-  return PA_OK;
+  auto kern = dispatch(f32, logL, C, [forward](auto lg, auto c, auto t) {
+    return forward ? k_r2r<lg, c, true, decltype(t)> : k_r2r<lg, c, false, decltype(t)>;
+  });
+  return launch_lines("r2r", kern, p, grid, C, p.pitch, f32, stream);
 }
 
 }  // namespace pa

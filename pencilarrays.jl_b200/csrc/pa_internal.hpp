@@ -194,6 +194,13 @@ struct Peer {
 
 struct TransposeState;  // streams/events, defined in transpose.cpp
 
+// one cached answer of plan_check: valid while `key` is the tunable it depends on (-1: not asked)
+struct Verdict {
+  int key = -1;
+  pa_status status = PA_OK;
+  std::string err;  // last_error() of a refusal
+};
+
 struct Plan {
   std::shared_ptr<Pencil> pin, pout;
   int n_extra = 0;
@@ -220,32 +227,8 @@ struct Plan {
   void* h_src_dev = nullptr;
   void* h_dst_dev = nullptr;
   i64 h_src_cap = 0, h_dst_cap = 0;
-  // cached answers of plan_fft_check, [0] ComplexF64 and [1] ComplexF32 (PA_FFT_F32), each
-  // valid while tunable fft_lines == fft_check_lines[i]
-  int fft_check_lines[2] = {-1, -1};
-  pa_status fft_check[2] = {PA_OK, PA_OK};
-  std::string fft_check_err[2];
-  // cached answers of plan_brfft_check, [0] ComplexF64 -> Float64, [1] ComplexF32 -> Float32
-  bool brfft_checked[2] = {false, false};
-  pa_status brfft_check[2] = {PA_OK, PA_OK};
-  std::string brfft_check_err[2];
-  // cached answers of plan_real_check, [0] Float64 and [1] Float32 (PA_FFT_F32)
-  bool real_checked[2] = {false, false};
-  pa_status real_check[2] = {PA_OK, PA_OK};
-  std::string real_check_err[2];
-  // cached answers of plan_fft_put_check ([0] ComplexF64, [1] ComplexF32; each valid while tunable
-  // fft_lines == fft_put_check_lines[i]) and of plan_rfft_put_check ([0] Float64 -> ComplexF64,
-  // [1] Float32 -> ComplexF32)
-  int fft_put_check_lines[2] = {-1, -1};
-  pa_status fft_put_check[2] = {PA_OK, PA_OK};
-  std::string fft_put_check_err[2];
-  bool rfft_put_checked[2] = {false, false};
-  pa_status rfft_put_check[2] = {PA_OK, PA_OK};
-  std::string rfft_put_check_err[2];
-  // cached answers of plan_real_put_check, [0] Float64 and [1] Float32 (PA_FFT_F32)
-  bool real_put_checked[2] = {false, false};
-  pa_status real_put_check[2] = {PA_OK, PA_OK};
-  std::string real_put_check_err[2];
+  // cached answers of plan_check, [question][0: Float64 / ComplexF64, 1: PA_FFT_F32]
+  Verdict verdicts[6][2];
   ~Plan();
 };
 
@@ -261,13 +244,24 @@ void comm_destroy(Comm* c);
 pa_status comm_flags_export(Comm* c, void* handle64, i64* offset);
 pa_status comm_flags_import(Comm* c, int rank, const void* handle64, i64 offset);
 
-// What the fused unpack of a transposition computes from the gathered lines
+// What a fused line kernel computes: from the lines it gathers on the receive side of a
+// transposition (unpack_fused, get_fft) or from the source lines it loads on the send side
+// (put_fft).  A plan moves the elements of one side; the array on the other side of the transform
+// may have the other element type.
 enum class FusedMode {
-  fft,    // the complex FFT (pa_transpose with PA_FFT_FORWARD / PA_FFT_BACKWARD)
-  brfft,  // N/2 + 1 complex bins -> N reals (pa_transpose_brfft, unpack_brfft)
-  r2r,    // N reals -> N reals, a DCT / DST (pa_transpose_r2r, unpack_r2r)
-  rfft,   // N reals -> N/2 + 1 complex bins (pa_transpose_rfft, unpack_rfft)
+  fft,    // the complex FFT: complex arrays on both sides
+  rfft,   // N reals -> N/2 + 1 complex bins
+  r2r,    // N reals -> N reals, a DCT / DST
+  brfft,  // N/2 + 1 complex bins -> N reals
 };
+// the plan moves reals: the destination's on the receive side, the source's on the send side
+inline bool unpack_moves_reals(FusedMode m) { return m == FusedMode::r2r || m == FusedMode::rfft; }
+inline bool put_moves_reals(FusedMode m) { return m == FusedMode::r2r || m == FusedMode::brfft; }
+
+// FFTW's r2r kinds: PA_REDFT10 (DCT-II) and PA_RODFT10 (DST-II) run forward, PA_REDFT01 (DCT-III)
+// and PA_RODFT01 (DST-III) backward; the RODFT kinds are the sine transforms
+inline bool r2r_forward(int kind) { return kind == PA_REDFT10 || kind == PA_RODFT10; }
+inline bool r2r_sine(int kind) { return kind == PA_RODFT10 || kind == PA_RODFT01; }
 
 // mode brfft / r2r / rfft: dst = brfft / r2r / rfft(transpose(src)) through the fused unpack;
 // flags then hold no FFT direction, PA_FFT_F32 selects the precision; r2r_kind: the PA_*ODFT*
@@ -298,48 +292,22 @@ pa_status host_chain_buffer(HostChain* c, int slot, int which, void** p, i64* by
 pa_status host_chain_time_begin(HostChain* c);
 pa_status host_chain_time_end(HostChain* c, float* ms);
 
-// fused unpack + 1-d FFT along the destination's contiguous dim (fft.cu): the blocks
-// together tile the destination box; srcs[i] = base pointer blocks[i] reads from.
-// f32: ComplexF32 elements and fp32 arithmetic (PA_FFT_F32), else ComplexF64
-pa_status unpack_fft(int nb, const BlockCopy* const* blocks, const void* const* srcs, void* dst,
-                     int sign, bool f32, void* stream);
-// the same kernel one-sided (fft.cu, k_get_fft): srcs[i] are the peers' src arrays as mapped here
-// (the self block's: the local src), read in place, and `mf` (NULL: none) the window protocol
-// spoken inside the launch.  *launched = false: this rank has no destination lines and nothing
-// was launched -- the caller then speaks the protocol with flag kernels
+// fused unpack + line transform along the destination's contiguous dim (fft.cu, k_unpack_fft /
+// k_unpack_rfft / k_unpack_r2r / k_unpack_brfft): the blocks together tile the destination box;
+// srcs[i] = base pointer blocks[i] reads from.  The plan's elements: fft ComplexF64, rfft / r2r
+// Float64, brfft ComplexF64, or their single-precision counterparts with f32 (PA_FFT_F32).  fft:
+// sign -1 forward, +1 backward.  rfft: `dst` is the complex array of N/2 + 1 bins per line that
+// replaces the real destination (same layout otherwise); brfft: `dst` is the real array of N reals
+// per line that replaces the complex one.  r2r: r2r_kind one of PA_REDFT10 / PA_REDFT01 /
+// PA_RODFT10 / PA_RODFT01
+pa_status unpack_fused(int nb, const BlockCopy* const* blocks, const void* const* srcs, void* dst, int sign,
+                       FusedMode mode, int r2r_kind, bool f32, void* stream);
+// the complex FFT's kernel one-sided (fft.cu, k_get_fft): srcs[i] are the peers' src arrays as
+// mapped here (the self block's: the local src), read in place, and `mf` (NULL: none) the window
+// protocol spoken inside the launch.  *launched = false: this rank has no destination lines and
+// nothing was launched -- the caller then speaks the protocol with flag kernels
 pa_status get_fft(int nb, const BlockCopy* const* blocks, const void* const* srcs, void* dst, int sign,
                   bool f32, const MultiFlags* mf, void* stream, bool* launched);
-// can pa_transpose fuse a FFT of the given precision into this plan's unpack?  The same answer
-// on every rank of the grid line (global geometry only); PA_EINVAL + last_error otherwise.
-// PeerGet plans: the one-sided gather of get_fft too.  No device call.
-pa_status plan_fft_check(Plan* plan, bool f32);
-// fused unpack + complex-to-real line transform (fft.cu, k_unpack_brfft): the blocks tile lines
-// of N/2 + 1 bins of the complex destination box; `dst` is the real array of N reals per line
-// that replaces it (same layout otherwise).  f32: ComplexF32 -> Float32, else ComplexF64 -> Float64
-pa_status unpack_brfft(int nb, const BlockCopy* const* blocks, const void* const* srcs, void* dst,
-                       bool f32, void* stream);
-// plan_fft_check's question for unpack_brfft; its own cache, the same uniformity over the line
-pa_status plan_brfft_check(Plan* plan, bool f32);
-// fused unpack + real line transforms (fft.cu, k_unpack_r2r / k_unpack_rfft): the blocks tile
-// lines of N reals (Float32 with f32, else Float64) of the real destination box.  r2r: `dst` is
-// that box, kind one of PA_REDFT10 / PA_REDFT01 / PA_RODFT10 / PA_RODFT01.  rfft: `dst` is the
-// complex array of N/2 + 1 bins per line that replaces it (same layout otherwise)
-pa_status unpack_r2r(int nb, const BlockCopy* const* blocks, const void* const* srcs, void* dst,
-                     int kind, bool f32, void* stream);
-pa_status unpack_rfft(int nb, const BlockCopy* const* blocks, const void* const* srcs, void* dst,
-                      bool f32, void* stream);
-// plan_fft_check's question for unpack_r2r and unpack_rfft (one verdict for both); its own
-// cache, the same uniformity over the line
-pa_status plan_real_check(Plan* plan, bool f32);
-// What the send-side fused put of a transposition computes from the source lines.  The plan moves
-// dst's elements; src is the counterpart of the plan's source with the other element type
-enum class PutMode {
-  fft,    // the complex FFT (pa_fft_put): a complex plan, src complex
-  rfft,   // N reals -> N/2 + 1 bins (pa_rfft_put): a complex plan, src the real counterpart
-  r2r,    // N reals -> N reals, a DCT / DST (pa_r2r_put): a real plan, src real
-  brfft,  // N/2 + 1 bins -> N reals (pa_brfft_put): a real plan, src the complex counterpart
-};
-
 // send-side fused transform + put (fft.cu, k_fft_put / k_rfft_put / k_r2r_put / k_brfft_put): the
 // transform along the first memory dim of the local `src`, every output element stored into the
 // block that owns it.  blocks[i] / dsts[i]: the self block (self_fused) into the local dst, the put
@@ -348,19 +316,20 @@ enum class PutMode {
 // none): the window protocol spoken inside the launch.  *launched = false: this rank has no source
 // lines and nothing was launched -- the caller then speaks the protocol with flag kernels
 pa_status put_fft(int nb, const BlockCopy* const* blocks, const void* src, void* const* dsts, int sign,
-                  PutMode mode, int r2r_kind, bool f32, const MultiFlags* mf, void* stream,
+                  FusedMode mode, int r2r_kind, bool f32, const MultiFlags* mf, void* stream,
                   bool* launched);
-// can put_fft run the complex FFT (rfft: the r2c transform; real: r2r and brfft, one verdict) on
-// this plan?  PeerPut plans and local transposes only; the same answer on every rank of the grid
-// line; own caches.  No device call.
-pa_status plan_fft_put_check(Plan* plan, bool f32);
-pa_status plan_rfft_put_check(Plan* plan, bool f32);
-pa_status plan_real_put_check(Plan* plan, bool f32);
+// Can the fused kernel of `mode` run on this plan, on the receive side (unpack_fused; the complex
+// FFT of a PeerGet plan: get_fft too) or on the send side (put_fft: PeerPut plans and local
+// transposes only)?  The same answer on every rank of the grid line (global geometry only);
+// PA_EINVAL + last_error otherwise.  Cached per plan, side, transform and precision; r2r shares
+// the answer of rfft (receive side) or brfft (send side).  No device call.
+enum class Side { unpack, put };
+pa_status plan_check(Plan* plan, Side side, FusedMode mode, bool f32);
 // dst = transpose(T(src)), T the transform of `mode` (fft: its direction from flags; r2r: kind
 // r2r_kind), on the caller's stream (local plans) or PeerPut's one-sided schedule; every argument
 // has been checked
 pa_status transpose_put_fft(Plan* plan, Comm* comm, const void* src, void* dst, unsigned flags,
-                            PutMode mode, int r2r_kind, void* stream);
+                            FusedMode mode, int r2r_kind, void* stream);
 // real-line transforms (fft.cu): `nlines` dense, consecutive lines of N reals (src when forward,
 // dst when backward) <-> N/2 + 1 complex bins; N a power of two in 16..2048.  f32: Float32 <->
 // ComplexF32, else Float64 <-> ComplexF64

@@ -684,7 +684,7 @@ static BlockCopy contiguous_block(i64 bytes, const void* src, const void* dst) {
 // loads every local source line, transforms it and stores its outputs into the local dst and the
 // peers' dst (fft_sign: the FFT's direction; r2r_kind: the DCT / DST).
 static pa_status one_sided(Plan* P, Comm* comm, const void* src, void* dst, unsigned flags,
-                           int fft_sign, const PutMode* send, int r2r_kind, cudaStream_t user) {
+                           int fft_sign, const FusedMode* send, int r2r_kind, cudaStream_t user) {
   TransposeState& S = *P->st;
   const int nproc = P->nproc, me = P->self_index;
   const bool get = P->method == PA_PEER_GET;
@@ -862,18 +862,6 @@ static pa_status one_sided(Plan* P, Comm* comm, const void* src, void* dst, unsi
     S.timed_once = true;
   }
   return PA_OK;
-}
-
-// the fused unpack of `mode` (fft_sign: the direction of FusedMode::fft)
-static pa_status unpack_fused(FusedMode mode, int r2r_kind, int nb, const BlockCopy* const* blocks,
-                              const void* const* srcs, void* dst, int fft_sign, bool f32,
-                              void* stream) {
-  switch (mode) {
-    case FusedMode::brfft: return unpack_brfft(nb, blocks, srcs, dst, f32, stream);
-    case FusedMode::r2r: return unpack_r2r(nb, blocks, srcs, dst, r2r_kind, f32, stream);
-    case FusedMode::rfft: return unpack_rfft(nb, blocks, srcs, dst, f32, stream);
-    default: return unpack_fft(nb, blocks, srcs, dst, fft_sign, f32, stream);
-  }
 }
 
 // ---- the staged schedules (PointToPoint / Alltoallv) --------------------------------
@@ -1109,7 +1097,7 @@ static pa_status staged(Plan* P, Comm* comm, const void* src, void* dst, unsigne
       sp.push_back(fused_self ? src : (const void*)rbuf);
     }
     const bool f32 = (flags & PA_FFT_F32) != 0;
-    RC(unpack_fused(mode, r2r_kind, nproc, bl.data(), sp.data(), dst, fft_sign, f32, S.unpack_s));
+    RC(unpack_fused(nproc, bl.data(), sp.data(), dst, fft_sign, mode, r2r_kind, f32, S.unpack_s));
   } else if (stage_self) {
     RC(launch_block(self.unpack, rbuf, dst, S.unpack_s, nullptr));  // local data first (:511)
   }
@@ -1176,12 +1164,7 @@ pa_status transpose(Plan* P, Comm* comm, const void* src, void* dst, unsigned fl
   }
   // a fused FFT this plan cannot run is refused before anything is enqueued -- and on every
   // rank of the line alike (the peers of a refusing rank must not start the exchange)
-  if (mode == FusedMode::brfft)
-    RC(plan_brfft_check(P, fft_f32));
-  else if (mode == FusedMode::r2r || mode == FusedMode::rfft)
-    RC(plan_real_check(P, fft_f32));
-  else if (fft_sign)
-    RC(plan_fft_check(P, fft_f32));
+  if (fft_sign) RC(plan_check(P, Side::unpack, mode, fft_f32));
   RC(ensure_state(P));
   TransposeState& S = *P->st;
   cudaStream_t user = (cudaStream_t)stream;
@@ -1202,7 +1185,7 @@ pa_status transpose(Plan* P, Comm* comm, const void* src, void* dst, unsigned fl
     // one block: the whole local array, src -> fft(permuted dest)
     if (P->length_out == 0) return PA_OK;
     const BlockCopy* b = &P->self_fused;
-    RC(unpack_fused(mode, r2r_kind, 1, &b, &src, dst, fft_sign, fft_f32, user));
+    RC(unpack_fused(1, &b, &src, dst, fft_sign, mode, r2r_kind, fft_f32, user));
     if (timing) {
       CU(cudaEventRecord(S.t[6], user));
       S.timed_once = true;
@@ -1292,7 +1275,7 @@ pa_status transpose(Plan* P, Comm* comm, const void* src, void* dst, unsigned fl
   return staged(P, comm, src, dst, flags, mode, r2r_kind, stage_self, user, buf_ev, buf_unpack_ev);
 }
 
-pa_status transpose_put_fft(Plan* P, Comm* comm, const void* src, void* dst, unsigned flags, PutMode mode,
+pa_status transpose_put_fft(Plan* P, Comm* comm, const void* src, void* dst, unsigned flags, FusedMode mode,
                             int r2r_kind, void* stream) {
   // (pa_fft_put / pa_rfft_put / pa_r2r_put / pa_brfft_put have checked the flags, the arrays and
   //  the plan's verdict, which admits PeerPut plans and local transposes only)
@@ -1300,7 +1283,7 @@ pa_status transpose_put_fft(Plan* P, Comm* comm, const void* src, void* dst, uns
   TransposeState& S = *P->st;
   cudaStream_t user = (cudaStream_t)stream;
   const bool timing = S.timing;
-  const int sign = mode != PutMode::fft || (flags & PA_FFT_FORWARD) ? -1 : 1;
+  const int sign = mode != FusedMode::fft || (flags & PA_FFT_FORWARD) ? -1 : 1;
   const bool f32 = (flags & PA_FFT_F32) != 0;
   if (timing) CU(cudaEventRecord(S.t[0], user));
   if (P->dim < 0 || P->nproc == 1) {

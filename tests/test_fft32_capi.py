@@ -218,8 +218,16 @@ def test_rfft_f32_overlap_is_sized_with_4_and_8_byte_elements():
             assert lib.pa_rfft(pr._h, pc._h, 0, None, flags | F32, buf.at(s), buf.at(d), None) \
                 == _lib.PA_EINVAL, (flags, s, d)
             assert b"overlap" in lib.pa_last_error()
-        # adjacent: past the overlap check (rb and cb are multiples of 16)
-        st = lib.pa_rfft(pr._h, pc._h, 0, None, flags | F32, buf.at(0), buf.at(nsrc), None)
+        # adjacent: past the overlap check (rb and cb are multiples of 16); with a GPU the transform
+        # runs, so on device memory (a kernel cannot address this host memory)
+        if no_gpu():
+            st = lib.pa_rfft(pr._h, pc._h, 0, None, flags | F32, buf.at(0), buf.at(nsrc), None)
+        else:
+            dev = torch.zeros(nsrc + ndst, dtype=torch.uint8, device="cuda")
+            st = lib.pa_rfft(pr._h, pc._h, 0, None, flags | F32, C.c_void_p(dev.data_ptr()),
+                             C.c_void_p(dev.data_ptr() + nsrc), None)
+            torch.cuda.synchronize()
+            assert st == _lib.PA_OK, lib.pa_last_error()
         assert st != _lib.PA_EINVAL or b"overlap" not in lib.pa_last_error()
         if no_gpu():
             assert st == _lib.PA_ENOGPU

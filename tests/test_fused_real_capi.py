@@ -271,7 +271,7 @@ def test_element_size_and_precision_mismatch():
 
 
 def test_unrelated_complex_pencils():
-    topo, px, py, pyc, plan, src_b, _, _ = setup()
+    topo, px, py, pyc, plan, src_b, _, rfft_b = setup()
     buf = HostBuf(1 << 16)
     other = pa.MPITopology(pa.COMM_SELF, (1, 1))
     wrong = [
@@ -286,7 +286,15 @@ def test_unrelated_complex_pencils():
     for cplx in wrong:
         assert rfft(plan, cplx, buf.at(0), buf.at(1 << 15)) == EINCOMPAT
         assert lib.pa_last_error().startswith(b"pa_transpose_rfft")
-    assert rfft(plan, pyc, buf.at(0), buf.at(1 << 15)) in (ENOGPU, OK)
+    # the matching pencil runs: on device arrays when there is a GPU (a kernel cannot address
+    # this host memory)
+    if no_gpu():
+        assert rfft(plan, pyc, buf.at(0), buf.at(1 << 15)) == ENOGPU
+    else:
+        src = torch.zeros(src_b, dtype=torch.uint8, device="cuda")
+        dst = torch.empty(rfft_b, dtype=torch.uint8, device="cuda")
+        assert rfft(plan, pyc, C.c_void_p(src.data_ptr()), C.c_void_p(dst.data_ptr())) == OK
+        torch.cuda.synchronize()
     assert lib.pa_transpose_rfft(plan.h, None, None, buf.at(0), buf.at(1 << 15), 0, None) == EINVAL
     # a plan whose output axis is decomposed (y -> x with the rfft along y): no match either
     back = _Plan(py, px, (), 8, pa.PointToPoint())
