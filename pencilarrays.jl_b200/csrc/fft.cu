@@ -64,6 +64,18 @@ struct Vec2<float> {
 __device__ __forceinline__ double2 vec2(double x, double y) { return make_double2(x, y); }
 __device__ __forceinline__ float2 vec2(float x, float y) { return make_float2(x, y); }
 
+// Entry STRIDE k of a twiddle table of the kernel's precision, read through the read-only cache:
+// W_L^k of the complex FFT's table, W_N^k of a real line's (STRIDE 2: W_N^(2i) = W_L^i, for its
+// L-point passes) or W_4N^k of the DCT / DST table
+template <class T, int STRIDE = 1>
+struct Twiddles {
+  const typename Vec2<T>::type* tab;
+  __device__ __forceinline__ cplx_t<T> operator()(int k) const {
+    const typename Vec2<T>::type w = __ldg(tab + STRIDE * k);
+    return cplx_t<T>{w.x, w.y};
+  }
+};
+
 constexpr int FFT_MAXB = 8;   // blocks gathered by one launch (ranks of a grid line on one box)
 constexpr int FFT_MAXO = PA_MAX_DIMS - 2;
 constexpr int FFT_THREADS = 256;
@@ -142,6 +154,13 @@ __device__ __forceinline__ int fft_pos(int k) {
     constexpr int LOGR = PassRadix<LOGM>::LOGR;
     return ((k & ((1 << LOGR) - 1)) << (LOGM - LOGR)) + fft_pos<LOGL, LOGM - LOGR>(k >> LOGR);
   }
+}
+
+// Real i of a line of N = 2L reals after the L-point passes (viewed as T: z[m] = x[2m] + i x[2m+1]
+// in natural order), part i & 1 of the slot of output m = i / 2 (the c2r and DCT-III read-outs)
+template <int LOGL, class T>
+__device__ __forceinline__ T out_real(const T* line, int i) {
+  return line[2 * pa_fft::pad_index(fft_pos<LOGL, LOGL>(i >> 1)) + (i & 1)];
 }
 
 // The gather of every block's rows of one line into shared memory (thread (c, r) owns column
@@ -288,10 +307,7 @@ __device__ __forceinline__ void fft_cta_lines(const FftParams& p, const long lon
   constexpr int RS = FftCtaShape<LOGL, C, T>::RS;
   constexpr int LOGR1 = FftCtaShape<LOGL, C, T>::LOGR1;
   const V* twp = reinterpret_cast<const V*>(p.tw);
-  auto tw = [twp](int i) {
-    const V w = __ldg(twp + i);
-    return cx{w.x, w.y};
-  };
+  const Twiddles<T> tw{twp};
   {
     // transposing gather: C consecutive threads read C consecutive columns of one source row;
     // linear gather (lines contiguous in the source): consecutive threads read along a line
@@ -447,14 +463,8 @@ __device__ __forceinline__ void rfft_forward_tail(cplx_t<T>* sm, int pitch, int 
   using V = typename Vec2<T>::type;
   constexpr int L = 1 << LOGL;
   constexpr int P = L / 2 + 1;  // pairs (k, L - k) per line
-  auto twN = [twp](int k) {
-    const V w = __ldg(twp + k);
-    return cx{w.x, w.y};
-  };
-  auto twL = [twp](int i) {  // W_L^i = W_N^(2i)
-    const V w = __ldg(twp + 2 * i);
-    return cx{w.x, w.y};
-  };
+  const Twiddles<T> twN{twp};
+  const Twiddles<T, 2> twL{twp};  // W_L^i = W_N^(2i)
   fft_passes<LOGL, LOGL, C>(sm, pitch, ncol, -1, twL);
 
   // ---- post-pass + store: N/2 + 1 bins per line, one contiguous run ----
@@ -472,6 +482,30 @@ __device__ __forceinline__ void rfft_forward_tail(cplx_t<T>* sm, int pitch, int 
       if (k != L - k) __stcs(o + (L - k), vec2(xl.x, xl.y));
     }
   }
+}
+
+// The c2r pre-pass in place (k_rfft backward, k_unpack_brfft, k_brfft_put), the mirror of r2r_pre:
+// a thread owns the slots k and L - k of its pair.  UNROLL: unroll the loop over a thread's pairs
+// (k_unpack_brfft keeps it rolled).  twN = W_N.
+template <int LOGL, int C, bool UNROLL, class T>
+__device__ __forceinline__ void brfft_pre(cplx_t<T>* sm, int pitch, int ncol, int t, const Twiddles<T>& twN) {
+  using cx = cplx_t<T>;
+  constexpr int L = 1 << LOGL;
+  constexpr int P = L / 2 + 1;  // pairs (k, L - k) per line
+  constexpr int TRIPS = (C * P + FFT_THREADS - 1) / FFT_THREADS;
+#pragma unroll(UNROLL ? TRIPS : 1)
+  for (int w0 = 0; w0 < C * P; w0 += FFT_THREADS) {
+    const int w = w0 + t, c = w / P, k = w % P;
+    if (w < C * P && c < ncol) {
+      cx* line = sm + c * pitch;
+      cx zk, zl;
+      pa_fft::brfft_pre_pair(k, line[pa_fft::pad_index(k)], line[pa_fft::pad_index(L - k)], twN(k),
+                             &zk, &zl);
+      line[pa_fft::pad_index(k)] = zk;
+      if (k > 0) line[pa_fft::pad_index(L - k)] = zl;
+    }
+  }
+  __syncthreads();
 }
 
 // The load of k_rfft (k_rfft_put loads its lines with it too), linear: consecutive threads walk
@@ -506,7 +540,6 @@ __global__ void __launch_bounds__(FFT_THREADS) k_rfft(const __grid_constant__ Rf
   using cx = cplx_t<T>;
   using V = typename Vec2<T>::type;
   constexpr int L = 1 << LOGL;
-  constexpr int P = L / 2 + 1;  // pairs (k, L - k) per line
   extern __shared__ __align__(16) unsigned char fft_smem[];
   cx* sm = reinterpret_cast<cx*>(fft_smem);
   const int t = threadIdx.x;
@@ -514,14 +547,6 @@ __global__ void __launch_bounds__(FFT_THREADS) k_rfft(const __grid_constant__ Rf
   const int ncol = (int)((p.nlines - l0) < C ? (p.nlines - l0) : C);
   const int pitch = p.pitch;
   const V* twp = reinterpret_cast<const V*>(p.tw);
-  auto twN = [twp](int k) {
-    const V w = __ldg(twp + k);
-    return cx{w.x, w.y};
-  };
-  auto twL = [twp](int i) {  // W_L^i = W_N^(2i)
-    const V w = __ldg(twp + 2 * i);
-    return cx{w.x, w.y};
-  };
 
   // ---- load (linear gather): consecutive threads walk along a line, one element per load ----
   rfft_load<LOGL, C, FWD, T>(sm, pitch, ncol, t, [&p, l0](int c) {
@@ -533,22 +558,8 @@ __global__ void __launch_bounds__(FFT_THREADS) k_rfft(const __grid_constant__ Rf
     rfft_forward_tail<LOGL, C, T>(sm, pitch, ncol, t, twp,
                                   [&p, l0](int c) { return p.dst + (l0 + c) * p.dst_line; });
   } else {
-    // ---- pre-pass in place: a thread owns the slots k and L - k of its pair ----
-#pragma unroll
-    for (int w0 = 0; w0 < C * P; w0 += FFT_THREADS) {
-      const int w = w0 + t, c = w / P, k = w % P;
-      if (w < C * P && c < ncol) {
-        cx* line = sm + c * pitch;
-        cx zk, zl;
-        pa_fft::brfft_pre_pair(k, line[pa_fft::pad_index(k)], line[pa_fft::pad_index(L - k)], twN(k),
-                               &zk, &zl);
-        line[pa_fft::pad_index(k)] = zk;
-        if (k > 0) line[pa_fft::pad_index(L - k)] = zl;
-      }
-    }
-    __syncthreads();
-
-    fft_passes<LOGL, LOGL, C>(sm, pitch, ncol, 1, twL);
+    brfft_pre<LOGL, C, true, T>(sm, pitch, ncol, t, Twiddles<T>{twp});
+    fft_passes<LOGL, LOGL, C>(sm, pitch, ncol, 1, Twiddles<T, 2>{twp});  // W_L^i = W_N^(2i)
 
     // ---- store: z[n] = x[2n] + i x[2n+1], the N reals of a line as L pair stores ----
 #pragma unroll
@@ -573,7 +584,6 @@ __global__ void __launch_bounds__(FFT_THREADS) k_unpack_brfft(const __grid_const
   using V = typename Vec2<T>::type;
   constexpr int L = 1 << LOGL;
   constexpr int RS = FFT_THREADS / C;
-  constexpr int P = L / 2 + 1;  // pairs (k, L - k) per line
   extern __shared__ __align__(16) unsigned char fft_smem[];
   cx* sm = reinterpret_cast<cx*>(fft_smem);
   const int t = threadIdx.x;
@@ -582,14 +592,6 @@ __global__ void __launch_bounds__(FFT_THREADS) k_unpack_brfft(const __grid_const
   const int ncol = (int)((p.ex - x0) < C ? (p.ex - x0) : C);
   const int pitch = p.pitch;
   const V* twp = reinterpret_cast<const V*>(p.tw);
-  auto twN = [twp](int k) {
-    const V w = __ldg(twp + k);
-    return cx{w.x, w.y};
-  };
-  auto twL = [twp](int i) {  // W_L^i = W_N^(2i)
-    const V w = __ldg(twp + 2 * i);
-    return cx{w.x, w.y};
-  };
 
   // ---- gather: transposing, or linear (lines contiguous in the source) ----
   {
@@ -598,22 +600,8 @@ __global__ void __launch_bounds__(FFT_THREADS) k_unpack_brfft(const __grid_const
   }
   __syncthreads();
 
-  // ---- pre-pass in place (k_rfft<..., false>): a thread owns the slots k and L - k ----
-#pragma unroll 1
-  for (int w0 = 0; w0 < C * P; w0 += FFT_THREADS) {
-    const int w = w0 + t, c = w / P, k = w % P;
-    if (w < C * P && c < ncol) {
-      cx* line = sm + c * pitch;
-      cx zk, zl;
-      pa_fft::brfft_pre_pair(k, line[pa_fft::pad_index(k)], line[pa_fft::pad_index(L - k)], twN(k), &zk,
-                             &zl);
-      line[pa_fft::pad_index(k)] = zk;
-      if (k > 0) line[pa_fft::pad_index(L - k)] = zl;
-    }
-  }
-  __syncthreads();
-
-  fft_passes<LOGL, LOGL, C>(sm, pitch, ncol, 1, twL);
+  brfft_pre<LOGL, C, false, T>(sm, pitch, ncol, t, Twiddles<T>{twp});
+  fft_passes<LOGL, LOGL, C>(sm, pitch, ncol, 1, Twiddles<T, 2>{twp});  // W_L^i = W_N^(2i)
 
   // ---- store: z[n] = x[2n] + i x[2n+1], the N reals of a line as L pair stores ----
   char* d = p.dst + x0 * p.dsx + d_off;
@@ -643,23 +631,13 @@ struct R2rParams {
 };
 
 // The DCT-III pre-pass of the 01 kinds in place (r2r_tail, k_r2r_put): a thread owns the slots k
-// and L - k of its pair.  tw = W_N, tw4 = W_4N.
+// and L - k of its pair.  twN = W_N, w4 = W_4N.
 template <int LOGL, int C, class T>
-__device__ __forceinline__ void r2r_pre(cplx_t<T>* sm, int pitch, int ncol, int t,
-                                        const typename Vec2<T>::type* twp,
-                                        const typename Vec2<T>::type* tw4p) {
+__device__ __forceinline__ void r2r_pre(cplx_t<T>* sm, int pitch, int ncol, int t, const Twiddles<T>& twN,
+                                        const Twiddles<T>& w4) {
   using cx = cplx_t<T>;
-  using V = typename Vec2<T>::type;
   constexpr int L = 1 << LOGL;
   constexpr int P = L / 2 + 1;  // pairs (k, L - k) per line
-  auto twN = [twp](int k) {
-    const V w = __ldg(twp + k);
-    return cx{w.x, w.y};
-  };
-  auto w4 = [tw4p](int k) {  // w_k = W_4N^k
-    const V w = __ldg(tw4p + k);
-    return cx{w.x, w.y};
-  };
 #pragma unroll
   for (int w0 = 0; w0 < C * P; w0 += FFT_THREADS) {
     const int w = w0 + t, c = w / P, k = w % P;
@@ -687,20 +665,11 @@ __device__ __forceinline__ void r2r_tail(cplx_t<T>* sm, int pitch, int ncol, int
   using V = typename Vec2<T>::type;
   constexpr int L = 1 << LOGL, N = 2 * L;
   constexpr int P = L / 2 + 1;  // pairs (k, L - k) per line
-  auto twN = [twp](int k) {
-    const V w = __ldg(twp + k);
-    return cx{w.x, w.y};
-  };
-  auto twL = [twp](int i) {  // W_L^i = W_N^(2i)
-    const V w = __ldg(twp + 2 * i);
-    return cx{w.x, w.y};
-  };
-  auto w4 = [tw4p](int k) {  // w_k = W_4N^k
-    const V w = __ldg(tw4p + k);
-    return cx{w.x, w.y};
-  };
+  const Twiddles<T> twN{twp};
+  const Twiddles<T, 2> twL{twp};  // W_L^i = W_N^(2i)
+  const Twiddles<T> w4{tw4p};  // w_k = W_4N^k
 
-  if constexpr (!FWD) r2r_pre<LOGL, C, T>(sm, pitch, ncol, t, twp, tw4p);
+  if constexpr (!FWD) r2r_pre<LOGL, C, T>(sm, pitch, ncol, t, twN, w4);
 
   fft_passes<LOGL, LOGL, C>(sm, pitch, ncol, FWD ? -1 : 1, twL);
 
@@ -735,8 +704,8 @@ __device__ __forceinline__ void r2r_tail(cplx_t<T>* sm, int pitch, int ncol, int
       if (c < ncol) {
         const T* line = reinterpret_cast<const T*>(sm + c * pitch);
         const int i = N - 1 - m;
-        const T a = line[2 * pa_fft::pad_index(fft_pos<LOGL, LOGL>(m >> 1)) + (m & 1)];
-        const T b = line[2 * pa_fft::pad_index(fft_pos<LOGL, LOGL>(i >> 1)) + (i & 1)];
+        const T a = out_real<LOGL>(line, m);
+        const T b = out_real<LOGL>(line, i);
         __stcs(reinterpret_cast<V*>(out(c)) + m, vec2(a, sine ? -b : b));
       }
     }
@@ -1028,14 +997,8 @@ __global__ void __maxnreg__(128) k_rfft_put(const __grid_constant__ FftPutParams
   });
   __syncthreads();
   const V* twp = reinterpret_cast<const V*>(p.tw);
-  auto twN = [twp](int k) {
-    const V w = __ldg(twp + k);
-    return cx{w.x, w.y};
-  };
-  auto twL = [twp](int i) {  // W_L^i = W_N^(2i)
-    const V w = __ldg(twp + 2 * i);
-    return cx{w.x, w.y};
-  };
+  const Twiddles<T> twN{twp};
+  const Twiddles<T, 2> twL{twp};  // W_L^i = W_N^(2i)
   fft_passes<LOGL, LOGL, C>(sm, pitch, ncol, -1, twL);
   put_ready_wait(pp.mf);
 
@@ -1092,11 +1055,8 @@ __global__ void __maxnreg__(128) k_r2r_put(const __grid_constant__ FftPutParams 
     return reinterpret_cast<const V*>(p.blk[0].src + so_off[0] + (x0 + c) * p.blk[0].ssx);
   });
   __syncthreads();
-  auto twL = [twp](int i) {  // W_L^i = W_N^(2i)
-    const V w = __ldg(twp + 2 * i);
-    return cx{w.x, w.y};
-  };
-  if constexpr (!FWD) r2r_pre<LOGL, C, T>(sm, pitch, ncol, t, twp, tw4p);
+  const Twiddles<T, 2> twL{twp};  // W_L^i = W_N^(2i)
+  if constexpr (!FWD) r2r_pre<LOGL, C, T>(sm, pitch, ncol, t, Twiddles<T>{twp}, Twiddles<T>{tw4p});
   fft_passes<LOGL, LOGL, C>(sm, pitch, ncol, FWD ? -1 : 1, twL);
   put_ready_wait(pp.mf);
 
@@ -1106,14 +1066,8 @@ __global__ void __maxnreg__(128) k_r2r_put(const __grid_constant__ FftPutParams 
   if constexpr (FWD) {
     // ---- post-pass + store: the pair k yields Y[k], Y[N-k], Y[L-k] and Y[L+k] (r2r_tail's);
     //      DST-II stores Y[j] at N-1-j ----
-    auto twN = [twp](int k) {
-      const V w = __ldg(twp + k);
-      return cx{w.x, w.y};
-    };
-    auto w4 = [tw4p](int k) {  // w_k = W_4N^k
-      const V w = __ldg(tw4p + k);
-      return cx{w.x, w.y};
-    };
+    const Twiddles<T> twN{twp};
+    const Twiddles<T> w4{tw4p};  // w_k = W_4N^k
     for (int w0 = 0; w0 < C * P; w0 += FFT_THREADS) {
       const int w = w0 + t;
       const int c = across ? (w & (C - 1)) : (w / P), k = across ? (w / C) : (w % P);
@@ -1141,7 +1095,7 @@ __global__ void __maxnreg__(128) k_r2r_put(const __grid_constant__ FftPutParams 
       if (w < C * N && c < ncol) {
         const T* line = reinterpret_cast<const T*>(sm + c * pitch);
         const int i = (n & 1) ? N - 1 - (n >> 1) : (n >> 1);
-        const T v = line[2 * pa_fft::pad_index(fft_pos<LOGL, LOGL>(i >> 1)) + (i & 1)];
+        const T v = out_real<LOGL>(line, i);
         __stcs(put_at<T>(pp, base, c, n), (sine && (n & 1)) ? -v : v);
       }
     }
@@ -1157,7 +1111,6 @@ __global__ void __maxnreg__(128) k_brfft_put(const __grid_constant__ FftPutParam
   using cx = cplx_t<T>;
   using V = typename Vec2<T>::type;
   constexpr int L = 1 << LOGL, N = 2 * L;
-  constexpr int P = L / 2 + 1;  // pairs (k, L - k) per line
   extern __shared__ __align__(16) unsigned char fft_smem[];
   cx* sm = reinterpret_cast<cx*>(fft_smem);
   const FftParams& p = pp.p;
@@ -1172,28 +1125,9 @@ __global__ void __maxnreg__(128) k_brfft_put(const __grid_constant__ FftPutParam
   });
   __syncthreads();
   const V* twp = reinterpret_cast<const V*>(p.tw);
-  auto twN = [twp](int k) {
-    const V w = __ldg(twp + k);
-    return cx{w.x, w.y};
-  };
-  auto twL = [twp](int i) {  // W_L^i = W_N^(2i)
-    const V w = __ldg(twp + 2 * i);
-    return cx{w.x, w.y};
-  };
-  // ---- pre-pass in place (k_rfft<..., false>): a thread owns the slots k and L - k ----
-#pragma unroll
-  for (int w0 = 0; w0 < C * P; w0 += FFT_THREADS) {
-    const int w = w0 + t, c = w / P, k = w % P;
-    if (w < C * P && c < ncol) {
-      cx* line = sm + c * pitch;
-      cx zk, zl;
-      pa_fft::brfft_pre_pair(k, line[pa_fft::pad_index(k)], line[pa_fft::pad_index(L - k)], twN(k),
-                             &zk, &zl);
-      line[pa_fft::pad_index(k)] = zk;
-      if (k > 0) line[pa_fft::pad_index(L - k)] = zl;
-    }
-  }
-  __syncthreads();
+  const Twiddles<T> twN{twp};
+  const Twiddles<T, 2> twL{twp};  // W_L^i = W_N^(2i)
+  brfft_pre<LOGL, C, true, T>(sm, pitch, ncol, t, twN);
   fft_passes<LOGL, LOGL, C>(sm, pitch, ncol, 1, twL);
   put_ready_wait(pp.mf);
 
@@ -1206,7 +1140,7 @@ __global__ void __maxnreg__(128) k_brfft_put(const __grid_constant__ FftPutParam
     const int c = across ? (w & (C - 1)) : (w >> (LOGL + 1)), n = across ? (w / C) : (w & (N - 1));
     if (w < C * N && c < ncol) {
       const T* line = reinterpret_cast<const T*>(sm + c * pitch);
-      __stcs(put_at<T>(pp, base, c, n), line[2 * pa_fft::pad_index(fft_pos<LOGL, LOGL>(n >> 1)) + (n & 1)]);
+      __stcs(put_at<T>(pp, base, c, n), out_real<LOGL>(line, n));
     }
   }
   put_done(pp.mf);
