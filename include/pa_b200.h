@@ -549,6 +549,52 @@ pa_status pa_put_all_brfft(pa_plan* plan, const pa_pencil* cplx, const void* src
  * plan and precision, apart from every other verdict.  Host-only.                                 */
 pa_status pa_plan_real_put_check(const pa_plan* plan, unsigned flags);
 
+/* ---- distributed reductions (reductions.jl:10-38) -------------------------------------
+ * mapreduce(f, op, u[, v]) over the parent arrays of PencilArrays (extra dims included), combined
+ * across every rank of the communicator: each rank gets the same global result, as a 0-d device
+ * value at `result`.  ONE kernel per rank and call: a streaming pass over the local array and the
+ * combine through the communicator's flag window (DESIGN §3k); ordered after prior work on
+ * `stream`, and the host is not synchronised.  Julia's semantics:
+ *   maps   PA_MAP_IDENTITY, PA_MAP_ABS (complex: hypot(re, im)), PA_MAP_ABS2 (integers wrap),
+ *          PA_MAP_DOT = real(x * conj(y)) of two arrays a, b (the same expression as abs2 when
+ *          a == b: mapreduce(dot, +, u, u) == sum(abs2, u) bit for bit);
+ *   ops    PA_OP_SUM, PA_OP_MAX, PA_OP_MIN (a NaN anywhere gives NaN; max(-0.0, 0.0) == 0.0),
+ *          PA_OP_ANY / PA_OP_ALL or-ed with one PA_PRED_*: the predicate of the mapped value,
+ *          against *pred_value (one value of the mapped type: the element type under
+ *          identity, the real type under abs / abs2 / dot) for the comparisons;
+ *   result pa_reduce_result_type: sum of Int32 gives Int64, abs / abs2 / dot of complex values
+ *          give the real type, any / all give Bool (one byte), otherwise the element type.
+ * Float32 / ComplexF32 sums accumulate in fp64; the result is deterministic (the same bits on
+ * every rank and for every call on the same data and grid).  Refused with PA_EINVAL: an unknown or
+ * invalid (dtype, map, op) -- max / min of complex values under identity, an ordered comparison of
+ * complex values --, `b` given for a one-array map or missing for PA_MAP_DOT, NULL pointers for a
+ * non-empty local array, arrays not aligned to their real component, a NULL `result` or one
+ * not aligned to the whole result type (16 bytes for ComplexF64, 8 for ComplexF32), a missing
+ * pred_value for a comparison, maximum / minimum of a globally empty array;
+ * PA_EINCOMPAT: the topology's rank count is not the communicator's, or comm == NULL with more
+ * than one rank.  Every refusal happens on the host before anything is enqueued; without a device
+ * PA_ENOGPU after those checks.  Reductions on one communicator are serialised in issue order.   */
+typedef enum pa_dtype {
+  PA_FLOAT64 = 0, PA_FLOAT32 = 1, PA_COMPLEXF64 = 2, PA_COMPLEXF32 = 3, PA_INT32 = 4, PA_INT64 = 5,
+  PA_BOOL = 6 /* result type of any / all only */
+} pa_dtype;
+typedef enum pa_reduce_map { PA_MAP_IDENTITY = 0, PA_MAP_ABS = 1, PA_MAP_ABS2 = 2, PA_MAP_DOT = 3 } pa_reduce_map;
+typedef enum pa_reduce_op { PA_OP_SUM = 0, PA_OP_MAX = 1, PA_OP_MIN = 2, PA_OP_ANY = 3, PA_OP_ALL = 4 } pa_reduce_op;
+#define PA_PRED_EQ       (1 << 4)  /* ==(value) */
+#define PA_PRED_NE       (2 << 4)  /* !=(value) */
+#define PA_PRED_LT       (3 << 4)  /* <(value)  */
+#define PA_PRED_LE       (4 << 4)  /* <=(value) */
+#define PA_PRED_GT       (5 << 4)  /* >(value)  */
+#define PA_PRED_GE       (6 << 4)  /* >=(value) */
+#define PA_PRED_ISNAN    (7 << 4)
+#define PA_PRED_ISFINITE (8 << 4)
+pa_status pa_reduce(const pa_pencil* pencil, int n_extra, const int64_t* extra_dims, pa_comm* comm,
+                    int dtype, int map, int op, const void* pred_value, const void* a,
+                    const void* b, void* result, void* stream);
+/* the result's pa_dtype of pa_reduce(dtype, map, op); PA_EINVAL (with the reason) for the
+ * combinations pa_reduce refuses.  Host-only.                                                  */
+pa_status pa_reduce_result_type(int dtype, int map, int op, int* result_dtype);
+
 /* ---- host chains -----------------------------------------------------------
  * A sequence of transpositions applied to HOST arrays (plan i+1 consumes what
  * plan i produces): one submit = upload of `host_src`, every transpose! on the

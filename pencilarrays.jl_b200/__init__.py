@@ -27,6 +27,10 @@ from .transpositions import (Transposition, transpose_, transpose_bang, Waitall,
                              rfft_, brfft_, r2r_)
 
 
+from . import reductions
+from .reductions import mapreduce, sum, maximum, minimum, any, all, abs2, realdot
+
+
 from . import pencilio as PencilIO
 from .pencilio import MPIIODriver, MPIFile, open_, read_, sizeof_global
 

@@ -5,6 +5,7 @@
 #include <vector>
 
 #include "pa_internal.hpp"
+#include "reduce_core.hpp"
 
 using namespace pa;
 
@@ -1362,6 +1363,115 @@ pa_status pa_io_read(const pa_pencil* p, int n_extra, const int64_t* extra_dims,
   GUARD({
     if (!p || !path || offset < 0 || (n_extra > 0 && !extra_dims)) return PA_EINVAL;
     return io_transfer(*p->p, n_extra, extra_dims, elsize, chunks, dev_array, path, offset, false);
+  })
+}
+
+// ---- distributed reductions -----------------------------------------------------------------
+pa_status pa_reduce_result_type(int dtype, int map, int op, int* result_dtype) {
+  const char* why = "";
+  const int r = red::result_dtype(dtype, map, op, &why);
+  if (r < 0) {
+    set_error("pa_reduce: dtype %d, map %d, op %d: %s", dtype, map, op, why);
+    return PA_EINVAL;
+  }
+  if (result_dtype) *result_dtype = r;
+  return PA_OK;
+}
+
+static int elem_bytes(int dtype) {  // element size of a pa_dtype
+  static const int sz[] = {8, 4, 16, 8, 4, 8, 1};
+  return dtype >= 0 && dtype <= PA_BOOL ? sz[dtype] : 0;
+}
+static int component_bytes(int dtype) {  // the alignment an array of dtype needs
+  return dtype == PA_COMPLEXF64 ? 8 : dtype == PA_COMPLEXF32 ? 4 : elem_bytes(dtype);
+}
+
+// Every check in the order of pa_b200.h, on the host before any device call.
+static pa_status reduce_checks(const pa_pencil* pencil, int n_extra, const int64_t* extra_dims,
+                               pa_comm* comm, int dtype, int map, int op, const void* pred_value,
+                               const void* a, const void* b, void* result, i64* n_local) {
+  const char* who = "pa_reduce";
+  if (!pencil) {
+    set_error("%s: null pencil", who);
+    return PA_EINVAL;
+  }
+  int rt = 0;
+  pa_status s = pa_reduce_result_type(dtype, map, op, &rt);
+  if (s != PA_OK) return s;
+  const Pencil& Pn = *pencil->p;
+  if (n_extra < 0 || (n_extra > 0 && !extra_dims) || Pn.N + n_extra > PA_MAX_DIMS) {
+    set_error("%s: %d extra dims on a %d-d pencil (at most %d dims in all)", who, n_extra, Pn.N,
+              PA_MAX_DIMS);
+    return PA_EINVAL;
+  }
+  i64 lo[PA_MAX_DIMS], hi[PA_MAX_DIMS];
+  Pn.range_local(lo, hi);
+  i64 n = 1, nglobal = 1;
+  for (int d = 0; d < Pn.N; ++d) {
+    n *= hi[d] - lo[d];
+    nglobal *= Pn.size_global[d];
+  }
+  for (int i = 0; i < n_extra; ++i) {
+    if (extra_dims[i] < 0) {
+      set_error("%s: negative extra dim", who);
+      return PA_EINVAL;
+    }
+    n *= extra_dims[i];
+    nglobal *= extra_dims[i];
+  }
+  if (map == PA_MAP_DOT ? (n > 0 && !b) : b != nullptr) {
+    set_error(map == PA_MAP_DOT ? "%s: PA_MAP_DOT reduces two arrays: `b` is missing"
+                                : "%s: a second array `b` goes with PA_MAP_DOT only", who);
+    return PA_EINVAL;
+  }
+  const uintptr_t al = (uintptr_t)component_bytes(dtype);
+  if (n > 0 && (!a || (map == PA_MAP_DOT && !b))) {
+    set_error("%s: null array pointer for a non-empty local array", who);
+    return PA_EINVAL;
+  }
+  if (((uintptr_t)a | (uintptr_t)b) % al) {
+    set_error("%s: arrays must be aligned to %d bytes (their real component)", who, (int)al);
+    return PA_EINVAL;
+  }
+  // (the kernels store the result whole: 16-byte stores for ComplexF64, 8-byte for ComplexF32)
+  const uintptr_t ral = (uintptr_t)elem_bytes(rt);
+  if (!result || (uintptr_t)result % ral) {
+    set_error("%s: `result` must be a device pointer aligned to %d bytes", who, (int)ral);
+    return PA_EINVAL;
+  }
+  const int p = op >> 4;
+  if (p >= (PA_PRED_EQ >> 4) && p <= (PA_PRED_GE >> 4) && !pred_value) {
+    set_error("%s: the comparison needs pred_value", who);
+    return PA_EINVAL;
+  }
+  const int base = op & 15;
+  if (nglobal == 0 && (base == PA_OP_MAX || base == PA_OP_MIN)) {
+    set_error("%s: reducing over an empty collection is not allowed (maximum / minimum of an "
+              "empty array)", who);
+    return PA_EINVAL;
+  }
+  const int nranks = Pn.topo->size;
+  if (comm ? comm_size(comm->p) != nranks : nranks > 1) {
+    set_error(comm ? "%s: the topology has %d ranks, the communicator %d"
+                   : "%s: a topology of %d ranks needs a communicator", who, nranks,
+              comm ? comm_size(comm->p) : 0);
+    return PA_EINCOMPAT;
+  }
+  *n_local = n;
+  return PA_OK;
+}
+
+pa_status pa_reduce(const pa_pencil* pencil, int n_extra, const int64_t* extra_dims, pa_comm* comm,
+                    int dtype, int map, int op, const void* pred_value, const void* a,
+                    const void* b, void* result, void* stream) {
+  GUARD({
+    i64 n = 0;
+    pa_status s = reduce_checks(pencil, n_extra, extra_dims, comm, dtype, map, op, pred_value, a, b,
+                                result, &n);
+    if (s != PA_OK) return s;
+    s = need_gpu();
+    if (s != PA_OK) return s;
+    return reduce(comm ? comm->p : nullptr, dtype, map, op, pred_value, n, a, b, result, stream);
   })
 }
 

@@ -244,6 +244,36 @@ void comm_destroy(Comm* c);
 pa_status comm_flags_export(Comm* c, void* handle64, i64* offset);
 pa_status comm_flags_import(Comm* c, int rank, const void* handle64, i64 offset);
 
+// What a reduction (reduce.cu) needs of a communicator.  The flag window carries the combine: the
+// words of kind FK_REDUCE and, behind all the words, two sets (the parity of the call) of one
+// 16-byte slot per source rank.
+constexpr int REDUCE_SLOT_BYTES = 16;
+struct ReduceState;  // workspace + serialising event of the reductions on one communicator
+struct ReduceWindow {
+  int nranks = 1, rank = 0;
+  bool flags = false;   // the flag window is mapped everywhere and not overridden by nccl_fences
+  bool nccl = false;    // an NCCL communicator exists (the fallback when !flags)
+  unsigned long long* local_words = nullptr;      // word from rank r: local_words[r * word_stride]
+  int word_stride = 0;
+  unsigned char* local_slots = nullptr;           // slot [parity][r] at (parity * nranks + r) * 16
+  int* err = nullptr;
+  unsigned long long timeout_ns = 0;
+  ReduceState** state = nullptr;  // owned by the communicator
+};
+pa_status comm_reduce_window(Comm* c, ReduceWindow* w);
+int comm_size(const Comm* c);
+// ncclAllGather of `bytes` per rank (the reductions' fallback without a flag window)
+pa_status comm_allgather(Comm* c, const void* send, void* recv, size_t bytes, void* stream);
+// a communicator's reduction state, made with the communicator (synchronous); its window tables
+// uploaded once the flag window is mapped everywhere
+pa_status reduce_state_create(int nranks, ReduceState** out);
+pa_status reduce_state_set_tables(ReduceState* s, int nranks, unsigned long long* const* remote_words,
+                                  unsigned char* const* peer_slots);
+void reduce_state_destroy(ReduceState* s);
+// the reduction itself (reduce.cu); every argument has been checked.  comm NULL: one rank
+pa_status reduce(Comm* comm, int dtype, int map, int op, const void* pred_value, i64 n,
+                 const void* a, const void* b, void* result, void* stream);
+
 // What a fused line kernel computes: from the lines it gathers on the receive side of a
 // transposition (unpack_fused, get_fft) or from the source lines it loads on the send side
 // (put_fft).  A plan moves the elements of one side; the array on the other side of the transform

@@ -1,0 +1,480 @@
+// Distributed reductions over a PencilArray's parent array (reductions.jl:10-38): the local
+// mapreduce and the combine across ranks in ONE kernel per rank and call.
+//
+// Local pass.  The array is one dense run of n elements.  G CTAs of RT threads (G =
+// ceil(n / (V * RT * RU)) with V = 16 / elsize, at most R_CTAS_PER_SM per SM: it depends only on n
+// and the device's SM count) each own a contiguous chunk of
+// 16-byte units; thread t of a CTA folds units t, t + RT, t + 2 RT, ... in that order, RU units in
+// flight per array (evict-first streaming loads: the data is read once).  The elements before the
+// first 16-byte boundary (head, CTA 0) and after the last whole unit (tail, last CTA) are folded
+// one by one, a whole array whose base is not 16-byte aligned modulo its element (ComplexF64 at an
+// odd 8 bytes) or a second array aligned differently from the first loads every element alone.
+// Each CTA reduces its threads with a warp shuffle tree (offsets 16 .. 1) and a tree over its
+// warps (4, 2, 1), and writes its partial to a workspace; the last CTA to finish (fence + atomic
+// ticket) folds the G partials with the same two trees, thread t taking partials t, t + RT, ...
+// in order, and resets the ticket.
+//
+// Tree depth of a Float64 sum (a bound on the roundings any one element goes through):
+//   run + 5 + 3 + ceil(G / RT) + 5 + 3 + (P - 1),
+// run = the per-thread sequential run, ceil(ceil(nunits / G) / RT) * (16 / elsize) + 2 (head,
+// tail); P - 1 for the fold of the P rank partials.  So |sum - exact| <= depth * eps * sum |f(x)|.
+// Float32 / ComplexF32 sums accumulate in fp64 and are rounded once at the end.  The order of a
+// float sum depends on n, the device, P and the base address modulo 16 (which elements are head
+// and tail): the same array at the same address gives the same bits on every call, the same
+// values at another alignment (an offset view) may differ in the last bits.
+//
+// Cross-rank step (P > 1), by thread 0 of the last CTA, through the communicator's flag window:
+// store the rank partial into slot [parity][me] of every rank's window, signal FK_REDUCE with the
+// call's sequence number seq to every peer, wait for every peer's signal >= seq, fold the P slots
+// [parity][0 .. P-1] of the local window in rank order, finalise, store the result.  Every rank
+// folds the same P values in the same order: every rank gets the same bits.
+//
+// Why two slot sets (parity = seq & 1) suffice.  Rank A stores into rank B's slot [k & 1][A] in
+// call k and next in call k + 2.  A's call k + 2 kernel starts after A's call k + 1 kernel has
+// finished (the reductions on one communicator are serialised by `done`), and that kernel waited
+// for B's signal of seq k + 1.  B sends that signal from its call k + 1 kernel, which started
+// after B's call k kernel finished -- the one that read slot [k & 1][A].  So the store of call
+// k + 2 cannot overtake the read of call k.  Call k + 1 uses the other set, which call k does not
+// touch.
+//
+// Without a flag window (an NCCL communicator across nodes, or nccl_fences) the kernel writes the
+// rank partial, ncclAllGather collects the P partials and a one-CTA kernel folds them in rank order.
+#include <cuda_runtime.h>
+
+#include <cstring>
+#include <map>
+#include <mutex>
+
+#include "flags.cuh"
+#include "pa_internal.hpp"
+#include "reduce_core.hpp"
+
+namespace pa {
+
+using namespace red;
+typedef unsigned long long ull;
+
+constexpr int RT = 256;            // threads per CTA
+constexpr int RU = 4;              // 16-byte units in flight per thread and array
+constexpr int R_CTAS_PER_SM = 4;   // grid cap: 1024 threads per SM, 64 KiB of loads in flight
+
+#define CU(call)                                                                  \
+  do {                                                                            \
+    cudaError_t e_ = (call);                                                      \
+    if (e_ != cudaSuccess) {                                                      \
+      cudaGetLastError();                                                         \
+      set_error("%s failed: %s", #call, cudaGetErrorString(e_));                  \
+      return e_ == cudaErrorMemoryAllocation ? PA_ENOMEM : PA_ECUDA;              \
+    }                                                                             \
+  } while (0)
+
+enum Combine { C_LOCAL = 0, C_FLAGS = 1, C_GATHER = 2 };
+
+struct RArgs {
+  const void* a;
+  const void* b;
+  i64 head, tail, nunits, chunk;  // elements before / after the units; units; units per CTA
+  int G;
+  int vec_a, vec_b;               // 16-byte loads possible on a / on b
+  int pred;
+  alignas(16) unsigned char ref[16];
+  unsigned* ticket;
+  unsigned char* part;            // G partials, 16 bytes each
+  int mode;                       // Combine
+  int nranks, rank;
+  ull seq;
+  ull* local_words;
+  int word_stride;
+  ull* const* remote_words;       // device table [nranks]
+  unsigned char* const* peer_slots;  // device table [nranks]
+  unsigned char* local_slots;
+  ull timeout_ns;
+  int* err;
+  void* result;
+  unsigned char* partial_out;     // C_GATHER: the rank partial
+};
+
+// ---- loads and 16-byte slots -----------------------------------------------------------------
+__device__ __forceinline__ double ld1(const double* p) { return __ldcs(p); }
+__device__ __forceinline__ float ld1(const float* p) { return __ldcs(p); }
+__device__ __forceinline__ int32_t ld1(const int32_t* p) { return __ldcs((const int*)p); }
+__device__ __forceinline__ long long ld1(const long long* p) { return __ldcs(p); }
+__device__ __forceinline__ c64 ld1(const c64* p) { return c64{__ldcs(&p->re), __ldcs(&p->im)}; }
+__device__ __forceinline__ c32 ld1(const c32* p) { return c32{__ldcs(&p->re), __ldcs(&p->im)}; }
+
+template <class E>
+__device__ __forceinline__ void ld_unit(const E* p, bool vec, E (&out)[16 / sizeof(E)]) {
+  constexpr int V = 16 / sizeof(E);
+  if (vec) {
+    const int4 w = __ldcs((const int4*)p);
+    memcpy(out, &w, 16);
+  } else {
+#pragma unroll
+    for (int j = 0; j < V; ++j) out[j] = ld1(p + j);
+  }
+}
+
+template <class A> __device__ __forceinline__ void st16(unsigned char* p, A v) {
+  int4 w = make_int4(0, 0, 0, 0);
+  memcpy(&w, &v, sizeof(A));
+  *(int4*)p = w;
+}
+template <class A> __device__ __forceinline__ A ld16_cg(const unsigned char* p) {  // other SMs' stores
+  const int4 w = __ldcg((const int4*)p);
+  A v;
+  memcpy(&v, &w, sizeof(A));
+  return v;
+}
+template <class A> __device__ __forceinline__ A ld16_cv(const unsigned char* p) {  // other GPUs' stores
+  const int4 w = __ldcv((const int4*)p);
+  A v;
+  memcpy(&v, &w, sizeof(A));
+  return v;
+}
+
+template <class A> __device__ __forceinline__ A shfl_down(A v, int o) { return __shfl_down_sync(~0u, v, o); }
+template <> __device__ __forceinline__ c64 shfl_down<c64>(c64 v, int o) {
+  return c64{__shfl_down_sync(~0u, v.re, o), __shfl_down_sync(~0u, v.im, o)};
+}
+
+// shuffle tree over each warp (16, 8, 4, 2, 1), then over the RT/32 warp results (4, 2, 1);
+// the CTA's value ends in thread 0
+template <class Rd>
+__device__ __forceinline__ typename Rd::A block_reduce(typename Rd::A v, typename Rd::A* sh) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = Rd::comb(v, shfl_down(v, o));
+  const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
+  __syncthreads();  // (sh may still be read from an earlier call)
+  if (l == 0) sh[w] = v;
+  __syncthreads();
+  if (w == 0) {
+    v = l < RT / 32 ? sh[l] : Rd::neutral();
+#pragma unroll
+    for (int o = RT / 64; o > 0; o >>= 1) v = Rd::comb(v, shfl_down(v, o));
+  }
+  return v;
+}
+
+template <class E, int M, int O>
+__global__ void __launch_bounds__(RT, R_CTAS_PER_SM) k_reduce(const RArgs g) {
+  using Rd = Red<E, M, O>;
+  using T = typename Rd::T;
+  using A = typename Rd::A;
+  constexpr int V = 16 / sizeof(E);
+  __shared__ A sh[RT / 32];
+  __shared__ int last;
+  const E* a = (const E*)g.a;
+  const E* b = M == M_DOT ? (const E*)g.b : a;
+  T ref;
+  memcpy(&ref, g.ref, sizeof(T));
+  const int t = threadIdx.x, c = blockIdx.x;
+
+  A acc = Rd::neutral();
+  if (c == 0 && t < g.head) acc = Rd::comb(acc, Rd::elem(ld1(a + t), ld1(b + t), ref, g.pred));
+  const E* ua = a + g.head;
+  const E* ub = b + g.head;
+  const i64 u1 = min(((i64)c + 1) * g.chunk, g.nunits);
+  for (i64 u = (i64)c * g.chunk + t; u < u1; u += (i64)RT * RU) {
+    E xa[RU][V], xb[RU][V];
+#pragma unroll
+    for (int k = 0; k < RU; ++k)
+      if (u + k * RT < u1) {
+        ld_unit(ua + (u + k * RT) * V, g.vec_a, xa[k]);
+        if (M == M_DOT) ld_unit(ub + (u + k * RT) * V, g.vec_b, xb[k]);
+      }
+#pragma unroll
+    for (int k = 0; k < RU; ++k)
+      if (u + k * RT < u1) {
+#pragma unroll
+        for (int j = 0; j < V; ++j)
+          acc = Rd::comb(acc, Rd::elem(xa[k][j], M == M_DOT ? xb[k][j] : xa[k][j], ref, g.pred));
+      }
+  }
+  if (c == g.G - 1 && t < g.tail) {
+    const i64 i = g.head + g.nunits * V + t;
+    acc = Rd::comb(acc, Rd::elem(ld1(a + i), ld1(b + i), ref, g.pred));
+  }
+
+  acc = block_reduce<Rd>(acc, sh);
+  if (g.G > 1) {
+    if (t == 0) {
+      st16(g.part + (size_t)c * 16, acc);
+      __threadfence();
+      last = atomicAdd(g.ticket, 1u) == (unsigned)g.G - 1;
+    }
+    __syncthreads();
+    if (!last) return;
+    __threadfence();
+    acc = Rd::neutral();
+    for (int i = t; i < g.G; i += RT) acc = Rd::comb(acc, ld16_cg<A>(g.part + (size_t)i * 16));
+    acc = block_reduce<Rd>(acc, sh);
+    if (t == 0) *g.ticket = 0;  // the next call (ordered after this one) starts from zero
+  }
+  if (t != 0) return;
+
+  if (g.mode == C_GATHER) {
+    st16(g.partial_out, acc);
+    return;
+  }
+  if (g.mode == C_FLAGS) {
+    const int P = g.nranks, me = g.rank;
+    const size_t set = (size_t)(g.seq & 1) * P;
+    st16(g.local_slots + (set + me) * 16, acc);
+    for (int k = 1; k < P; ++k) {
+      const int q = (me + k) % P;
+      st16(g.peer_slots[q] + (set + me) * 16, acc);
+    }
+    for (int k = 1; k < P; ++k) flag_signal(g.remote_words[(me + k) % P], g.seq);
+    for (int k = 1; k < P; ++k) {
+      const int q = (me + P - k) % P;
+      flag_wait(g.local_words + (size_t)q * g.word_stride, g.seq, g.timeout_ns, g.err);
+    }
+    acc = Rd::neutral();
+    for (int q = 0; q < P; ++q) acc = Rd::comb(acc, ld16_cv<A>(g.local_slots + (set + q) * 16));
+  }
+  *(typename Rd::R*)g.result = Rd::finish(acc);
+}
+
+// the NCCL fallback's second kernel: fold the P gathered partials in rank order
+template <class E, int M, int O>
+__global__ void k_reduce_fold(const unsigned char* slots, int P, void* result) {
+  using Rd = Red<E, M, O>;
+  typename Rd::A acc = Rd::neutral();
+  for (int q = 0; q < P; ++q) acc = Rd::comb(acc, ld16_cg<typename Rd::A>(slots + (size_t)q * 16));
+  *(typename Rd::R*)result = Rd::finish(acc);
+}
+
+// ---- state: workspace, window tables and the event serialising the calls ----------------------
+struct ReduceState {
+  int device = 0, G_max = 1;
+  unsigned* ticket = nullptr;
+  unsigned char* part = nullptr;    // G_max partials
+  unsigned char* gather = nullptr;  // [0]: the rank partial; [1 + r]: gathered partials (fallback)
+  void** tables = nullptr;          // remote_words[nranks], peer_slots[nranks] (flag window)
+  bool tables_ready = false;
+  cudaEvent_t done = nullptr;       // the previous reduction's last kernel
+  ull seq = 0;
+  // held from the wait on `done` to its record: host threads calling at once cannot both order
+  // their kernels after the same previous call and run them together on one workspace
+  std::mutex mu;
+};
+
+void reduce_state_destroy(ReduceState* s) {
+  if (!s) return;
+  if (s->done) {
+    cudaEventSynchronize(s->done);
+    cudaEventDestroy(s->done);
+  }
+  cudaFree(s->ticket);
+  cudaFree(s->part);
+  cudaFree(s->gather);
+  cudaFree(s->tables);
+  cudaGetLastError();
+  delete s;
+}
+
+// A communicator's state is made while the communicator is set up (comm_init*, synchronous
+// like the rest of that setup) and its window tables are uploaded when the flag window is complete
+// (reduce_state_set_tables), so no reduction on it touches the host's timeline.  The one-rank
+// state of a device is made by its first reduction with stream-ordered allocations on the
+// caller's stream, so that call does not synchronise the host either.
+static pa_status make_state(int nranks, cudaStream_t stream, bool ordered, ReduceState** out) {
+  std::unique_ptr<ReduceState> s(new ReduceState);
+  CU(cudaGetDevice(&s->device));
+  int sms = 0;
+  CU(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, s->device));
+  s->G_max = R_CTAS_PER_SM * sms;
+  auto alloc = [&](void** p, size_t bytes) {
+    return ordered ? cudaMallocAsync(p, bytes, stream) : cudaMalloc(p, bytes);
+  };
+  CU(alloc((void**)&s->ticket, sizeof(unsigned)));
+  CU(cudaMemsetAsync(s->ticket, 0, sizeof(unsigned), stream));
+  CU(alloc((void**)&s->part, (size_t)s->G_max * 16));
+  CU(alloc((void**)&s->gather, (size_t)(nranks + 1) * 16));
+  if (nranks > 1) CU(alloc((void**)&s->tables, 2 * sizeof(void*) * (size_t)nranks));
+  CU(cudaEventCreateWithFlags(&s->done, cudaEventDisableTiming));
+  if (!ordered) CU(cudaStreamSynchronize(stream));
+  *out = s.release();
+  return PA_OK;
+}
+
+pa_status reduce_state_create(int nranks, ReduceState** out) {
+  return make_state(nranks, nullptr, false, out);
+}
+
+pa_status reduce_state_set_tables(ReduceState* s, int nranks, unsigned long long* const* remote_words,
+                                  unsigned char* const* peer_slots) {
+  std::vector<void*> tab(2 * (size_t)nranks);
+  for (int r = 0; r < nranks; ++r) {
+    tab[r] = remote_words[r];
+    tab[nranks + r] = peer_slots[r];
+  }
+  CU(cudaMemcpy(s->tables, tab.data(), tab.size() * sizeof(void*), cudaMemcpyHostToDevice));
+  s->tables_ready = true;
+  return PA_OK;
+}
+
+// the state of one-rank reductions without a communicator: one per device
+static std::mutex g_local_mu;
+static std::map<int, ReduceState*> g_local_states;
+
+// ---- dispatch over (element type, map, op) -----------------------------------------------------
+struct Launch {
+  RArgs g;
+  cudaStream_t stream;
+  const unsigned char* gathered;  // C_GATHER: the fold kernel's input (NULL: no fold)
+  int nranks;
+};
+
+template <class E, int M, int O> static pa_status run(const Launch& L) {
+  k_reduce<E, M, O><<<L.g.G, RT, 0, L.stream>>>(L.g);
+  count_launch();
+  CU(cudaGetLastError());
+  return PA_OK;
+}
+template <class E, int M, int O> static pa_status run_fold(const Launch& L) {
+  k_reduce_fold<E, M, O><<<1, 1, 0, L.stream>>>(L.gathered, L.nranks, L.g.result);
+  count_launch();
+  CU(cudaGetLastError());
+  return PA_OK;
+}
+
+template <class E, int M> static pa_status by_op(int op, bool fold, const Launch& L) {
+  switch (op & 15) {
+    case O_SUM: return fold ? run_fold<E, M, O_SUM>(L) : run<E, M, O_SUM>(L);
+    case O_ANY: return fold ? run_fold<E, M, O_ANY>(L) : run<E, M, O_ANY>(L);
+    case O_ALL: return fold ? run_fold<E, M, O_ALL>(L) : run<E, M, O_ALL>(L);
+  }
+  if constexpr (Ordered<typename Mapped<E, M>::T>::value) {
+    if ((op & 15) == O_MAX) return fold ? run_fold<E, M, O_MAX>(L) : run<E, M, O_MAX>(L);
+    if ((op & 15) == O_MIN) return fold ? run_fold<E, M, O_MIN>(L) : run<E, M, O_MIN>(L);
+  }
+  set_error("reduction: op %d not instantiated", op);
+  return PA_EINVAL;
+}
+template <class E> static pa_status by_map(int map, int op, bool fold, const Launch& L) {
+  switch (map) {
+    case M_ID: return by_op<E, M_ID>(op, fold, L);
+    case M_ABS: return by_op<E, M_ABS>(op, fold, L);
+    case M_ABS2: return by_op<E, M_ABS2>(op, fold, L);
+    case M_DOT: return by_op<E, M_DOT>(op, fold, L);
+  }
+  set_error("reduction: map %d not instantiated", map);
+  return PA_EINVAL;
+}
+static pa_status dispatch(int dtype, int map, int op, bool fold, const Launch& L) {
+  switch (dtype) {
+    case D_F64: return by_map<double>(map, op, fold, L);
+    case D_F32: return by_map<float>(map, op, fold, L);
+    case D_C64: return by_map<c64>(map, op, fold, L);
+    case D_C32: return by_map<c32>(map, op, fold, L);
+    case D_I32: return by_map<int32_t>(map, op, fold, L);
+    case D_I64: return by_map<long long>(map, op, fold, L);
+  }
+  set_error("reduction: dtype %d not instantiated", dtype);
+  return PA_EINVAL;
+}
+
+static int dtype_size(int dtype) {
+  switch (dtype) {
+    case D_F64: case D_C32: case D_I64: return 8;
+    case D_F32: case D_I32: return 4;
+    case D_C64: return 16;
+  }
+  return 0;
+}
+
+pa_status reduce(Comm* comm, int dtype, int map, int op, const void* pred_value, i64 n,
+                 const void* a, const void* b, void* result, void* stream) {
+  ReduceWindow w;
+  if (comm) {
+    pa_status s = comm_reduce_window(comm, &w);
+    if (s != PA_OK) return s;
+  }
+  const int P = w.nranks;
+  if (P > 1 && !w.flags && !w.nccl) {
+    set_error("reduction: the communicator has neither a flag window nor NCCL");
+    return PA_ESTATE;
+  }
+  ReduceState* st = nullptr;
+  if (comm) {
+    st = *w.state;  // made with the communicator
+  } else {
+    int dev = 0;
+    CU(cudaGetDevice(&dev));
+    std::lock_guard<std::mutex> lock(g_local_mu);
+    ReduceState*& s0 = g_local_states[dev];
+    if (!s0) {
+      pa_status s = make_state(1, (cudaStream_t)stream, true, &s0);
+      if (s != PA_OK) return s;
+    }
+    st = s0;
+  }
+  std::lock_guard<std::mutex> serial(st->mu);
+  const bool flags = P > 1 && w.flags;
+  if (flags && !st->tables_ready) {
+    set_error("reduction: the flag window's tables were not uploaded (pa_comm_flags_import)");
+    return PA_ESTATE;
+  }
+
+  Launch L;
+  memset(&L, 0, sizeof L);
+  RArgs& g = L.g;
+  const int es = dtype_size(dtype);
+  const int V = 16 / es;
+  // 16-byte units: from the first 16-byte boundary of `a` that is a whole number of elements in
+  const uintptr_t pa_ = (uintptr_t)a, pb = (uintptr_t)b;
+  const i64 head_bytes = (i64)((16 - (pa_ & 15)) & 15);
+  const bool vec = n > 0 && head_bytes % es == 0;
+  g.head = vec ? std::min<i64>(head_bytes / es, n) : 0;
+  g.nunits = (n - g.head) / V;
+  g.tail = n - g.head - g.nunits * V;
+  g.vec_a = vec;
+  g.vec_b = vec && map == M_DOT && ((pb - pa_) & 15) == 0;
+  // the CTA count depends on n and the device only; the split into head, units and tail (and so
+  // the summation order) also on the base address modulo 16
+  const i64 want = (n + (i64)V * RT * RU - 1) / ((i64)V * RT * RU);
+  g.G = (int)std::max<i64>(1, std::min<i64>(want, st->G_max));
+  g.chunk = (g.nunits + g.G - 1) / g.G;
+  g.a = a;
+  g.b = map == M_DOT ? b : a;
+  g.pred = op >> 4;
+  if (pred_value) {
+    int vs = (map == M_ID) ? es : (dtype == D_C64 ? 8 : dtype == D_C32 ? 4 : es);  // the mapped value
+    memcpy(g.ref, pred_value, (size_t)vs);
+  }
+  g.ticket = st->ticket;
+  g.part = st->part;
+  g.result = result;
+  g.nranks = P;
+  g.rank = w.rank;
+  g.mode = P == 1 ? C_LOCAL : flags ? C_FLAGS : C_GATHER;
+  if (flags) {
+    g.seq = ++st->seq;
+    g.local_words = w.local_words;
+    g.word_stride = w.word_stride;
+    g.remote_words = (ull* const*)st->tables;
+    g.peer_slots = (unsigned char* const*)(st->tables + P);
+    g.local_slots = w.local_slots;
+    g.timeout_ns = w.timeout_ns;
+    g.err = w.err;
+  }
+  g.partial_out = st->gather;
+  L.stream = (cudaStream_t)stream;
+  L.gathered = st->gather + 16;
+  L.nranks = P;
+
+  CU(cudaStreamWaitEvent(L.stream, st->done, 0));
+  pa_status s = dispatch(dtype, map, op, false, L);
+  if (s != PA_OK) return s;
+  if (g.mode == C_GATHER) {
+    s = comm_allgather(comm, st->gather, st->gather + 16, 16, stream);
+    if (s != PA_OK) return s;
+    s = dispatch(dtype, map, op, true, L);
+    if (s != PA_OK) return s;
+  }
+  CU(cudaEventRecord(st->done, L.stream));
+  return PA_OK;
+}
+
+}  // namespace pa

@@ -188,6 +188,7 @@ struct NcclApi {
   decltype(&ncclMemFree) MemFree = nullptr;
   decltype(&ncclCommRegister) CommRegister = nullptr;
   decltype(&ncclCommDeregister) CommDeregister = nullptr;
+  decltype(&ncclAllGather) AllGather = nullptr;
   bool ok = false;
 };
 
@@ -216,6 +217,7 @@ static NcclApi& nccl() {
     LOAD(MemFree);
     LOAD(CommRegister);
     LOAD(CommDeregister);
+    LOAD(AllGather);
 #undef LOAD
     api.ok = api.GetUniqueId && api.CommInitRank && api.CommDestroy && api.Send && api.Recv &&
              api.GroupStart && api.GroupEnd && api.GetErrorString;
@@ -235,7 +237,7 @@ static NcclApi& nccl() {
 // ---- communicator -------------------------------------------------------------
 // Flag window: PA_FLAG_WORDS 64-bit words per source rank, written by that rank
 // over NVLink (monotonic max, release.sys) and polled locally (acquire.sys).
-enum FlagKind { FK_READY = 0, FK_DONE = 1, FK_DATA = 2, FK_KINDS = 4 };
+enum FlagKind { FK_READY = 0, FK_DONE = 1, FK_DATA = 2, FK_REDUCE = 3, FK_KINDS = 4 };
 
 struct Comm {
   ncclComm_t comm = nullptr;  // nullptr: NCCL-free communicator (pa_comm_init_local)
@@ -247,7 +249,16 @@ struct Comm {
   int* fence_err = nullptr;              // mapped pinned host word set on time-out
   bool flags_ready = false;
   std::vector<std::string> imported;     // handles of the peers' flag windows (released on destroy)
+  ReduceState* reduce = nullptr;         // the reductions' workspace and event (reduce.cu)
 };
+
+// the window: the words [source rank][kind], then the reductions' slots [parity][source rank]
+static size_t reduce_slots_offset(int nranks) {
+  return (sizeof(ull) * (size_t)nranks * FK_KINDS + 15) / 16 * 16;
+}
+static size_t window_bytes(int nranks) {
+  return reduce_slots_offset(nranks) + 2 * (size_t)nranks * REDUCE_SLOT_BYTES;
+}
 
 static ull* remote_word(Comm* c, int peer_rank, int kind) {
   return c->peer_flags[peer_rank] + (size_t)c->rank * FK_KINDS + kind;
@@ -313,6 +324,11 @@ pa_status comm_init(const void* id128, int nranks, int rank, Comm** out) {
     std::lock_guard<std::mutex> lock(g_live_mu);
     g_live_comms.insert((void*)c->comm);
   }
+  pa_status rs = reduce_state_create(nranks, &c->reduce);
+  if (rs != PA_OK) {
+    comm_destroy(c.release());
+    return rs;
+  }
   *out = c.release();
   return PA_OK;
 }
@@ -326,6 +342,7 @@ pa_status comm_init_local(int nranks, int rank, Comm** out) {
   c->nranks = nranks;
   c->rank = rank;
   CU(cudaGetDevice(&c->device));
+  RC(reduce_state_create(nranks, &c->reduce));
   *out = c.release();
   return PA_OK;
 }
@@ -339,6 +356,7 @@ void comm_destroy(Comm* c) {
     }
     if (nccl().ok) nccl().CommDestroy(c->comm);
   }
+  reduce_state_destroy(c->reduce);
   for (const std::string& h : c->imported) ipc_release_handle(h.data());
   if (c->flags) cudaFree(c->flags);
   if (c->fence_err) cudaFreeHost(c->fence_err);
@@ -350,7 +368,7 @@ pa_status comm_flags_export(Comm* c, void* handle64, i64* offset) {
   if (!c->flags) {
     // (a whole 2 MiB block of its own: small cudaMalloc allocations share a block, and
     //  a block can be opened only once per importing process)
-    const size_t bytes = std::max<size_t>(sizeof(ull) * (size_t)c->nranks * FK_KINDS, IPC_BLOCK);
+    const size_t bytes = std::max<size_t>(window_bytes(c->nranks), IPC_BLOCK);
     CU(cudaMalloc((void**)&c->flags, bytes));
     CU(cudaMemset(c->flags, 0, bytes));
     CU(cudaHostAlloc((void**)&c->fence_err, sizeof(int), cudaHostAllocMapped));
@@ -379,6 +397,45 @@ pa_status comm_flags_import(Comm* c, int rank, const void* handle64, i64 offset)
   for (int r = 0; r < c->nranks; ++r)
     if (r != c->rank && !c->peer_flags[r]) all = false;
   c->flags_ready = all;
+  if (all && c->nranks > 1) {  // the reductions' peer words and slots (reduce.cu)
+    const size_t so = reduce_slots_offset(c->nranks);
+    std::vector<ull*> words(c->nranks, nullptr);
+    std::vector<unsigned char*> slots(c->nranks, nullptr);
+    for (int r = 0; r < c->nranks; ++r)
+      if (r != c->rank) {
+        words[r] = remote_word(c, r, FK_REDUCE);
+        slots[r] = (unsigned char*)c->peer_flags[r] + so;
+      }
+    RC(reduce_state_set_tables(c->reduce, c->nranks, words.data(), slots.data()));
+  }
+  return PA_OK;
+}
+
+int comm_size(const Comm* c) { return c->nranks; }
+
+pa_status comm_reduce_window(Comm* c, ReduceWindow* w) {
+  RC(check_fence_err(c));
+  w->nranks = c->nranks;
+  w->rank = c->rank;
+  w->flags = c->flags_ready && !g_tun.nccl_fences;
+  w->nccl = c->comm != nullptr;
+  w->state = &c->reduce;
+  w->err = c->fence_err;
+  w->timeout_ns = timeout_ns();
+  if (!w->flags) return PA_OK;
+  const size_t so = reduce_slots_offset(c->nranks);
+  w->local_words = c->flags + FK_REDUCE;
+  w->word_stride = FK_KINDS;
+  w->local_slots = (unsigned char*)c->flags + so;
+  return PA_OK;
+}
+
+pa_status comm_allgather(Comm* c, const void* send, void* recv, size_t bytes, void* stream) {
+  if (!c->comm || !nccl().AllGather) {
+    set_error("reduction: the communicator has neither a flag window nor ncclAllGather");
+    return PA_ESTATE;
+  }
+  NC(nccl().AllGather(send, recv, bytes, ncclUint8, c->comm, (cudaStream_t)stream));
   return PA_OK;
 }
 

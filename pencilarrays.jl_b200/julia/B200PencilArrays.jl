@@ -603,4 +603,104 @@ real_first_fusable(dest::PencilArray{R}, pr::Pencil; method = PeerPut()) where {
     ccall((:pa_plan_real_put_check, libpa), Cint, (Ptr{Cvoid}, Cuint), first(real_put_plan(pr, dest, method)),
           R === Float32 ? Cuint(32) : Cuint(0)) == 0
 
+# ---- global reductions (reductions.jl:10-38) ------------------------------------------------------
+# mapreduce / sum / maximum / minimum / any / all of CuArray-backed PencilArrays with the functions
+# pa_reduce recognises run as ONE kernel per rank (local pass + combine through the flag window);
+# the result is read back as a scalar, as the reference's MPI.Allreduce returns one.  Any other
+# function falls back to the reference's generic method (local mapreduce + MPI.Allreduce).
+const PA_DTYPE = IdDict{Type,Cint}(Float64 => 0, Float32 => 1, ComplexF64 => 2, ComplexF32 => 3,
+                                   Int32 => 4, Int64 => 5)
+const PA_RESULT = Dict{Cint,Type}(0 => Float64, 1 => Float32, 2 => ComplexF64, 3 => ComplexF32,
+                                  4 => Int32, 5 => Int64, 6 => Bool)
+realdot(x, y) = real(x * conj(y))
+pa_map(::typeof(identity)) = Cint(0)
+pa_map(::typeof(abs)) = Cint(1)
+pa_map(::typeof(abs2)) = Cint(2)
+pa_map(::typeof(realdot)) = Cint(3)
+pa_map(::Any) = nothing
+pa_op(::typeof(+)) = Cint(0)
+pa_op(::typeof(Base.add_sum)) = Cint(0)
+pa_op(::typeof(max)) = Cint(1)
+pa_op(::typeof(min)) = Cint(2)
+pa_op(::Any) = nothing
+# predicates: Base.Fix2 of a comparison (==(2), >(0), ...) or isnan / isfinite
+pa_pred(f::Base.Fix2{typeof(==)}) = (Cint(1) << 4, f.x)
+pa_pred(f::Base.Fix2{typeof(!=)}) = (Cint(2) << 4, f.x)
+pa_pred(f::Base.Fix2{typeof(<)}) = (Cint(3) << 4, f.x)
+pa_pred(f::Base.Fix2{typeof(<=)}) = (Cint(4) << 4, f.x)
+pa_pred(f::Base.Fix2{typeof(>)}) = (Cint(5) << 4, f.x)
+pa_pred(f::Base.Fix2{typeof(>=)}) = (Cint(6) << 4, f.x)
+pa_pred(::typeof(isnan)) = (Cint(7) << 4, nothing)
+pa_pred(::typeof(isfinite)) = (Cint(8) << 4, nothing)
+pa_pred(::Any) = nothing
+
+const CuPencilArray{T,N} = PencilArray{T,N,<:CuArray}
+
+function pa_reduce(u::CuPencilArray{T}, v, map::Cint, op::Cint, value) where {T}
+    v === nothing || PencilArrays._check_compatible_arrays(u, v)
+    H = handles(topology(pencil(u)))
+    dt = PA_DTYPE[T]
+    rt = Ref{Cint}()
+    check(ccall((:pa_reduce_result_type, libpa), Cint, (Cint, Cint, Cint, Ptr{Cint}), dt, map, op, rt))
+    R = PA_RESULT[rt[]]
+    result = CuArray{R}(undef, 1)
+    VT = map == 0 ? T : real(T)
+    ref = value === nothing ? C_NULL : Ref{VT}(convert(VT, value))
+    ex = Int64[extra_dims(u)...]
+    ptr_or_null(A) = isempty(A) ? C_NULL : devptr(A)
+    GC.@preserve ref check(ccall((:pa_reduce, libpa), Cint,
+        (Ptr{Cvoid}, Cint, Ptr{Int64}, Ptr{Cvoid}, Cint, Cint, Cint, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid},
+         Ptr{Cvoid}, Ptr{Cvoid}),
+        pencil_handle(H, pencil(u)), length(ex), ex, H.comm, dt, map, op,
+        ref === C_NULL ? C_NULL : Base.unsafe_convert(Ptr{Cvoid}, ref), ptr_or_null(parent(u)),
+        v === nothing ? C_NULL : ptr_or_null(parent(v)), devptr(result), stream_ptr()))
+    CUDA.@allowscalar result[1]
+end
+
+const PA_ELTYPES = Union{Float64,Float32,ComplexF64,ComplexF32,Int32,Int64}
+
+function Base.mapreduce(f::F, op::OP, u::CuPencilArray{T}, etc::Vararg{CuPencilArray{T}};
+                        kws...) where {F,OP,T<:PA_ELTYPES}
+    m, o = pa_map(f), pa_op(op)
+    nargs = 1 + length(etc)
+    if isempty(kws) && m !== nothing && o !== nothing && (nargs == 2) == (m == 3) && nargs <= 2
+        return pa_reduce(u, nargs == 2 ? etc[1] : nothing, m, o, nothing)
+    end
+    # the reference's generic method (reductions.jl:10-18)
+    foreach(v -> PencilArrays._check_compatible_arrays(u, v), etc)
+    rlocal = mapreduce(f, op, map(parent, (u, etc...))...; kws...)
+    MPI.Allreduce(rlocal, MPI.Op(op, typeof(rlocal); iscommutative = true), get_comm(u))
+end
+
+Base.sum(f::F, u::CuPencilArray{<:PA_ELTYPES}) where {F} = mapreduce(f, Base.add_sum, u)
+Base.sum(u::CuPencilArray{<:PA_ELTYPES}) = mapreduce(identity, Base.add_sum, u)
+Base.maximum(f::F, u::CuPencilArray{<:PA_ELTYPES}) where {F} = mapreduce(f, max, u)
+Base.maximum(u::CuPencilArray{<:PA_ELTYPES}) = mapreduce(identity, max, u)
+Base.minimum(f::F, u::CuPencilArray{<:PA_ELTYPES}) where {F} = mapreduce(f, min, u)
+Base.minimum(u::CuPencilArray{<:PA_ELTYPES}) = mapreduce(identity, min, u)
+
+# The kernel compares in the element type; Julia compares in the promoted type.  The two agree
+# only when the value converts exactly (0.1 against Float32 data does not: 0.1f0 > 0.1).
+function exact_in(::Type{T}, x) where {T}
+    x isa Number || return false
+    y = try
+        convert(T, x)
+    catch
+        return false
+    end
+    return y == x || (isnan(y) && isnan(x))
+end
+
+for (fn, code) in ((:any, 3), (:all, 4))
+    @eval function Base.$fn(f::F, u::CuPencilArray{T}) where {F<:Function,T<:PA_ELTYPES}
+        p = pa_pred(f)
+        if p === nothing || !(p[2] === nothing || exact_in(T, p[2]))
+            # the reference's generic method (reductions.jl:30-38)
+            xlocal = $fn(f, parent(u))::Bool
+            return MPI.Allreduce(xlocal, $(fn === :any ? :| : :&), get_comm(u))
+        end
+        pa_reduce(u, nothing, Cint(0), Cint($code) | p[1], p[2])::Bool
+    end
+end
+
 end # module
