@@ -516,64 +516,6 @@ static pa_status fused_pointers(const char* who, const void* src, i64 src_bytes,
   return PA_OK;
 }
 
-// The one-sided fused gather + FFT without the window protocol.  Every check runs on the host
-// before any device call.
-static pa_status get_all_fft(pa_plan* plan, const void* src, void* const* peers, void* dst,
-                             unsigned flags, void* stream) {
-  const char* who = "pa_get_all_fft";
-  if (!plan) {
-    set_error("%s: null plan", who);
-    return PA_EINVAL;
-  }
-  Plan& P = *plan->p;
-  if (P.dim < 0) {
-    set_error("%s: plan has no exchange", who);
-    return PA_EINVAL;
-  }
-  const unsigned dir = flags & ~PA_FFT_F32;
-  if (dir != PA_FFT_FORWARD && dir != PA_FFT_BACKWARD) {
-    set_error("%s: flags must be exactly PA_FFT_FORWARD or PA_FFT_BACKWARD, optionally with "
-              "PA_FFT_F32", who);
-    return PA_EINVAL;
-  }
-  const bool f32 = (flags & PA_FFT_F32) != 0;
-  // the verdict pa_transpose asks (for a PeerGet plan it covers this gather)
-  pa_status s = plan_check(&P, Side::unpack, FusedMode::fft, f32);
-  if (s != PA_OK) return s;
-  const i64 es = P.elsize;
-  const i64 src_bytes = P.length_in * es, dst_bytes = P.length_out * es;
-  std::vector<const BlockCopy*> blocks;
-  std::vector<const void*> srcs;
-  for (int n = 0; n < P.nproc; ++n) {
-    const bool self = n == P.self_index;
-    const BlockCopy& b = self ? P.self_fused : P.peers[n].get;
-    const void* p = self ? src : (peers ? peers[n] : nullptr);
-    if (b.count > 0 && !p) {
-      set_error(self ? "%s: null src for a non-empty self block"
-                     : "%s: null peer array for a non-empty block (peer %d)", who, n + 1);
-      return PA_EINVAL;
-    }
-    if (b.count > 0 && ((uintptr_t)p % es)) {
-      set_error("%s: arrays must be aligned to the %lld-byte element", who, (long long)es);
-      return PA_EINVAL;
-    }
-    blocks.push_back(&b);
-    srcs.push_back(p);
-  }
-  s = fused_pointers(who, src, src_bytes, dst, dst_bytes);
-  if (s != PA_OK) return s;
-  s = need_gpu();
-  if (s != PA_OK) return s;
-  bool launched = false;
-  return get_fft(P.nproc, blocks.data(), srcs.data(), dst, dir == PA_FFT_FORWARD ? -1 : 1, f32, nullptr,
-                 stream, &launched);
-}
-
-pa_status pa_get_all_fft(pa_plan* plan, const void* src, void* const* peers, void* dst, unsigned flags,
-                         void* stream) {
-  GUARD({ return get_all_fft(plan, src, peers, dst, flags, stream); })
-}
-
 pa_status pa_copy_self(pa_plan* plan, const void* src, void* dst, void* stream) {
   if (!plan) return PA_EINVAL;
   pa_status s = need_gpu();
@@ -701,19 +643,6 @@ pa_status pa_plan_set_recv_window(pa_plan* plan, int n, void* peer_recv_buf) {
   GUARD({
     if (!plan) return PA_EINVAL;
     return plan_set_recv_window(plan->p, n - 1, peer_recv_buf);
-  })
-}
-
-// ---- transpose! ------------------------------------------------------------------
-pa_status pa_transpose(pa_plan* plan, pa_comm* comm, const void* src, void* dst, unsigned flags,
-                       void* stream) {
-  GUARD({
-    if (!plan) {
-      set_error("pa_transpose: null plan");
-      return PA_EINVAL;
-    }
-    // src / dst may be NULL on a rank whose local array is empty (checked against the plan)
-    return transpose(plan->p, comm ? comm->p : nullptr, src, dst, flags, stream);
   })
 }
 
@@ -943,140 +872,217 @@ pa_status pa_r2r(const pa_pencil* pencil, int n_extra, const int64_t* extra_dims
   GUARD({ return r2r(pencil, n_extra, extra_dims, kind, flags, src, dst, stream); })
 }
 
-// ---- fused transpose + line transform (pa_transpose_brfft, _r2r, _rfft) ------------------
-// flags any of PA_WAITALL, PA_NO_OVERLAP, PA_STAGE_SELF, PA_FFT_F32 (the direction is implied)
-static pa_status fused_flags(const char* who, unsigned flags) {
-  if (flags & ~(PA_WAITALL | PA_NO_OVERLAP | PA_STAGE_SELF | PA_FFT_F32)) {
-    set_error("%s: flags may combine PA_WAITALL, PA_NO_OVERLAP, PA_STAGE_SELF and PA_FFT_F32 only "
-              "(the direction is implied)", who);
+// ---- fused transpose + line transform -----------------------------------------------------
+// Every entry point of a fused line transform is one (side, mode); `all`: the launch without the
+// window protocol (pa_get_all_fft, pa_put_all_*).
+static const char* line_op_name(Side side, FusedMode mode, bool all) {
+  switch (mode) {
+    case FusedMode::fft:
+      if (side == Side::unpack) return all ? "pa_get_all_fft" : "pa_transpose";
+      return all ? "pa_put_all_fft" : "pa_fft_put";
+    case FusedMode::rfft:
+      if (side == Side::unpack) return "pa_transpose_rfft";
+      return all ? "pa_put_all_rfft" : "pa_rfft_put";
+    case FusedMode::r2r:
+      if (side == Side::unpack) return "pa_transpose_r2r";
+      return all ? "pa_put_all_r2r" : "pa_r2r_put";
+    case FusedMode::brfft: break;
+  }
+  if (side == Side::unpack) return "pa_transpose_brfft";
+  return all ? "pa_put_all_brfft" : "pa_brfft_put";
+}
+
+// The LineOp an entry point's flags (and r2r's kind) ask for, or its refusal.  The flags besides
+// PA_FFT_F32:
+// - pa_transpose: PA_FFT_FORWARD or PA_FFT_BACKWARD (both: forward), PA_FFT_F32 only with one;
+// - pa_transpose_brfft / _r2r / _rfft: the direction is implied; any of PA_WAITALL,
+//   PA_NO_OVERLAP and PA_STAGE_SELF;
+// - pa_get_all_fft and the send side: never PA_STAGE_SELF; fft exactly one direction, the other
+//   modes none; PA_WAITALL except for the launches without the window protocol.
+static pa_status line_op(Side side, FusedMode mode, bool all, unsigned flags, int kind, LineOp* op) {
+  const char* who = line_op_name(side, mode, all);
+  const bool fft = mode == FusedMode::fft;
+  if (side == Side::put && (flags & PA_STAGE_SELF)) {
+    set_error("%s: PA_STAGE_SELF does not apply: the send-side fusion stores the self block "
+              "straight into dst", who);
     return PA_EINVAL;
+  }
+  if (side == Side::put || all) {
+    const unsigned dir = flags & ~(all ? PA_FFT_F32 : PA_FFT_F32 | PA_WAITALL);
+    if (fft ? (dir != PA_FFT_FORWARD && dir != PA_FFT_BACKWARD) : dir != 0) {
+      if (fft)
+        set_error("%s: flags must be exactly PA_FFT_FORWARD or PA_FFT_BACKWARD, optionally with %s", who,
+                  all ? "PA_FFT_F32" : "PA_FFT_F32 and PA_WAITALL");
+      else
+        set_error("%s: flags may combine %s only (the direction is implied)", who,
+                  all ? "PA_FFT_F32" : "PA_WAITALL and PA_FFT_F32");
+      return PA_EINVAL;
+    }
+  } else if (!fft) {
+    if (flags & ~(PA_WAITALL | PA_NO_OVERLAP | PA_STAGE_SELF | PA_FFT_F32)) {
+      set_error("%s: flags may combine PA_WAITALL, PA_NO_OVERLAP, PA_STAGE_SELF and PA_FFT_F32 only "
+                "(the direction is implied)", who);
+      return PA_EINVAL;
+    }
+  } else if ((flags & PA_FFT_F32) && !(flags & (PA_FFT_FORWARD | PA_FFT_BACKWARD))) {
+    set_error("pa_transpose: PA_FFT_F32 without PA_FFT_FORWARD / PA_FFT_BACKWARD");
+    return PA_EINVAL;
+  }
+  const bool r2r = mode == FusedMode::r2r;
+  if (r2r) RC(r2r_kind_check(who, kind));
+  *op = LineOp{side, mode, !fft ? 0 : (flags & PA_FFT_FORWARD) ? -1 : 1, r2r ? kind : 0,
+               (flags & PA_FFT_F32) != 0};
+  return PA_OK;
+}
+
+// The plan's elements: reals (Float64; Float32 with PA_FFT_F32) or complex ones
+static pa_status plan_elsize(const char* who, const Plan& P, bool real, bool f32) {
+  if (P.elsize == (real ? 4 : 8) * (f32 ? 1 : 2)) return PA_OK;
+  const char* t32 = real ? "Float32" : "ComplexF32";
+  if (f32)
+    set_error("%s: PA_FFT_F32 takes a %s (elsize %d) plan", who, t32, real ? 4 : 8);
+  else
+    set_error("%s: a %s (elsize %d) plan, or PA_FFT_F32 for %s", who, real ? "Float64" : "ComplexF64",
+              real ? 8 : 16, t32);
+  return PA_EINVAL;
+}
+
+// The per-rank table of a launch over every block of the grid line without the window protocol:
+// this rank's self block with `local` (get: src, put: dst), peer n's get / put block with peers[n],
+// its array as mapped here.  A non-empty block needs an array aligned to the plan's element.
+static pa_status peer_table(const char* who, const Plan& P, bool get, const void* local,
+                            void* const* peers, std::vector<const BlockCopy*>* blocks,
+                            std::vector<void*>* arrays) {
+  for (int n = 0; n < P.nproc; ++n) {
+    const bool self = n == P.self_index;
+    const BlockCopy& b = self ? P.self_fused : get ? P.peers[n].get : P.peers[n].put;
+    void* p = self ? (void*)local : (peers ? peers[n] : nullptr);
+    if (b.count > 0 && !p) {
+      if (self)
+        set_error("%s: null %s for a non-empty self block", who, get ? "src" : "dst");
+      else
+        set_error("%s: null peer array for a non-empty block (peer %d)", who, n + 1);
+      return PA_EINVAL;
+    }
+    if (b.count > 0 && ((uintptr_t)p % P.elsize)) {
+      set_error("%s: arrays must be aligned to the %lld-byte element", who, (long long)P.elsize);
+      return PA_EINVAL;
+    }
+    blocks->push_back(&b);
+    arrays->push_back(p);
   }
   return PA_OK;
 }
 
-static pa_status transpose_brfft(pa_plan* plan, pa_comm* comm, const pa_pencil* real,
-                                 const void* src, void* dst, unsigned flags, void* stream) {
+// pa_transpose and the receive-side fused transforms (pa_transpose_brfft, _r2r, _rfft).  Every
+// check runs on the host before any device call.  `pen`: brfft the real pencil of dst, rfft the
+// complex one, against the plan's output pencil as pa_rfft relates them; r2r: `kind`.
+static pa_status transpose_unpack(pa_plan* plan, pa_comm* comm, const pa_pencil* pen, int kind,
+                                  const void* src, void* dst, unsigned flags, void* stream,
+                                  FusedMode mode) {
+  const char* who = line_op_name(Side::unpack, mode, false);
   if (!plan) {
-    set_error("pa_transpose_brfft: null plan");
+    set_error("%s: null plan", who);
     return PA_EINVAL;
   }
-  pa_status s = fused_flags("pa_transpose_brfft", flags);
-  if (s != PA_OK) return s;
   Plan& P = *plan->p;
-  const bool f32 = (flags & PA_FFT_F32) != 0;
-  if (P.elsize != (f32 ? 8 : 16)) {
-    set_error(f32 ? "pa_transpose_brfft: PA_FFT_F32 takes a ComplexF32 (elsize 8) plan"
-                  : "pa_transpose_brfft: a ComplexF64 (elsize 16) plan, or PA_FFT_F32 for ComplexF32");
-    return PA_EINVAL;
+  Comm* c = comm ? comm->p : nullptr;
+  LineOp op;
+  if (mode == FusedMode::fft) {
+    // a rank may own nothing (more processes than points, Pencils.jl:193-218): its empty arrays
+    // have no storage, yet it takes part in the exchange
+    if ((!src && P.length_in > 0) || (!dst && P.length_out > 0)) {
+      set_error("pa_transpose: null array pointer");
+      return PA_EINVAL;
+    }
+    bool fused = false;
+    RC(transpose_fft_op(&P, flags, src, dst, &op, &fused));
+    return transpose(&P, c, src, dst, flags, stream, fused ? &op : nullptr);
   }
-  // `real` against the plan's output pencil, as pa_rfft relates them; the pointers below
-  const pa_pencil out{P.pout};
-  int N = 0;
-  i64 nlines = 0;
-  s = rfft_checks("pa_transpose_brfft", real, &out, P.n_extra, P.extra,
-                  PA_FFT_BACKWARD | (flags & PA_FFT_F32), nullptr, nullptr, false, &N, &nlines);
-  if (s != PA_OK) return s;
-  const i64 src_bytes = P.length_in * P.elsize, dst_bytes = nlines * N * (f32 ? 4 : 8);
-  s = fused_pointers("pa_transpose_brfft", src, src_bytes, dst, dst_bytes);
-  if (s != PA_OK) return s;
+  RC(line_op(Side::unpack, mode, false, flags, kind, &op));
+  RC(plan_elsize(who, P, unpack_moves_reals(mode), op.f32));
+  const i64 es = P.elsize;
+  i64 dst_bytes = P.length_out * es;
+  if (mode == FusedMode::r2r) {
+    int ax = 0;  // the transform axis, the output pencil's first memory dim, must be whole (as pa_r2r)
+    RC(line_axis(who, *P.pout, &ax));
+  } else {
+    // dst on `pen`, the other side of the transform from the plan's output pencil
+    const bool rfft = mode == FusedMode::rfft;
+    const pa_pencil out{P.pout};
+    int N = 0;
+    i64 nlines = 0;
+    RC(rfft_checks(who, rfft ? &out : pen, rfft ? pen : &out, P.n_extra, P.extra,
+                   (rfft ? PA_FFT_FORWARD : PA_FFT_BACKWARD) | (op.f32 ? PA_FFT_F32 : 0u), nullptr,
+                   nullptr, false, &N, &nlines));
+    const i64 rs = op.f32 ? 4 : 8;  // bytes of a real
+    dst_bytes = rfft ? nlines * (N / 2 + 1) * 2 * rs : nlines * N * rs;
+  }
+  RC(fused_pointers(who, src, P.length_in * es, dst, dst_bytes));
   // the same verdict on every rank of the grid line: a refusal launches nothing anywhere
-  s = plan_check(&P, Side::unpack, FusedMode::brfft, f32);
-  if (s != PA_OK) return s;
-  s = need_gpu();
-  if (s != PA_OK) return s;
-  return transpose(&P, comm ? comm->p : nullptr, src, dst, flags, stream, FusedMode::brfft);
+  RC(plan_check(&P, Side::unpack, mode, op.f32));
+  RC(need_gpu());
+  return transpose(&P, c, src, dst, flags, stream, &op);
+}
+
+pa_status pa_transpose(pa_plan* plan, pa_comm* comm, const void* src, void* dst, unsigned flags,
+                       void* stream) {
+  GUARD({ return transpose_unpack(plan, comm, nullptr, 0, src, dst, flags, stream, FusedMode::fft); })
 }
 
 pa_status pa_transpose_brfft(pa_plan* plan, pa_comm* comm, const pa_pencil* real, const void* src,
                              void* dst, unsigned flags, void* stream) {
-  GUARD({ return transpose_brfft(plan, comm, real, src, dst, flags, stream); })
+  GUARD({ return transpose_unpack(plan, comm, real, 0, src, dst, flags, stream, FusedMode::brfft); })
+}
+
+pa_status pa_transpose_r2r(pa_plan* plan, pa_comm* comm, int kind, const void* src, void* dst,
+                           unsigned flags, void* stream) {
+  GUARD({ return transpose_unpack(plan, comm, nullptr, kind, src, dst, flags, stream, FusedMode::r2r); })
+}
+
+pa_status pa_transpose_rfft(pa_plan* plan, pa_comm* comm, const pa_pencil* cplx, const void* src,
+                            void* dst, unsigned flags, void* stream) {
+  GUARD({ return transpose_unpack(plan, comm, cplx, 0, src, dst, flags, stream, FusedMode::rfft); })
 }
 
 pa_status pa_plan_brfft_check(const pa_plan* plan, unsigned flags) {
   return plan_verdict("pa_plan_brfft_check", plan, Side::unpack, FusedMode::brfft, (flags & PA_FFT_F32) != 0);
 }
 
-// A real plan (Float64, elsize 8; Float32, elsize 4 with PA_FFT_F32) for pa_transpose_r2r /
-// pa_transpose_rfft
-static pa_status real_plan(const char* who, const Plan& P, bool f32) {
-  if (P.elsize != (f32 ? 4 : 8)) {
-    set_error(f32 ? "%s: PA_FFT_F32 takes a Float32 (elsize 4) plan"
-                  : "%s: a Float64 (elsize 8) plan, or PA_FFT_F32 for Float32", who);
-    return PA_EINVAL;
-  }
-  return PA_OK;
-}
-
-static pa_status transpose_r2r(pa_plan* plan, pa_comm* comm, int kind, const void* src, void* dst,
-                               unsigned flags, void* stream) {
-  const char* who = "pa_transpose_r2r";
-  if (!plan) {
-    set_error("%s: null plan", who);
-    return PA_EINVAL;
-  }
-  pa_status s = fused_flags(who, flags);
-  if (s != PA_OK) return s;
-  s = r2r_kind_check(who, kind);
-  if (s != PA_OK) return s;
-  Plan& P = *plan->p;
-  const bool f32 = (flags & PA_FFT_F32) != 0;
-  s = real_plan(who, P, f32);
-  if (s != PA_OK) return s;
-  int ax = 0;  // the transform axis, the output pencil's first memory dim, must be whole (as pa_r2r)
-  s = line_axis(who, *P.pout, &ax);
-  if (s != PA_OK) return s;
-  s = fused_pointers(who, src, P.length_in * P.elsize, dst, P.length_out * P.elsize);
-  if (s != PA_OK) return s;
-  // the same verdict on every rank of the grid line: a refusal launches nothing anywhere
-  s = plan_check(&P, Side::unpack, FusedMode::r2r, f32);
-  if (s != PA_OK) return s;
-  s = need_gpu();
-  if (s != PA_OK) return s;
-  return transpose(&P, comm ? comm->p : nullptr, src, dst, flags, stream, FusedMode::r2r, kind);
-}
-
-pa_status pa_transpose_r2r(pa_plan* plan, pa_comm* comm, int kind, const void* src, void* dst,
-                           unsigned flags, void* stream) {
-  GUARD({ return transpose_r2r(plan, comm, kind, src, dst, flags, stream); })
-}
-
-static pa_status transpose_rfft(pa_plan* plan, pa_comm* comm, const pa_pencil* cplx, const void* src,
-                                void* dst, unsigned flags, void* stream) {
-  const char* who = "pa_transpose_rfft";
-  if (!plan) {
-    set_error("%s: null plan", who);
-    return PA_EINVAL;
-  }
-  pa_status s = fused_flags(who, flags);
-  if (s != PA_OK) return s;
-  Plan& P = *plan->p;
-  const bool f32 = (flags & PA_FFT_F32) != 0;
-  s = real_plan(who, P, f32);
-  if (s != PA_OK) return s;
-  // `cplx` against the plan's output pencil, as pa_rfft relates them; the pointers below
-  const pa_pencil out{P.pout};
-  int N = 0;
-  i64 nlines = 0;
-  s = rfft_checks(who, &out, cplx, P.n_extra, P.extra, PA_FFT_FORWARD | (flags & PA_FFT_F32), nullptr,
-                  nullptr, false, &N, &nlines);
-  if (s != PA_OK) return s;
-  const i64 dst_bytes = nlines * (N / 2 + 1) * 2 * P.elsize;
-  s = fused_pointers(who, src, P.length_in * P.elsize, dst, dst_bytes);
-  if (s != PA_OK) return s;
-  s = plan_check(&P, Side::unpack, FusedMode::rfft, f32);
-  if (s != PA_OK) return s;
-  s = need_gpu();
-  if (s != PA_OK) return s;
-  return transpose(&P, comm ? comm->p : nullptr, src, dst, flags, stream, FusedMode::rfft);
-}
-
-pa_status pa_transpose_rfft(pa_plan* plan, pa_comm* comm, const pa_pencil* cplx, const void* src,
-                            void* dst, unsigned flags, void* stream) {
-  GUARD({ return transpose_rfft(plan, comm, cplx, src, dst, flags, stream); })
-}
-
 pa_status pa_plan_real_check(const pa_plan* plan, unsigned flags) {
   return plan_verdict("pa_plan_real_check", plan, Side::unpack, FusedMode::r2r, (flags & PA_FFT_F32) != 0);
+}
+
+// The one-sided fused gather + FFT without the window protocol.  Every check runs on the host
+// before any device call.
+static pa_status get_all_fft(pa_plan* plan, const void* src, void* const* peers, void* dst,
+                             unsigned flags, void* stream) {
+  const char* who = "pa_get_all_fft";
+  if (!plan) {
+    set_error("%s: null plan", who);
+    return PA_EINVAL;
+  }
+  Plan& P = *plan->p;
+  if (P.dim < 0) {
+    set_error("%s: plan has no exchange", who);
+    return PA_EINVAL;
+  }
+  LineOp op;
+  RC(line_op(Side::unpack, FusedMode::fft, true, flags, 0, &op));
+  // the verdict pa_transpose asks (for a PeerGet plan it covers this gather)
+  RC(plan_check(&P, Side::unpack, FusedMode::fft, op.f32));
+  std::vector<const BlockCopy*> blocks;
+  std::vector<void*> srcs;
+  RC(peer_table(who, P, true, src, peers, &blocks, &srcs));
+  RC(fused_pointers(who, src, P.length_in * P.elsize, dst, P.length_out * P.elsize));
+  RC(need_gpu());
+  bool launched = false;
+  return get_fft(P.nproc, blocks.data(), srcs.data(), dst, op, nullptr, stream, &launched);
+}
+
+pa_status pa_get_all_fft(pa_plan* plan, const void* src, void* const* peers, void* dst, unsigned flags,
+                         void* stream) {
+  GUARD({ return get_all_fft(plan, src, peers, dst, flags, stream); })
 }
 
 // ---- send-side fused transform + put (pa_fft_put, pa_rfft_put, pa_r2r_put, pa_brfft_put and
@@ -1086,19 +1092,18 @@ pa_status pa_plan_real_check(const pa_plan* plan, unsigned flags) {
 // complex one), then src / dst (NULL only when empty, not overlapping, aligned: fft / rfft to the
 // complex element; r2r / brfft src to a pair of reals or a complex element, dst to the real).
 static pa_status put_args(const char* who, Plan& P, const pa_pencil* pen, const void* src,
-                          const void* dst, FusedMode mode, bool f32) {
+                          const void* dst, const LineOp& op) {
+  const FusedMode mode = op.mode;
   const bool rfft = mode == FusedMode::rfft, real = put_moves_reals(mode);
-  pa_status s = plan_check(&P, Side::put, mode, f32);
-  if (s != PA_OK) return s;
+  RC(plan_check(&P, Side::put, mode, op.f32));
   const i64 es = P.elsize;
   i64 src_bytes = P.length_in * es;
   if (rfft || mode == FusedMode::brfft) {
     const pa_pencil in{P.pin};
     int N = 0;
     i64 nlines = 0;
-    s = rfft_checks(who, rfft ? pen : &in, rfft ? &in : pen, P.n_extra, P.extra,
-                    PA_FFT_FORWARD | (f32 ? PA_FFT_F32 : 0u), nullptr, nullptr, false, &N, &nlines);
-    if (s != PA_OK) return s;
+    RC(rfft_checks(who, rfft ? pen : &in, rfft ? &in : pen, P.n_extra, P.extra,
+                   PA_FFT_FORWARD | (op.f32 ? PA_FFT_F32 : 0u), nullptr, nullptr, false, &N, &nlines));
     src_bytes = rfft ? nlines * N * (es / 2) : nlines * (N / 2 + 1) * 2 * es;
   }
   const i64 dst_bytes = P.length_out * es;
@@ -1129,140 +1134,76 @@ static pa_status put_args(const char* who, Plan& P, const pa_pencil* pen, const 
   return PA_OK;
 }
 
-// flags: exactly one of PA_FFT_FORWARD / PA_FFT_BACKWARD (fft), or none (rfft, r2r, brfft: the
-// direction is implied), with any of `extra`
-static pa_status put_flags(const char* who, unsigned flags, FusedMode mode, unsigned extra) {
-  if (flags & PA_STAGE_SELF) {
-    set_error("%s: PA_STAGE_SELF does not apply: the send-side fusion stores the self block "
-              "straight into dst", who);
-    return PA_EINVAL;
-  }
-  const bool implied = mode != FusedMode::fft;
-  const unsigned dir = flags & ~extra;
-  if (implied ? dir != 0 : (dir != PA_FFT_FORWARD && dir != PA_FFT_BACKWARD)) {
-    if (implied)
-      set_error("%s: flags may combine %s only (the direction is implied)", who,
-                (extra & PA_WAITALL) ? "PA_WAITALL and PA_FFT_F32" : "PA_FFT_F32");
-    else
-      set_error("%s: flags must be exactly PA_FFT_FORWARD or PA_FFT_BACKWARD, optionally with %s", who,
-                (extra & PA_WAITALL) ? "PA_FFT_F32 and PA_WAITALL" : "PA_FFT_F32");
-    return PA_EINVAL;
-  }
-  return PA_OK;
-}
-
-static const char* put_name(FusedMode mode, bool all) {
-  switch (mode) {
-    case FusedMode::fft: return all ? "pa_put_all_fft" : "pa_fft_put";
-    case FusedMode::rfft: return all ? "pa_put_all_rfft" : "pa_rfft_put";
-    case FusedMode::r2r: return all ? "pa_put_all_r2r" : "pa_r2r_put";
-    case FusedMode::brfft: break;
-  }
-  return all ? "pa_put_all_brfft" : "pa_brfft_put";
-}
-
-static pa_status fft_put(pa_plan* plan, pa_comm* comm, const pa_pencil* pen, const void* src, void* dst,
-                         unsigned flags, void* stream, FusedMode mode, int r2r_kind = 0) {
-  const char* who = put_name(mode, false);
+// all = false: dst = transpose(T(src)) through transpose(), PeerPut's one-sided schedule for a plan
+// with an exchange.  all = true: the fused kernel without the window protocol, the self block into
+// `dst`, the put block of peer n into peers[n - 1] (its dst, as mapped here; the self entry is
+// ignored).
+static pa_status put_fused(pa_plan* plan, pa_comm* comm, const pa_pencil* pen, int kind, const void* src,
+                           void* const* peers, void* dst, unsigned flags, void* stream, FusedMode mode,
+                           bool all) {
+  const char* who = line_op_name(Side::put, mode, all);
   if (!plan) {
     set_error("%s: null plan", who);
     return PA_EINVAL;
   }
-  pa_status s = put_flags(who, flags, mode, PA_FFT_F32 | PA_WAITALL);
-  if (s != PA_OK) return s;
-  if (mode == FusedMode::r2r && (s = r2r_kind_check(who, r2r_kind)) != PA_OK) return s;
   Plan& P = *plan->p;
-  const bool f32 = (flags & PA_FFT_F32) != 0;
-  s = put_args(who, P, pen, src, dst, mode, f32);
-  if (s != PA_OK) return s;
-  s = need_gpu();
-  if (s != PA_OK) return s;
-  return transpose_put_fft(&P, comm ? comm->p : nullptr, src, dst, flags, mode, r2r_kind, stream);
+  if (all && P.dim < 0) {
+    set_error("%s: plan has no exchange", who);
+    return PA_EINVAL;
+  }
+  LineOp op;
+  RC(line_op(Side::put, mode, all, flags, kind, &op));
+  RC(put_args(who, P, pen, src, dst, op));
+  if (!all) {
+    RC(need_gpu());
+    return transpose(&P, comm ? comm->p : nullptr, src, dst, flags, stream, &op);
+  }
+  std::vector<const BlockCopy*> blocks;
+  std::vector<void*> dsts;
+  RC(peer_table(who, P, false, dst, peers, &blocks, &dsts));
+  RC(need_gpu());
+  bool launched = false;
+  return put_fft(P.nproc, blocks.data(), src, dsts.data(), op, nullptr, stream, &launched);
 }
 
 pa_status pa_fft_put(pa_plan* plan, pa_comm* comm, const void* src, void* dst, unsigned flags,
                      void* stream) {
-  GUARD({ return fft_put(plan, comm, nullptr, src, dst, flags, stream, FusedMode::fft); })
+  GUARD({ return put_fused(plan, comm, nullptr, 0, src, nullptr, dst, flags, stream, FusedMode::fft, false); })
 }
 
 pa_status pa_rfft_put(pa_plan* plan, pa_comm* comm, const pa_pencil* real, const void* src, void* dst,
                       unsigned flags, void* stream) {
-  GUARD({ return fft_put(plan, comm, real, src, dst, flags, stream, FusedMode::rfft); })
+  GUARD({ return put_fused(plan, comm, real, 0, src, nullptr, dst, flags, stream, FusedMode::rfft, false); })
 }
 
 pa_status pa_r2r_put(pa_plan* plan, pa_comm* comm, int kind, const void* src, void* dst, unsigned flags,
                      void* stream) {
-  GUARD({ return fft_put(plan, comm, nullptr, src, dst, flags, stream, FusedMode::r2r, kind); })
+  GUARD({ return put_fused(plan, comm, nullptr, kind, src, nullptr, dst, flags, stream, FusedMode::r2r, false); })
 }
 
 pa_status pa_brfft_put(pa_plan* plan, pa_comm* comm, const pa_pencil* cplx, const void* src, void* dst,
                        unsigned flags, void* stream) {
-  GUARD({ return fft_put(plan, comm, cplx, src, dst, flags, stream, FusedMode::brfft); })
-}
-
-// The send-side fused kernel without the window protocol: the self block into `dst`, the put
-// block of peer n into peers[n - 1] (its dst, as mapped here; the self entry is ignored).
-static pa_status put_all_fft(pa_plan* plan, const pa_pencil* pen, const void* src, void* const* peers,
-                             void* dst, unsigned flags, void* stream, FusedMode mode, int r2r_kind = 0) {
-  const char* who = put_name(mode, true);
-  if (!plan) {
-    set_error("%s: null plan", who);
-    return PA_EINVAL;
-  }
-  Plan& P = *plan->p;
-  if (P.dim < 0) {
-    set_error("%s: plan has no exchange", who);
-    return PA_EINVAL;
-  }
-  pa_status s = put_flags(who, flags, mode, PA_FFT_F32);
-  if (s != PA_OK) return s;
-  if (mode == FusedMode::r2r && (s = r2r_kind_check(who, r2r_kind)) != PA_OK) return s;
-  const bool f32 = (flags & PA_FFT_F32) != 0;
-  s = put_args(who, P, pen, src, dst, mode, f32);
-  if (s != PA_OK) return s;
-  const i64 es = P.elsize;
-  std::vector<const BlockCopy*> blocks;
-  std::vector<void*> dsts;
-  for (int n = 0; n < P.nproc; ++n) {
-    const bool self = n == P.self_index;
-    const BlockCopy& b = self ? P.self_fused : P.peers[n].put;
-    void* d = self ? dst : (peers ? peers[n] : nullptr);
-    if (!self && b.count > 0 && !d) {
-      set_error("%s: null peer array for a non-empty block (peer %d)", who, n + 1);
-      return PA_EINVAL;
-    }
-    if (b.count > 0 && ((uintptr_t)d % es)) {
-      set_error("%s: arrays must be aligned to the %lld-byte element", who, (long long)es);
-      return PA_EINVAL;
-    }
-    blocks.push_back(&b);
-    dsts.push_back(d);
-  }
-  s = need_gpu();
-  if (s != PA_OK) return s;
-  bool launched = false;
-  return put_fft(P.nproc, blocks.data(), src, dsts.data(), (flags & PA_FFT_BACKWARD) ? 1 : -1, mode,
-                 r2r_kind, f32, nullptr, stream, &launched);
+  GUARD({ return put_fused(plan, comm, cplx, 0, src, nullptr, dst, flags, stream, FusedMode::brfft, false); })
 }
 
 pa_status pa_put_all_fft(pa_plan* plan, const void* src, void* const* peers, void* dst, unsigned flags,
                          void* stream) {
-  GUARD({ return put_all_fft(plan, nullptr, src, peers, dst, flags, stream, FusedMode::fft); })
+  GUARD({ return put_fused(plan, nullptr, nullptr, 0, src, peers, dst, flags, stream, FusedMode::fft, true); })
 }
 
 pa_status pa_put_all_rfft(pa_plan* plan, const pa_pencil* real, const void* src, void* const* peers,
                           void* dst, unsigned flags, void* stream) {
-  GUARD({ return put_all_fft(plan, real, src, peers, dst, flags, stream, FusedMode::rfft); })
+  GUARD({ return put_fused(plan, nullptr, real, 0, src, peers, dst, flags, stream, FusedMode::rfft, true); })
 }
 
 pa_status pa_put_all_r2r(pa_plan* plan, int kind, const void* src, void* const* peers, void* dst,
                          unsigned flags, void* stream) {
-  GUARD({ return put_all_fft(plan, nullptr, src, peers, dst, flags, stream, FusedMode::r2r, kind); })
+  GUARD({ return put_fused(plan, nullptr, nullptr, kind, src, peers, dst, flags, stream, FusedMode::r2r, true); })
 }
 
 pa_status pa_put_all_brfft(pa_plan* plan, const pa_pencil* cplx, const void* src, void* const* peers,
                            void* dst, unsigned flags, void* stream) {
-  GUARD({ return put_all_fft(plan, cplx, src, peers, dst, flags, stream, FusedMode::brfft); })
+  GUARD({ return put_fused(plan, nullptr, cplx, 0, src, peers, dst, flags, stream, FusedMode::brfft, true); })
 }
 
 pa_status pa_plan_real_put_check(const pa_plan* plan, unsigned flags) {
@@ -1486,3 +1427,25 @@ pa_status pa_plan_enable_timing(pa_plan* plan, int on) {
 }
 
 }  // extern "C"
+
+pa_status pa::transpose_fft_op(Plan* P, unsigned flags, const void* src, const void* dst, LineOp* op,
+                               bool* fused) {
+  *fused = (flags & (PA_FFT_FORWARD | PA_FFT_BACKWARD | PA_FFT_F32)) != 0;
+  if (!*fused) return PA_OK;
+  RC(line_op(Side::unpack, FusedMode::fft, false, flags, 0, op));
+  // a fused FFT this plan cannot run is refused before anything is enqueued -- and on every
+  // rank of the line alike (the peers of a refusing rank must not start the exchange)
+  RC(plan_check(P, Side::unpack, FusedMode::fft, op->f32));
+  // src and dst may not alias -- except for the plain in-place transform along the contiguous
+  // dim (same pencil on both sides, src == dst): a CTA reads its lines completely before it
+  // writes them back
+  const uintptr_t a = (uintptr_t)src, b = (uintptr_t)dst;
+  const bool in_place = src && src == dst && P->dim < 0 && P->same_perm;
+  if (!in_place && src && dst &&
+      (a == b || (a < b + (uintptr_t)(P->length_out * P->elsize) &&
+                  b < a + (uintptr_t)(P->length_in * P->elsize)))) {
+    set_error("fused FFT: src and dst must not alias (in place only between identical pencils)");
+    return PA_EINVAL;
+  }
+  return PA_OK;
+}

@@ -1477,22 +1477,24 @@ static pa_status fft_geometry(int nb, const BlockCopy* const* blocks, const void
   return PA_OK;
 }
 
-pa_status unpack_fused(int nb, const BlockCopy* const* blocks, const void* const* srcs, void* dst, int sign,
-                       FusedMode mode, int r2r_kind, bool f32, void* stream) {
+pa_status unpack_fused(int nb, const BlockCopy* const* blocks, const void* const* srcs, void* dst,
+                       const LineOp& op, void* stream) {
   // (the entry points have already asked plan_check, for every rank of the line, before they
   //  enqueued anything: these checks only guard direct callers)
+  const FusedMode mode = op.mode;
+  const bool f32 = op.f32;
   FftParams p;
   int C = 0;
   unsigned long long grid = 0;
   pa_status s = fft_geometry(nb, blocks, srcs, dst, f32, mode, p, &C, &grid);
   if (s != PA_OK || grid == 0) return s;
   const int logL = p.logL;
-  const bool forward = r2r_forward(r2r_kind);
+  const bool forward = r2r_forward(op.r2r_kind);
   const char* what = "fused FFT";
   void (*kern)(FftParams) = nullptr;
+  p.sign = op.sign;
   switch (mode) {
     case FusedMode::fft:
-      p.sign = sign < 0 ? -1 : 1;
       kern = dispatch<true>(f32, logL, C, [](auto lg, auto c, auto t) { return k_unpack_fft<lg, c, decltype(t)>; });
       break;
     case FusedMode::rfft:
@@ -1503,14 +1505,13 @@ pa_status unpack_fused(int nb, const BlockCopy* const* blocks, const void* const
     case FusedMode::r2r:
       what = "fused r2r";
       p.pitch = pa_fft::padded_pitch(forward ? p.L : p.L + 1);  // as r2r_lines
-      p.sine = r2r_sine(r2r_kind) ? 1 : 0;
+      p.sine = r2r_sine(op.r2r_kind) ? 1 : 0;
       kern = dispatch(f32, logL, C, [forward](auto lg, auto c, auto t) {
         return forward ? k_unpack_r2r<lg, c, true, decltype(t)> : k_unpack_r2r<lg, c, false, decltype(t)>;
       });
       break;
     case FusedMode::brfft:
       what = "fused brfft";
-      p.sign = 1;
       kern = dispatch(f32, logL, C, [](auto lg, auto c, auto t) { return k_unpack_brfft<lg, c, decltype(t)>; });
       break;
   }
@@ -1521,10 +1522,11 @@ pa_status unpack_fused(int nb, const BlockCopy* const* blocks, const void* const
   return launch_lines(what, kern, p, grid, C, p.pitch, f32, stream);
 }
 
-pa_status get_fft(int nb, const BlockCopy* const* blocks, const void* const* srcs, void* dst, int sign,
-                  bool f32, const MultiFlags* mf, void* stream, bool* launched) {
+pa_status get_fft(int nb, const BlockCopy* const* blocks, const void* const* srcs, void* dst,
+                  const LineOp& op, const MultiFlags* mf, void* stream, bool* launched) {
   // (pa_transpose and pa_get_all_fft have already asked plan_check)
   *launched = false;
+  const bool f32 = op.f32;
   FftGetParams gp;
   int C = 0;
   unsigned long long grid = 0;
@@ -1533,7 +1535,7 @@ pa_status get_fft(int nb, const BlockCopy* const* blocks, const void* const* src
   FftParams& p = gp.p;
   memset(&gp.mf, 0, sizeof gp.mf);
   if (mf) gp.mf = *mf;
-  p.sign = sign < 0 ? -1 : 1;
+  p.sign = op.sign;
   s = line_twiddles("fused FFT", f32, p.L, &p.tw);
   if (s != PA_OK) return s;
   auto kern = dispatch<true>(f32, p.logL, C, [](auto lg, auto c, auto t) { return k_get_fft<lg, c, decltype(t)>; });
@@ -1725,10 +1727,12 @@ static pa_status put_fft_geometry(int nb, const BlockCopy* const* blocks, const 
   return PA_OK;
 }
 
-pa_status put_fft(int nb, const BlockCopy* const* blocks, const void* src, void* const* dsts, int sign,
-                  FusedMode mode, int r2r_kind, bool f32, const MultiFlags* mf, void* stream, bool* launched) {
+pa_status put_fft(int nb, const BlockCopy* const* blocks, const void* src, void* const* dsts,
+                  const LineOp& op, const MultiFlags* mf, void* stream, bool* launched) {
   // (the entry points have already asked plan_check)
   *launched = false;
+  const FusedMode mode = op.mode;
+  const bool f32 = op.f32;
   FftPutParams pp;
   int C = 0;
   unsigned long long grid = 0;
@@ -1738,8 +1742,8 @@ pa_status put_fft(int nb, const BlockCopy* const* blocks, const void* src, void*
   FftParams& p = pp.p;
   const int logL = p.logL;
   // r2r: the 10 kinds run k_r2r's forward path, the 01 kinds its backward one
-  const bool r2r_fwd = r2r_forward(r2r_kind);
-  p.sign = mode == FusedMode::rfft ? -1 : (sign < 0 ? -1 : 1);
+  const bool r2r_fwd = r2r_forward(op.r2r_kind);
+  p.sign = op.sign;
   void (*kern)(FftPutParams) = nullptr;
   switch (mode) {
     case FusedMode::fft:
@@ -1749,7 +1753,7 @@ pa_status put_fft(int nb, const BlockCopy* const* blocks, const void* src, void*
       kern = dispatch(f32, logL, C, [](auto lg, auto c, auto t) { return k_rfft_put<lg, c, decltype(t)>; });
       break;
     case FusedMode::r2r:
-      p.sine = r2r_sine(r2r_kind) ? 1 : 0;
+      p.sine = r2r_sine(op.r2r_kind) ? 1 : 0;
       kern = dispatch(f32, logL, C, [r2r_fwd](auto lg, auto c, auto t) {
         return r2r_fwd ? k_r2r_put<lg, c, true, decltype(t)> : k_r2r_put<lg, c, false, decltype(t)>;
       });

@@ -20,6 +20,13 @@ using i64 = int64_t;
 void set_error(const char* fmt, ...);
 const char* last_error();
 
+// return a failed status to the caller
+#define RC(call)                    \
+  do {                              \
+    pa_status rc_ = (call);         \
+    if (rc_ != PA_OK) return rc_;   \
+  } while (0)
+
 // ---- MPITopology (MPITopologies.jl:72-119) ---------------------------------
 struct Topology {
   int M = 0;
@@ -284,6 +291,17 @@ enum class FusedMode {
   r2r,    // N reals -> N reals, a DCT / DST
   brfft,  // N/2 + 1 complex bins -> N reals
 };
+enum class Side { unpack, put };
+// What a fused line kernel computes, and on which side of the exchange.  The entry points decode
+// it from their flags (and r2r's kind) and check it once; below them flags carry the schedule bits
+// only (PA_WAITALL, PA_NO_OVERLAP, PA_STAGE_SELF).
+struct LineOp {
+  Side side;       // unpack: unpack_fused / get_fft; put: put_fft
+  FusedMode mode;
+  int sign;        // fft only: -1 forward, +1 backward (0 otherwise: no kernel reads it)
+  int r2r_kind;    // r2r only: PA_REDFT10 / PA_REDFT01 / PA_RODFT10 / PA_RODFT01
+  bool f32;        // PA_FFT_F32: single precision
+};
 // the plan moves reals: the destination's on the receive side, the source's on the send side
 inline bool unpack_moves_reals(FusedMode m) { return m == FusedMode::r2r || m == FusedMode::rfft; }
 inline bool put_moves_reals(FusedMode m) { return m == FusedMode::r2r || m == FusedMode::brfft; }
@@ -293,11 +311,15 @@ inline bool put_moves_reals(FusedMode m) { return m == FusedMode::r2r || m == Fu
 inline bool r2r_forward(int kind) { return kind == PA_REDFT10 || kind == PA_RODFT10; }
 inline bool r2r_sine(int kind) { return kind == PA_RODFT10 || kind == PA_RODFT01; }
 
-// mode brfft / r2r / rfft: dst = brfft / r2r / rfft(transpose(src)) through the fused unpack;
-// flags then hold no FFT direction, PA_FFT_F32 selects the precision; r2r_kind: the PA_*ODFT*
-// kind of r2r
+// dst = transpose(src); op (NULL: none) fuses a line transform into it: op->side unpack, dst =
+// T(transpose(src)) through the fused unpack; put, dst = transpose(T(src)) on the caller's stream
+// (local plans) or PeerPut's one-sided schedule.  Every argument has been checked.
 pa_status transpose(Plan* plan, Comm* comm, const void* src, void* dst, unsigned flags,
-                    void* stream, FusedMode mode = FusedMode::fft, int r2r_kind = 0);
+                    void* stream, const LineOp* op = nullptr);
+// pa_transpose's fused FFT (capi.cpp): the PA_FFT_* bits of flags decoded into *op and checked
+// (the plan's verdict, the alias rule); *fused = false when flags hold none
+pa_status transpose_fft_op(Plan* plan, unsigned flags, const void* src, const void* dst, LineOp* op,
+                           bool* fused);
 pa_status wait_sends(Plan* plan, void* stream);
 pa_status permute_local(Plan* plan, const void* src, void* dst, void* scratch, void* stream);
 pa_status transpose_host(Plan* plan, Comm* comm, const void* hsrc, void* hdst, unsigned flags);
@@ -322,44 +344,34 @@ pa_status host_chain_buffer(HostChain* c, int slot, int which, void** p, i64* by
 pa_status host_chain_time_begin(HostChain* c);
 pa_status host_chain_time_end(HostChain* c, float* ms);
 
-// fused unpack + line transform along the destination's contiguous dim (fft.cu, k_unpack_fft /
+// fused unpack + line transform op along the destination's contiguous dim (fft.cu, k_unpack_fft /
 // k_unpack_rfft / k_unpack_r2r / k_unpack_brfft): the blocks together tile the destination box;
 // srcs[i] = base pointer blocks[i] reads from.  The plan's elements: fft ComplexF64, rfft / r2r
-// Float64, brfft ComplexF64, or their single-precision counterparts with f32 (PA_FFT_F32).  fft:
-// sign -1 forward, +1 backward.  rfft: `dst` is the complex array of N/2 + 1 bins per line that
-// replaces the real destination (same layout otherwise); brfft: `dst` is the real array of N reals
-// per line that replaces the complex one.  r2r: r2r_kind one of PA_REDFT10 / PA_REDFT01 /
-// PA_RODFT10 / PA_RODFT01
-pa_status unpack_fused(int nb, const BlockCopy* const* blocks, const void* const* srcs, void* dst, int sign,
-                       FusedMode mode, int r2r_kind, bool f32, void* stream);
+// Float64, brfft ComplexF64, or their single-precision counterparts with op.f32.  rfft: `dst` is
+// the complex array of N/2 + 1 bins per line that replaces the real destination (same layout
+// otherwise); brfft: `dst` is the real array of N reals per line that replaces the complex one
+pa_status unpack_fused(int nb, const BlockCopy* const* blocks, const void* const* srcs, void* dst,
+                       const LineOp& op, void* stream);
 // the complex FFT's kernel one-sided (fft.cu, k_get_fft): srcs[i] are the peers' src arrays as
 // mapped here (the self block's: the local src), read in place, and `mf` (NULL: none) the window
 // protocol spoken inside the launch.  *launched = false: this rank has no destination lines and
 // nothing was launched -- the caller then speaks the protocol with flag kernels
-pa_status get_fft(int nb, const BlockCopy* const* blocks, const void* const* srcs, void* dst, int sign,
-                  bool f32, const MultiFlags* mf, void* stream, bool* launched);
+pa_status get_fft(int nb, const BlockCopy* const* blocks, const void* const* srcs, void* dst,
+                  const LineOp& op, const MultiFlags* mf, void* stream, bool* launched);
 // send-side fused transform + put (fft.cu, k_fft_put / k_rfft_put / k_r2r_put / k_brfft_put): the
 // transform along the first memory dim of the local `src`, every output element stored into the
 // block that owns it.  blocks[i] / dsts[i]: the self block (self_fused) into the local dst, the put
-// block of every other rank into that rank's dst as mapped here.  fft: sign -1 forward, +1
-// backward; r2r: r2r_kind one of PA_REDFT10 / PA_REDFT01 / PA_RODFT10 / PA_RODFT01.  `mf` (NULL:
-// none): the window protocol spoken inside the launch.  *launched = false: this rank has no source
-// lines and nothing was launched -- the caller then speaks the protocol with flag kernels
-pa_status put_fft(int nb, const BlockCopy* const* blocks, const void* src, void* const* dsts, int sign,
-                  FusedMode mode, int r2r_kind, bool f32, const MultiFlags* mf, void* stream,
-                  bool* launched);
+// block of every other rank into that rank's dst as mapped here.  `mf` (NULL: none): the window
+// protocol spoken inside the launch.  *launched = false: this rank has no source lines and nothing
+// was launched -- the caller then speaks the protocol with flag kernels
+pa_status put_fft(int nb, const BlockCopy* const* blocks, const void* src, void* const* dsts,
+                  const LineOp& op, const MultiFlags* mf, void* stream, bool* launched);
 // Can the fused kernel of `mode` run on this plan, on the receive side (unpack_fused; the complex
 // FFT of a PeerGet plan: get_fft too) or on the send side (put_fft: PeerPut plans and local
 // transposes only)?  The same answer on every rank of the grid line (global geometry only);
 // PA_EINVAL + last_error otherwise.  Cached per plan, side, transform and precision; r2r shares
 // the answer of rfft (receive side) or brfft (send side).  No device call.
-enum class Side { unpack, put };
 pa_status plan_check(Plan* plan, Side side, FusedMode mode, bool f32);
-// dst = transpose(T(src)), T the transform of `mode` (fft: its direction from flags; r2r: kind
-// r2r_kind), on the caller's stream (local plans) or PeerPut's one-sided schedule; every argument
-// has been checked
-pa_status transpose_put_fft(Plan* plan, Comm* comm, const void* src, void* dst, unsigned flags,
-                            FusedMode mode, int r2r_kind, void* stream);
 // real-line transforms (fft.cu): `nlines` dense, consecutive lines of N reals (src when forward,
 // dst when backward) <-> N/2 + 1 complex bins; N a power of two in 16..2048.  f32: Float32 <->
 // ComplexF32, else Float64 <-> ComplexF64

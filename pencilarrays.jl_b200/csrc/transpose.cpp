@@ -56,12 +56,6 @@ constexpr size_t IPC_BLOCK = 2u << 20;
     }                                                                             \
   } while (0)
 
-#define RC(call)                    \
-  do {                              \
-    pa_status rc_ = (call);         \
-    if (rc_ != PA_OK) return rc_;   \
-  } while (0)
-
 pa_status set_device(int dev) {
   CU(cudaSetDevice(dev));
   return PA_OK;
@@ -733,19 +727,18 @@ static BlockCopy contiguous_block(i64 bytes, const void* src, const void* dst) {
 // READY ("my side of the window may be touched": my dest may be overwritten /
 // my src is final) before the first remote access, DONE ("all my accesses to
 // your memory are complete") after the last.
-// fft_sign != 0 (PeerGet only): the fused gather + FFT (k_get_fft) replaces the get kernel and
-// the self block -- ONE kernel reads every line from the peers' src and the local src,
-// transforms and stores it; the protocol around it is the same.
-// send != NULL (PeerPut only): the send-side fused transform of mode *send (k_fft_put,
-// k_rfft_put, k_r2r_put, k_brfft_put) replaces the put kernel and the self block -- ONE kernel
-// loads every local source line, transforms it and stores its outputs into the local dst and the
-// peers' dst (fft_sign: the FFT's direction; r2r_kind: the DCT / DST).
+// op on the receive side (PeerGet only, the complex FFT): the fused gather + FFT (k_get_fft)
+// replaces the get kernel and the self block -- ONE kernel reads every line from the peers' src and
+// the local src, transforms and stores it; the protocol around it is the same.
+// op on the send side (PeerPut only): the send-side fused transform (k_fft_put, k_rfft_put,
+// k_r2r_put, k_brfft_put) replaces the put kernel and the self block -- ONE kernel loads every
+// local source line, transforms it and stores its outputs into the local dst and the peers' dst.
 static pa_status one_sided(Plan* P, Comm* comm, const void* src, void* dst, unsigned flags,
-                           int fft_sign, const FusedMode* send, int r2r_kind, cudaStream_t user) {
+                           const LineOp* op, cudaStream_t user) {
   TransposeState& S = *P->st;
   const int nproc = P->nproc, me = P->self_index;
   const bool get = P->method == PA_PEER_GET;
-  const bool fft = fft_sign != 0 || send;  // one fused kernel replaces the blocks
+  const bool fft = op != nullptr;  // one fused kernel replaces the blocks
   const bool timing = S.timing;
   // (a rank none of whose peers owns anything has no window to register: nothing will be
   //  put / got, but it still speaks the protocol)
@@ -803,11 +796,8 @@ static pa_status one_sided(Plan* P, Comm* comm, const void* src, void* dst, unsi
     fd.push_back(n == me ? dst : win[n]);
   }
   auto fused = [&](const MultiFlags* mf, bool* launched) {
-    const bool f32 = (flags & PA_FFT_F32) != 0;
-    if (send)
-      return put_fft(nproc, fb.data(), src, fd.data(), fft_sign, *send, r2r_kind, f32, mf, S.comm_s,
-                     launched);
-    return get_fft(nproc, fb.data(), fs.data(), dst, fft_sign, f32, mf, S.comm_s, launched);
+    if (op->side == Side::put) return put_fft(nproc, fb.data(), src, fd.data(), *op, mf, S.comm_s, launched);
+    return get_fft(nproc, fb.data(), fs.data(), dst, *op, mf, S.comm_s, launched);
   };
   bool launched = false;
 
@@ -914,16 +904,13 @@ static pa_status one_sided(Plan* P, Comm* comm, const void* src, void* dst, unsi
     CU(cudaStreamWaitEvent(user, S.ev_comm_done, 0));
     S.sends_pending = false;
   }
-  if (timing) {
-    CU(cudaEventRecord(S.t[6], user));
-    S.timed_once = true;
-  }
   return PA_OK;
 }
 
 // ---- the staged schedules (PointToPoint / Alltoallv) --------------------------------
+// op (NULL: none): the fused unpack (receive side) that replaces the unpacks and the self block
 static pa_status staged(Plan* P, Comm* comm, const void* src, void* dst, unsigned flags,
-                        FusedMode mode, int r2r_kind, bool stage_self, cudaStream_t user, cudaEvent_t buf_ev,
+                        const LineOp* op, bool stage_self, cudaStream_t user, cudaEvent_t buf_ev,
                         cudaEvent_t buf_unpack_ev) {
   TransposeState& S = *P->st;
   Buffers& B = *P->pout->bufs;
@@ -967,13 +954,11 @@ static pa_status staged(Plan* P, Comm* comm, const void* src, void* dst, unsigne
   // same stream (fused K3: src -> dest in one pass) and fills the HBM time the
   // NVLink-bound exchange leaves idle.  tunable "self_first" = 1 restores the
   // reference's order (self block packed first, :393-403).
-  // (brfft / r2r / rfft: flags hold no direction, the fused unpack is that mode's)
-  const int fft_sign = mode != FusedMode::fft ? 1
-                       : (flags & PA_FFT_FORWARD) ? -1 : ((flags & PA_FFT_BACKWARD) ? 1 : 0);
+  const bool fused = op != nullptr;
   const bool self_first = stage_self || g_tun.self_first;
   if (stage_self) {
     RC(launch_block(self.pack, src, rbuf, S.pack_s, nullptr));  // tail of recv_buf (:393-403)
-  } else if (fft_sign) {
+  } else if (fused) {
     // (the fused unpack+FFT kernel gathers the self block straight out of src)
   } else if (self_first) {
     RC(launch_block(P->self_fused, src, dst, S.unpack_s, nullptr));  // K3, one pass
@@ -987,7 +972,7 @@ static pa_status staged(Plan* P, Comm* comm, const void* src, void* dst, unsigne
   }
   CU(cudaEventRecord(S.ev_allpacked, S.pack_s));
   if (timing) CU(cudaEventRecord(S.t[1], S.pack_s));
-  if (!self_first && !fft_sign) RC(launch_block(P->self_fused, src, dst, S.pack_s, nullptr, cap));
+  if (!self_first && !fused) RC(launch_block(P->self_fused, src, dst, S.pack_s, nullptr, cap));
   CU(cudaEventRecord(S.ev_self_done, S.pack_s));
 
   // ---- 2. exchange -------------------------------------------------------------
@@ -1081,7 +1066,7 @@ static pa_status staged(Plan* P, Comm* comm, const void* src, void* dst, unsigne
         }
       }
     }
-    if (ipc && (!overlap || fft_sign)) {
+    if (ipc && (!overlap || fused)) {
       // sequential phases: every block has landed before the first unpack
       for (int k = 1; k < nproc; ++k)
         for (int c = 0; c < C; ++c) {
@@ -1142,7 +1127,7 @@ static pa_status staged(Plan* P, Comm* comm, const void* src, void* dst, unsigne
   // the reference finishes transpose_send! before transpose_recv! (:326-340).
   if (stage_self) CU(cudaStreamWaitEvent(S.unpack_s, S.ev_allpacked, 0));
   if (timing) CU(cudaEventRecord(S.t[4], S.unpack_s));
-  if (fft_sign) {
+  if (fused) {
     // ONE kernel: gather every block (remote ones from recv_buf, the self block from src
     // or from the tail of recv_buf), transform along the now-local contiguous dim, store
     CU(cudaStreamWaitEvent(S.unpack_s, S.ev_comm_done, 0));
@@ -1153,12 +1138,11 @@ static pa_status staged(Plan* P, Comm* comm, const void* src, void* dst, unsigne
       bl.push_back(fused_self ? &P->self_fused : &P->peers[n].unpack);
       sp.push_back(fused_self ? src : (const void*)rbuf);
     }
-    const bool f32 = (flags & PA_FFT_F32) != 0;
-    RC(unpack_fused(nproc, bl.data(), sp.data(), dst, fft_sign, mode, r2r_kind, f32, S.unpack_s));
+    RC(unpack_fused(nproc, bl.data(), sp.data(), dst, *op, S.unpack_s));
   } else if (stage_self) {
     RC(launch_block(self.unpack, rbuf, dst, S.unpack_s, nullptr));  // local data first (:511)
   }
-  if (fft_sign) {
+  if (fused) {
     // (nothing else to unpack)
   } else if (p2p && overlap) {
     for (int k = 1; k < nproc; ++k) {
@@ -1195,59 +1179,37 @@ static pa_status staged(Plan* P, Comm* comm, const void* src, void* dst, unsigne
     CU(cudaStreamWaitEvent(user, S.ev_comm_done, 0));  // MPI.Waitall(t) (:174-176)
     S.sends_pending = false;
   }
-  if (timing) {
-    CU(cudaEventRecord(S.t[6], user));
-    S.timed_once = true;
-  }
   return PA_OK;
 }
 
 pa_status transpose(Plan* P, Comm* comm, const void* src, void* dst, unsigned flags,
-                    void* stream, FusedMode mode, int r2r_kind) {
-  // a rank may own nothing (more processes than points, Pencils.jl:193-218): its
-  // empty arrays have no storage, yet it takes part in the exchange
-  if ((!src && P->length_in > 0) || (!dst && P->length_out > 0)) {
-    set_error("pa_transpose: null array pointer");
-    return PA_EINVAL;
-  }
-  // (real_line -- brfft, r2r, rfft: a real array on one side; their entry points have checked src
-  //  against dst, whose element type or length the plan may not know)
-  const bool real_line = mode != FusedMode::fft;
-  const int fft_sign = real_line ? 1 : (flags & PA_FFT_FORWARD) ? -1 : ((flags & PA_FFT_BACKWARD) ? 1 : 0);
-  const bool fft_f32 = (flags & PA_FFT_F32) != 0;  // ComplexF32 elements (elsize 8)
-  if (fft_f32 && !fft_sign) {
-    set_error("pa_transpose: PA_FFT_F32 without PA_FFT_FORWARD / PA_FFT_BACKWARD");
-    return PA_EINVAL;
-  }
-  // a fused FFT this plan cannot run is refused before anything is enqueued -- and on every
-  // rank of the line alike (the peers of a refusing rank must not start the exchange)
-  if (fft_sign) RC(plan_check(P, Side::unpack, mode, fft_f32));
+                    void* stream, const LineOp* op) {
   RC(ensure_state(P));
   TransposeState& S = *P->st;
   cudaStream_t user = (cudaStream_t)stream;
   const i64 ES = P->elsize;
   const bool timing = S.timing;
   if (timing) CU(cudaEventRecord(S.t[0], user));
-
-  // src and dst may not alias -- except for the plain in-place transform along the contiguous
-  // dim (same pencil on both sides, src == dst): a CTA reads its lines completely before it
-  // writes them back.  (real_line: checked by the entry point)
-  const bool fft_in_place = fft_sign && !real_line && src && src == dst && P->dim < 0 && P->same_perm;
-  if (fft_sign && !real_line && !fft_in_place && src && dst &&
-      (src == dst || ranges_overlap(src, P->length_in * ES, dst, P->length_out * ES))) {
-    set_error("fused FFT: src and dst must not alias (in place only between identical pencils)");
-    return PA_EINVAL;
-  }
-  if (fft_sign && (P->dim < 0 || P->nproc == 1)) {
-    // one block: the whole local array, src -> fft(permuted dest)
-    if (P->length_out == 0) return PA_OK;
-    const BlockCopy* b = &P->self_fused;
-    RC(unpack_fused(1, &b, &src, dst, fft_sign, mode, r2r_kind, fft_f32, user));
+  auto timed_end = [&]() -> pa_status {
     if (timing) {
       CU(cudaEventRecord(S.t[6], user));
       S.timed_once = true;
     }
     return PA_OK;
+  };
+
+  if (op && (P->dim < 0 || P->nproc == 1)) {
+    // one block, the whole local array: src -> T(permuted dest) / permuted T(src), one kernel on the
+    // caller's stream
+    const BlockCopy* b = &P->self_fused;
+    if (op->side == Side::put) {
+      bool launched = false;
+      RC(put_fft(1, &b, src, &dst, *op, nullptr, user, &launched));
+    } else {
+      if (P->length_out == 0) return PA_OK;
+      RC(unpack_fused(1, &b, &src, dst, *op, user));
+    }
+    return timed_end();
   }
 
   if (P->dim < 0) {
@@ -1263,11 +1225,7 @@ pa_status transpose(Plan* P, Comm* comm, const void* src, void* dst, unsigned fl
     }
     RC(local_transpose(P, src, dst, scratch, user));
     if (staged_local) RC(arena_release(*P->pin->bufs, user));
-    if (timing) {
-      CU(cudaEventRecord(S.t[6], user));
-      S.timed_once = true;
-    }
-    return PA_OK;
+    return timed_end();
   }
 
   const int nproc = P->nproc, me = P->self_index;
@@ -1278,14 +1236,17 @@ pa_status transpose(Plan* P, Comm* comm, const void* src, void* dst, unsigned fl
   }
   Buffers& B = *P->pout->bufs;  // Po.send_buf / Po.recv_buf (:313-317)
   // (same base pointer counts even when one side is empty on this rank: every rank of
-  //  an in-place transpose must take the same schedule)
-  const bool aliased = !real_line && src && dst &&
+  //  an in-place transpose must take the same schedule.  The real-line modes and the send side
+  //  have refused aliased arrays at their entry points)
+  const bool may_alias = !op || (op->side == Side::unpack && op->mode == FusedMode::fft);
+  const bool aliased = may_alias && src && dst &&
       (src == dst || ranges_overlap(src, P->length_in * ES, dst, P->length_out * ES));
   const bool stage_self = aliased || (flags & PA_STAGE_SELF);
   const bool one = (P->method == PA_PEER_PUT || P->method == PA_PEER_GET) && !stage_self && nproc > 1;
   // (PeerGet runs the complex FFT one-sided, k_get_fft; a put has nothing to fuse with, and the
-  //  real-line modes have been refused for both methods by their plan checks)
-  if (fft_sign && one && (P->method == PA_PEER_PUT || real_line)) {
+  //  real-line modes have been refused for both methods by their plan checks.  The send side runs
+  //  on PeerPut plans only: their verdict)
+  if (op && op->side == Side::unpack && one && (P->method == PA_PEER_PUT || op->mode != FusedMode::fft)) {
     set_error("fused FFT: the one-sided methods have no unpack pass to fuse with; use "
               "PointToPoint / Alltoallv");
     return PA_EINVAL;
@@ -1310,11 +1271,7 @@ pa_status transpose(Plan* P, Comm* comm, const void* src, void* dst, unsigned fl
     } else {
       RC(launch_block(P->self_fused, src, dst, user, nullptr, 0, true));
     }
-    if (timing) {
-      CU(cudaEventRecord(S.t[6], user));
-      S.timed_once = true;
-    }
-    return PA_OK;
+    return timed_end();
   }
 
   cudaEvent_t buf_ev, buf_unpack_ev;
@@ -1328,48 +1285,11 @@ pa_status transpose(Plan* P, Comm* comm, const void* src, void* dst, unsigned fl
     CU(cudaStreamWaitEvent(s, buf_ev, 0));
     CU(cudaStreamWaitEvent(s, buf_unpack_ev, 0));
   }
-  if (one) return one_sided(P, comm, src, dst, flags, fft_sign, nullptr, 0, user);
-  return staged(P, comm, src, dst, flags, mode, r2r_kind, stage_self, user, buf_ev, buf_unpack_ev);
-}
-
-pa_status transpose_put_fft(Plan* P, Comm* comm, const void* src, void* dst, unsigned flags, FusedMode mode,
-                            int r2r_kind, void* stream) {
-  // (pa_fft_put / pa_rfft_put / pa_r2r_put / pa_brfft_put have checked the flags, the arrays and
-  //  the plan's verdict, which admits PeerPut plans and local transposes only)
-  RC(ensure_state(P));
-  TransposeState& S = *P->st;
-  cudaStream_t user = (cudaStream_t)stream;
-  const bool timing = S.timing;
-  const int sign = mode != FusedMode::fft || (flags & PA_FFT_FORWARD) ? -1 : 1;
-  const bool f32 = (flags & PA_FFT_F32) != 0;
-  if (timing) CU(cudaEventRecord(S.t[0], user));
-  if (P->dim < 0 || P->nproc == 1) {
-    // one block, the whole local array: one kernel on the caller's stream
-    const BlockCopy* b = &P->self_fused;
-    bool launched = false;
-    RC(put_fft(1, &b, src, &dst, sign, mode, r2r_kind, f32, nullptr, user, &launched));
-    if (timing) {
-      CU(cudaEventRecord(S.t[6], user));
-      S.timed_once = true;
-    }
-    return PA_OK;
-  }
-  if (!comm) {
-    set_error("this transposition exchanges data among %d ranks: a communicator is required",
-              P->nproc);
-    return PA_ESTATE;
-  }
-  // fork as transpose() does for the one-sided methods
-  Buffers& B = *P->pout->bufs;
-  cudaEvent_t buf_ev, buf_unpack_ev;
-  RC(buffer_events(B, &buf_ev, &buf_unpack_ev));
-  CU(cudaEventRecord(S.ev_start, user));
-  for (cudaStream_t s : {S.pack_s, S.comm_s, S.unpack_s}) {
-    CU(cudaStreamWaitEvent(s, S.ev_start, 0));
-    CU(cudaStreamWaitEvent(s, buf_ev, 0));
-    CU(cudaStreamWaitEvent(s, buf_unpack_ev, 0));
-  }
-  return one_sided(P, comm, src, dst, flags, sign, &mode, r2r_kind, user);
+  if (one)
+    RC(one_sided(P, comm, src, dst, flags, op, user));
+  else
+    RC(staged(P, comm, src, dst, flags, op, stage_self, user, buf_ev, buf_unpack_ev));
+  return timed_end();
 }
 
 // MPI.Waitall(t::Transposition) (Transpositions.jl:127-130)
@@ -1485,8 +1405,12 @@ pa_status transpose_host(Plan* P, Comm* comm, const void* hsrc, void* hdst, unsi
     return PA_OK;
   }
   cudaStream_t s = S.host_s;
+  // (PA_FFT_* pass through to the one-call path only: the cuts above run plain copies)
+  LineOp op;
+  bool fused = false;
+  RC(transpose_fft_op(P, flags, P->h_src_dev, P->h_dst_dev, &op, &fused));
   if (nin > 0) CU(cudaMemcpyAsync(P->h_src_dev, hsrc, (size_t)nin, cudaMemcpyHostToDevice, s));
-  RC(transpose(P, comm, P->h_src_dev, P->h_dst_dev, flags | PA_WAITALL, s));
+  RC(transpose(P, comm, P->h_src_dev, P->h_dst_dev, flags | PA_WAITALL, s, fused ? &op : nullptr));
   if (nout > 0) CU(cudaMemcpyAsync(hdst, P->h_dst_dev, (size_t)nout, cudaMemcpyDeviceToHost, s));
   CU(cudaStreamSynchronize(s));
   return PA_OK;

@@ -24,6 +24,7 @@ from __future__ import annotations
 
 import ctypes as C
 import threading
+from typing import NamedTuple
 
 import torch
 
@@ -294,8 +295,62 @@ def _rfft_pencil(cplx: Pencil) -> Pencil:
     return pr
 
 
-_BRFFT_PAIRS = {(torch.float64, torch.complex128): 0, (torch.float32, torch.complex64): _lib.PA_FFT_F32}
-_REAL_FLAGS = {torch.float64: 0, torch.float32: _lib.PA_FFT_F32}
+_BRFFT_PAIRS = {(torch.float64, torch.complex128), (torch.float32, torch.complex64)}
+_REAL_DTYPES = (torch.float64, torch.float32)
+
+
+class _Fused(NamedTuple):
+    """One fused line transform, keyed by (side, mode) in :data:`_FUSED`."""
+    kw: str          # the kwarg that asks for it, as the messages name it
+    real: str        # the real array: "Ai" (src), "Ao" (dest), "both" or "" (complex on both sides)
+    pencils: object  # (Ai, Ao) -> the plan's (Pi, Po): a derived pencil on the complex side
+    elsize: str      # the array that gives the plan's element size
+    verdict: str     # the pa_plan_*check* that answers whether the fused kernel can run
+    call: object     # (t, comm, src, dst, flags, stream) -> status
+
+
+def _own(Ai, Ao):
+    return Ai.pencil, Ao.pencil
+
+
+def _brfft_first_pencils(Ai, Ao):
+    # the plan's input: the real counterpart of src, N points as in dest
+    ax = as_tuple(Ai.pencil.perm, Ai.pencil.ndims)[0] - 1
+    return _real_pencil_of(Ai.pencil, Ao.pencil.size_global[ax]), Ao.pencil
+
+
+# receive side: dest = T(transpose(src)); send side: dest = transpose(T(src))
+_FUSED = {
+    ("unpack", "fft"): _Fused(
+        "fft", "", _own, "Ai", "pa_plan_fft_check_ex",
+        lambda t, comm, s, d, f, st: lib.pa_transpose(t.plan.h, comm, s, d, f, st)),
+    ("unpack", "brfft"): _Fused(
+        "brfft", "Ao", lambda Ai, Ao: (Ai.pencil, _brfft_pencil(Ao.pencil)), "Ai", "pa_plan_brfft_check",
+        lambda t, comm, s, d, f, st: lib.pa_transpose_brfft(t.plan.h, comm, t.Ao.pencil._h, s, d, f, st)),
+    ("unpack", "r2r"): _Fused(
+        "r2r", "both", _own, "Ai", "pa_plan_real_check",
+        lambda t, comm, s, d, f, st: lib.pa_transpose_r2r(t.plan.h, comm, _R2R_KINDS[t._op[2]], s, d, f, st)),
+    ("unpack", "rfft"): _Fused(
+        "rfft", "Ai", lambda Ai, Ao: (Ai.pencil, _rfft_pencil(Ao.pencil)), "Ai", "pa_plan_real_check",
+        lambda t, comm, s, d, f, st: lib.pa_transpose_rfft(t.plan.h, comm, t.Ao.pencil._h, s, d, f, st)),
+    ("put", "fft"): _Fused(
+        "fft_first", "", _own, "Ai", "pa_plan_fft_put_check",
+        lambda t, comm, s, d, f, st: lib.pa_fft_put(t.plan.h, comm, s, d, f, st)),
+    ("put", "rfft"): _Fused(
+        "rfft_first", "Ai", lambda Ai, Ao: (_brfft_pencil(Ai.pencil), Ao.pencil), "Ao",
+        "pa_plan_rfft_put_check",
+        lambda t, comm, s, d, f, st: lib.pa_rfft_put(t.plan.h, comm, t.Ai.pencil._h, s, d, f, st)),
+    ("put", "r2r"): _Fused(
+        "r2r_first", "both", _own, "Ai", "pa_plan_real_put_check",
+        lambda t, comm, s, d, f, st: lib.pa_r2r_put(t.plan.h, comm, _R2R_KINDS[t._op[2]], s, d, f, st)),
+    ("put", "brfft"): _Fused(
+        "brfft_first", "Ao", _brfft_first_pencils, "Ao", "pa_plan_real_put_check",
+        lambda t, comm, s, d, f, st: lib.pa_brfft_put(t.plan.h, comm, t.Ai.pencil._h, s, d, f, st)),
+}
+
+
+def _article(kw: str) -> str:
+    return "a" if kw.startswith("b") else "an"
 
 
 class Transposition:
@@ -337,86 +392,57 @@ class Transposition:
     def __init__(self, Ao: PencilArray, Ai: PencilArray, *, method=None, brfft=False, r2r=None,
                  rfft=False, rfft_first=False, r2r_first=None, brfft_first=False):
         method = PointToPoint() if method is None else method
-        Pi, Po = Ai.pencil, Ao.pencil
-        self.brfft = bool(brfft)
-        self.r2r = r2r
-        self.rfft = bool(rfft)
-        self.rfft_first = bool(rfft_first)
-        self.r2r_first = r2r_first
-        self.brfft_first = bool(brfft_first)
-        if self.brfft + (r2r is not None) + self.rfft + self.rfft_first > 1:
-            raise ArgumentError(_lib.PA_EINVAL, "brfft=, r2r=, rfft= and rfft_first= exclude each other")
-        if (self.brfft + (r2r is not None) + self.rfft + self.rfft_first + (r2r_first is not None)
-                + self.brfft_first > 1):
-            raise ArgumentError(_lib.PA_EINVAL, "brfft=, r2r=, rfft=, rfft_first=, r2r_first= and "
-                                "brfft_first= exclude each other")
+        asked = [(("unpack", "brfft", None), bool(brfft)), (("unpack", "r2r", r2r), r2r is not None),
+                 (("unpack", "rfft", None), bool(rfft)), (("put", "rfft", None), bool(rfft_first)),
+                 (("put", "r2r", r2r_first), r2r_first is not None),
+                 (("put", "brfft", None), bool(brfft_first))]
+        ops = [op for op, on in asked if on]
+        if len(ops) > 1:
+            raise ArgumentError(_lib.PA_EINVAL, "brfft=, r2r=, rfft= and rfft_first= exclude each other"
+                                if sum(on for _, on in asked[:4]) > 1 else
+                                "brfft=, r2r=, rfft=, rfft_first=, r2r_first= and brfft_first= exclude "
+                                "each other")
+        # (side, mode, r2r kind) of the fused transform; None: a complex transposition, fft= /
+        # fft_first= choose at transpose_
+        self._op = ops[0] if ops else None
         if Ai.extra_dims != Ao.extra_dims:  # :99-103
             raise ArgumentError(_lib.PA_EINVAL,
                                 "incompatible number of extra dimensions of PencilArrays: "
                                 f"{Ai.extra_dims} != {Ao.extra_dims}")
-        if r2r is not None:
-            if r2r not in _R2R_KINDS:
+        row = _FUSED[self._op[:2]] if self._op else _FUSED[("unpack", "fft")]
+        kw = row.kw
+        if row.real == "both":
+            if self._op[2] not in _R2R_KINDS:
                 raise ArgumentError(_lib.PA_EINVAL,
-                                    f"r2r must be one of {sorted(_R2R_KINDS)}: got {r2r!r}")
-            if Ai.dtype != Ao.dtype or Ai.dtype not in _REAL_FLAGS:
-                raise ArgumentError(_lib.PA_EINVAL, "r2r: dest and src must be two float64 or two "
+                                    f"{kw} must be one of {sorted(_R2R_KINDS)}: got {self._op[2]!r}")
+            if Ai.dtype != Ao.dtype or Ai.dtype not in _REAL_DTYPES:
+                raise ArgumentError(_lib.PA_EINVAL, f"{kw}: dest and src must be two float64 or two "
                                     f"float32 arrays: got {Ao.dtype} and {Ai.dtype}")
-        elif self.rfft:
-            if (Ai.dtype, Ao.dtype) not in _BRFFT_PAIRS:
-                raise ArgumentError(_lib.PA_EINVAL, "rfft: src and dest must be float64 and "
-                                    "complex128, or float32 and complex64: got "
-                                    f"{Ai.dtype} and {Ao.dtype}")
-            Po = _rfft_pencil(Ao.pencil)  # the plan's output: the real y-pencil
-        elif self.rfft_first:
-            if (Ai.dtype, Ao.dtype) not in _BRFFT_PAIRS:
-                raise ArgumentError(_lib.PA_EINVAL, "rfft_first: src and dest must be float64 and "
-                                    "complex128, or float32 and complex64: got "
-                                    f"{Ai.dtype} and {Ao.dtype}")
-            Pi = _brfft_pencil(Ai.pencil)  # the plan's input: the complex counterpart of src
-        elif r2r_first is not None:
-            if r2r_first not in _R2R_KINDS:
-                raise ArgumentError(_lib.PA_EINVAL,
-                                    f"r2r_first must be one of {sorted(_R2R_KINDS)}: got {r2r_first!r}")
-            if Ai.dtype != Ao.dtype or Ai.dtype not in _REAL_FLAGS:
-                raise ArgumentError(_lib.PA_EINVAL, "r2r_first: dest and src must be two float64 or "
-                                    f"two float32 arrays: got {Ao.dtype} and {Ai.dtype}")
-        elif self.brfft_first:
-            if (Ao.dtype, Ai.dtype) not in _BRFFT_PAIRS:
-                raise ArgumentError(_lib.PA_EINVAL, "brfft_first: dest and src must be float64 and "
-                                    "complex128, or float32 and complex64: got "
-                                    f"{Ao.dtype} and {Ai.dtype}")
-            ax = as_tuple(Ai.pencil.perm, Ai.pencil.ndims)[0] - 1
-            # the plan's input: the real counterpart of src, N points as in dest
-            Pi = _real_pencil_of(Ai.pencil, Ao.pencil.size_global[ax])
-        elif self.brfft:
-            if (Ao.dtype, Ai.dtype) not in _BRFFT_PAIRS:
-                raise ArgumentError(_lib.PA_EINVAL, "brfft: dest and src must be float64 and "
-                                    "complex128, or float32 and complex64: got "
-                                    f"{Ao.dtype} and {Ai.dtype}")
-            Po = _brfft_pencil(Ao.pencil)  # the plan's output: the complex x-pencil
+        elif row.real:
+            real, cplx, names = (Ai, Ao, "src and dest") if row.real == "Ai" else (Ao, Ai, "dest and src")
+            if (real.dtype, cplx.dtype) not in _BRFFT_PAIRS:
+                raise ArgumentError(_lib.PA_EINVAL, f"{kw}: {names} must be float64 and complex128, "
+                                    f"or float32 and complex64: got {real.dtype} and {cplx.dtype}")
         elif Ai.dtype != Ao.dtype:  # PencilArray{T,N} for both arguments
             raise ArgumentError(_lib.PA_EINVAL, f"element types differ: {Ai.dtype} != {Ao.dtype}")
+        Pi, Po = row.pencils(Ai, Ao)
         if Pi.topology is not Po.topology:  # assert_compatible uses `!==` (:182-184)
             raise ArgumentError(_lib.PA_EINCOMPAT, "pencil topologies must be the same.")
         self.Pi, self.Po, self.Ai, self.Ao = Pi, Po, Ai, Ao
         self.method = method
-        # (rfft_first: the complex plan; brfft_first: the real plan)
-        elsize = Ao.elsize if (self.rfft_first or self.brfft_first) else Ai.elsize
+        elsize = (Ao if row.elsize == "Ao" else Ai).elsize
         self._plan = _get_plan(Pi, Po, Ai.extra_dims, elsize, method)  # remaining checks in C
         d = self._plan.info.dim
         self.dim = None if d == 0 else d  # :110
-        if self.rfft_first:
+        exchange = d != 0 and self._plan.info.nproc > 1
+        if self._op and self._op[0] == "put":
             # (the same verdict on every rank of the line: refused before the collective window setup)
-            check(lib.pa_plan_rfft_put_check(self._plan.h, _BRFFT_PAIRS[(Ai.dtype, Ao.dtype)]))
-        if r2r_first is not None or self.brfft_first:
-            # (likewise: one verdict for both, the same on every rank of the line)
-            check(lib.pa_plan_real_put_check(self._plan.h, _REAL_FLAGS[Ao.dtype]))
-        fused = "brfft" if self.brfft else "rfft" if self.rfft else "r2r" if r2r is not None else None
-        if fused and d != 0 and self._plan.info.nproc > 1 and isinstance(method, (PeerPut, PeerGet)):
+            check(getattr(lib, row.verdict)(self._plan.h, self._precision()))
+        elif self._op and exchange and isinstance(method, (PeerPut, PeerGet)):
             # (the same on every rank of the line: refused before the collective window setup)
-            raise ArgumentError(_lib.PA_EINVAL, f"{fused}: the one-sided methods have no unpack "
+            raise ArgumentError(_lib.PA_EINVAL, f"{kw}: the one-sided methods have no unpack "
                                 "pass to fuse with; use PointToPoint / Alltoallv")
-        if d != 0 and self._plan.info.nproc > 1 and Pi.topology.comm.handle is not None:
+        if exchange and Pi.topology.comm.handle is not None:
             comm = Pi.topology.comm
             if isinstance(method, PeerPut):
                 _register_window(self._plan, Ao, Ai, comm)
@@ -424,6 +450,29 @@ class Transposition:
                 _register_window(self._plan, Ai, Ao, comm)
             else:
                 _register_arenas(self._plan, Po, comm)
+
+    def _is(self, side, mode):
+        return self._op is not None and self._op[:2] == (side, mode)
+
+    brfft = property(lambda self: self._is("unpack", "brfft"))
+    r2r = property(lambda self: self._op[2] if self._is("unpack", "r2r") else None)
+    rfft = property(lambda self: self._is("unpack", "rfft"))
+    rfft_first = property(lambda self: self._is("put", "rfft"))
+    r2r_first = property(lambda self: self._op[2] if self._is("put", "r2r") else None)
+    brfft_first = property(lambda self: self._is("put", "brfft"))
+
+    def _precision(self) -> int:
+        """PA_FFT_F32 for single precision: a plan only knows its element size, and 8 bytes is
+        float64 as well as complex64.  A complex transposition is single precision for complex64
+        arrays only."""
+        single = (torch.complex64,) if self._op is None else (torch.float32, torch.complex64)
+        return _lib.PA_FFT_F32 if self.Ai.dtype in single else 0
+
+    def _fusable(self, side) -> bool:
+        op = self._op or (side, "fft")
+        if op[0] != side:
+            return False
+        return getattr(lib, _FUSED[op[:2]].verdict)(self._plan.h, self._precision()) == _lib.PA_OK
 
     @property
     def plan(self) -> _Plan:
@@ -449,14 +498,7 @@ class Transposition:
         ``pa_transpose_rfft`` can (``pa_plan_real_check``, one answer for both); for an
         ``rfft_first=True`` (``r2r_first=``, ``brfft_first=True``) one: False (see
         :meth:`fft_first_fusable`)."""
-        if self.rfft_first or self.r2r_first is not None or self.brfft_first:
-            return False
-        if self.r2r is not None or self.rfft:
-            return lib.pa_plan_real_check(self._plan.h, _REAL_FLAGS[self.Ai.dtype]) == _lib.PA_OK
-        if self.brfft:
-            return lib.pa_plan_brfft_check(self._plan.h, _fft_precision_flag(self.Ai)) == _lib.PA_OK
-        return lib.pa_plan_fft_check_ex(self._plan.h, _fft_precision_flag(self.Ai)) == _lib.PA_OK
-
+        return self._fusable("unpack")
 
     def fft_first_fusable(self) -> bool:
         """Whether the send-side fused kernel can run on this transposition: for a complex one
@@ -465,20 +507,7 @@ class Transposition:
         ``brfft_first=True`` one ``transpose_(self)`` (``pa_plan_real_put_check``).  Needs ``PeerPut``
         when the transposition exchanges data; the answer is the same on every rank of the grid
         line."""
-        if self.r2r_first is not None or self.brfft_first:
-            return lib.pa_plan_real_put_check(self._plan.h, _REAL_FLAGS[self.Ao.dtype]) == _lib.PA_OK
-        if self.rfft_first:
-            flag = _BRFFT_PAIRS[(self.Ai.dtype, self.Ao.dtype)]
-            return lib.pa_plan_rfft_put_check(self._plan.h, flag) == _lib.PA_OK
-        if self.brfft or self.rfft or self.r2r is not None:
-            return False
-        return lib.pa_plan_fft_put_check(self._plan.h, _fft_precision_flag(self.Ai)) == _lib.PA_OK
-
-
-def _fft_precision_flag(u: PencilArray) -> int:
-    """PA_FFT_F32 for complex64 arrays: a plan only knows its element size, and 8 bytes is
-    float64 as well as complex64."""
-    return _lib.PA_FFT_F32 if u.dtype == torch.complex64 else 0
+        return self._fusable("put")
 
 
 def Waitall(t: Transposition):
@@ -521,78 +550,39 @@ def transpose_(*args, method=None, waitall=True, overlap=True, stage_self=False,
         raise TypeError("transpose_(dest, src; method) or transpose_(t; waitall)")
     flags = (_lib.PA_WAITALL if waitall else 0) | (0 if overlap else _lib.PA_NO_OVERLAP) | (
         _lib.PA_STAGE_SELF if stage_self else 0)
-    if t.rfft_first:
-        if fft is not None or fft_first is not None:
-            raise ArgumentError(_lib.PA_EINVAL, "an rfft_first transposition implies its transform: "
-                                "transpose_(t) without fft= / fft_first=")
-        check(lib.pa_rfft_put(t.plan.h, t.Pi.topology.comm.handle, t.Ai.pencil._h,
-                              C.c_void_p(t.Ai.data_ptr() or None), C.c_void_p(t.Ao.data_ptr() or None),
-                              flags | _BRFFT_PAIRS[(t.Ai.dtype, t.Ao.dtype)], _stream_ptr()))
-        return t if len(args) == 1 else args[0]
-    if t.r2r_first is not None or t.brfft_first:
-        what = "an r2r_first" if t.r2r_first is not None else "a brfft_first"
-        if fft is not None or fft_first is not None:
-            raise ArgumentError(_lib.PA_EINVAL, f"{what} transposition implies its transform: "
-                                "transpose_(t) without fft= / fft_first=")
-        comm = t.Pi.topology.comm.handle
-        src, dst = C.c_void_p(t.Ai.data_ptr() or None), C.c_void_p(t.Ao.data_ptr() or None)
-        flags |= _REAL_FLAGS[t.Ao.dtype]
-        if t.brfft_first:
-            check(lib.pa_brfft_put(t.plan.h, comm, t.Ai.pencil._h, src, dst, flags, _stream_ptr()))
-        else:
-            check(lib.pa_r2r_put(t.plan.h, comm, _R2R_KINDS[t.r2r_first], src, dst, flags, _stream_ptr()))
-        return t if len(args) == 1 else args[0]
-    if fft_first is not None and (t.brfft or t.rfft or t.r2r is not None):
-        raise ArgumentError(_lib.PA_EINVAL, "fft_first= applies to complex transpositions only")
-    if t.brfft:
-        if fft is not None:
-            raise ArgumentError(_lib.PA_EINVAL, "a brfft transposition implies its transform: "
-                                "transpose_(t) without fft=")
-        check(lib.pa_transpose_brfft(t.plan.h, t.Pi.topology.comm.handle, t.Ao.pencil._h,
-                                     C.c_void_p(t.Ai.data_ptr() or None),
-                                     C.c_void_p(t.Ao.data_ptr() or None),
-                                     flags | _fft_precision_flag(t.Ai), _stream_ptr()))
-        return t if len(args) == 1 else args[0]
-    if t.r2r is not None or t.rfft:
-        what = "an rfft" if t.rfft else "an r2r"
-        if fft is not None:
-            raise ArgumentError(_lib.PA_EINVAL, f"{what} transposition implies its transform: "
-                                "transpose_(t) without fft=")
-        comm = t.Pi.topology.comm.handle
-        src, dst = C.c_void_p(t.Ai.data_ptr() or None), C.c_void_p(t.Ao.data_ptr() or None)
-        flags |= _REAL_FLAGS[t.Ai.dtype]
-        if t.rfft:
-            check(lib.pa_transpose_rfft(t.plan.h, comm, t.Ao.pencil._h, src, dst, flags, _stream_ptr()))
-        else:
-            check(lib.pa_transpose_r2r(t.plan.h, comm, _R2R_KINDS[t.r2r], src, dst, flags,
-                                       _stream_ptr()))
-        return t if len(args) == 1 else args[0]
-    if fft_first is not None:
+    op = t._op
+    if op is not None:
+        kw = _FUSED[op[:2]].kw
+        if op[0] == "put":
+            if fft is not None or fft_first is not None:
+                raise ArgumentError(_lib.PA_EINVAL, f"{_article(kw)} {kw} transposition implies its "
+                                    "transform: transpose_(t) without fft= / fft_first=")
+        elif fft_first is not None:
+            raise ArgumentError(_lib.PA_EINVAL, "fft_first= applies to complex transpositions only")
+        elif fft is not None:
+            raise ArgumentError(_lib.PA_EINVAL, f"{_article(kw)} {kw} transposition implies its "
+                                "transform: transpose_(t) without fft=")
+    elif fft_first is not None:
         if fft is not None:
             raise ArgumentError(_lib.PA_EINVAL, "fft= and fft_first= exclude each other")
-        if fft_first in ("forward", -1):
-            flags |= _lib.PA_FFT_FORWARD
-        elif fft_first in ("backward", 1):
-            flags |= _lib.PA_FFT_BACKWARD
-        else:
-            raise ArgumentError(_lib.PA_EINVAL, "fft_first must be 'forward' or 'backward'")
-        check(lib.pa_fft_put(t.plan.h, t.Pi.topology.comm.handle, C.c_void_p(t.Ai.data_ptr() or None),
-                             C.c_void_p(t.Ao.data_ptr() or None), flags | _fft_precision_flag(t.Ai),
-                             _stream_ptr()))
-        return t if len(args) == 1 else args[0]
-    if fft is not None:
-        if fft in ("forward", -1):
-            flags |= _lib.PA_FFT_FORWARD
-        elif fft in ("backward", 1):
-            flags |= _lib.PA_FFT_BACKWARD
-        else:
-            raise ArgumentError(_lib.PA_EINVAL, "fft must be 'forward' or 'backward'")
-        flags |= _fft_precision_flag(t.Ai)
-    comm = t.Pi.topology.comm.handle
+        op, flags = ("put", "fft"), flags | _direction("fft_first", fft_first)
+    elif fft is not None:
+        op, flags = ("unpack", "fft"), flags | _direction("fft", fft)
+    if op is not None:
+        flags |= t._precision()
+    row = _FUSED[op[:2]] if op else _FUSED[("unpack", "fft")]
     # (an empty local array may have a null data pointer: the library accepts that)
-    check(lib.pa_transpose(t.plan.h, comm, C.c_void_p(t.Ai.data_ptr() or None),
-                           C.c_void_p(t.Ao.data_ptr() or None), flags, _stream_ptr()))
+    check(row.call(t, t.Pi.topology.comm.handle, C.c_void_p(t.Ai.data_ptr() or None),
+                   C.c_void_p(t.Ao.data_ptr() or None), flags, _stream_ptr()))
     return t if len(args) == 1 else args[0]
+
+
+def _direction(kw: str, value) -> int:
+    if value in ("forward", -1):
+        return _lib.PA_FFT_FORWARD
+    if value in ("backward", 1):
+        return _lib.PA_FFT_BACKWARD
+    raise ArgumentError(_lib.PA_EINVAL, f"{kw} must be 'forward' or 'backward'")
 
 
 transpose_bang = transpose_
