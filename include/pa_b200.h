@@ -595,6 +595,33 @@ pa_status pa_reduce(const pa_pencil* pencil, int n_extra, const int64_t* extra_d
  * combinations pa_reduce refuses.  Host-only.                                                  */
 pa_status pa_reduce_result_type(int dtype, int map, int op, int* result_dtype);
 
+/* mapreduce(f, op, u[, v]; dims): the reduction of pa_reduce (same maps, ops, predicates, result
+ * types and rules) over the logical dims `dims` only (n_dims of them, 1-based: 1..N the pencil's
+ * spatial dims, N+1..N+n_extra its extra dims; any order; no duplicates).  Each rank gets, at
+ * `result`, a dense array laid out like its parent array (memory order, extra dims last) with extent
+ * 1 along every reduced dim and its local extent along every kept dim: entry I holds the reduction
+ * over the GLOBAL ranges of the reduced dims at this rank's global index I of the kept dims.  A rank
+ * combines with the ranks whose grid coordinates agree with its own on every grid dim that
+ * decomposes a kept dim, folding their partials in rank order; every member gets the same bits.
+ * `dims` covering every dim is pa_reduce.  ONE kernel per rank and call (DESIGN §3l), ordered on
+ * `stream`, collective over the communicator (ranks with an empty array or result take part), the
+ * host is not synchronised.  Refused with PA_EINVAL, checked in this order (error texts start with
+ * "pa_reduce_dims:"): a NULL pencil; an invalid (dtype, map, op) as pa_reduce_result_type decides
+ * it; bad extra dims; bad `dims` (none, NULL, out of 1..N+n_extra, or one given twice); then
+ * pa_reduce's array checks in its order -- `b` given or missing, NULL arrays for a non-empty local
+ * array, alignment, `result` (which may be NULL when the local result is empty), a comparison
+ * without pred_value --; max / min over a globally empty reduced range (a sum gives zeros); with
+ * more than one rank, a local result larger than the flag window's partial area (524288 elements
+ * on the rank with the most), decided from the global geometry.  PA_EINCOMPAT: the topology and the
+ * communicator disagree on the rank count, as in pa_reduce.  Then without a device PA_ENOGPU.
+ * PA_ESTATE: more than one rank on a communicator without a flag window (NCCL alone, or the
+ * nccl_fences tunable).
+ * pa_reduce and pa_reduce_dims on one communicator share one serialisation, in issue order.      */
+pa_status pa_reduce_dims(const pa_pencil* pencil, int n_extra, const int64_t* extra_dims,
+                         pa_comm* comm, int dtype, int map, int op, const void* pred_value,
+                         const void* a, const void* b, int n_dims, const int* dims, void* result,
+                         void* stream);
+
 /* ---- host chains -----------------------------------------------------------
  * A sequence of transpositions applied to HOST arrays (plan i+1 consumes what
  * plan i produces): one submit = upload of `host_src`, every transpose! on the

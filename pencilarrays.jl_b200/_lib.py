@@ -169,6 +169,8 @@ SIGNATURES = {
     "pa_io_read": (C.c_int, [_P, C.c_int, _I64P, C.c_int, C.c_int, _P, C.c_char_p, C.c_int64]),
     "pa_reduce": (C.c_int, [_P, C.c_int, _I64P, _P, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P]),
     "pa_reduce_result_type": (C.c_int, [C.c_int, C.c_int, C.c_int, _IP]),
+    "pa_reduce_dims": (C.c_int, [_P, C.c_int, _I64P, _P, C.c_int, C.c_int, C.c_int, _P, _P, _P,
+                                 C.c_int, _IP, _P, _P]),
     "pa_plan_timings": (C.c_int, [_P, C.POINTER(Timings)]),
     "pa_plan_enable_timing": (C.c_int, [_P, C.c_int]),
 }

@@ -1327,18 +1327,79 @@ static int component_bytes(int dtype) {  // the alignment an array of dtype need
   return dtype == PA_COMPLEXF64 ? 8 : dtype == PA_COMPLEXF32 ? 4 : elem_bytes(dtype);
 }
 
-// Every check in the order of pa_b200.h, on the host before any device call.
+// pa_reduce_dims: `dims` checked (1-based logical dims, extra dims N+1..) and turned into the
+// local geometry; *nout = the local result's elements, *nred_global = the reduced dims' global
+// element count, *nout_max = the largest local result over every rank of the grid
+static pa_status dims_geom(const Pencil& Pn, int n_extra, const int64_t* extra_dims, int n_dims,
+                           const int* dims, DimsGeom* g, i64* nout, i64* nred_global, i64* nout_max) {
+  const int nl = Pn.N + n_extra;
+  if (n_dims < 1 || !dims) {
+    set_error("pa_reduce_dims: `dims` must name at least one dim");
+    return PA_EINVAL;
+  }
+  bool red_logical[PA_MAX_DIMS] = {false};
+  for (int i = 0; i < n_dims; ++i) {
+    if (dims[i] < 1 || dims[i] > nl) {
+      set_error("pa_reduce_dims: dim %d out of range 1..%d (%d spatial dims, then %d extra)",
+                dims[i], nl, Pn.N, n_extra);
+      return PA_EINVAL;
+    }
+    if (red_logical[dims[i] - 1]) {
+      set_error("pa_reduce_dims: dim %d given twice", dims[i]);
+      return PA_EINVAL;
+    }
+    red_logical[dims[i] - 1] = true;
+  }
+  i64 lo[PA_MAX_DIMS], hi[PA_MAX_DIMS];
+  Pn.range_local(lo, hi);
+  g->nd = nl;
+  *nout = 1;
+  *nred_global = 1;
+  for (int i = 0; i < nl; ++i) {
+    const int l = i < Pn.N ? Pn.perm[i] : i;  // memory dim i holds logical dim l
+    g->red[i] = red_logical[l];
+    g->ext[i] = l < Pn.N ? hi[l] - lo[l] : extra_dims[l - Pn.N];
+    if (g->red[i]) *nred_global *= l < Pn.N ? Pn.size_global[l] : extra_dims[l - Pn.N];
+    else *nout *= g->ext[i];
+  }
+  const Topology& T = *Pn.topo;
+  g->topo_M = T.M;
+  for (int i = 0; i < T.M; ++i) {
+    g->topo_dims[i] = T.dims[i];
+    g->coords[i] = T.coords[i];
+    if (!red_logical[Pn.decomp[i]]) g->keep_grid |= 1u << i;
+  }
+  // (the capacity refusal must come out the same on every rank: the largest local result)
+  *nout_max = 0;
+  for (int r = 0; r < T.size; ++r) {
+    i64 c[PA_MAX_TOPO], rlo[PA_MAX_DIMS], rhi[PA_MAX_DIMS], k = 1;
+    T.coords_of(r, c);
+    Pn.range_of(c, rlo, rhi);
+    for (int l = 0; l < nl; ++l)
+      if (!red_logical[l]) k *= l < Pn.N ? rhi[l] - rlo[l] : extra_dims[l - Pn.N];
+    *nout_max = std::max(*nout_max, k);
+  }
+  return PA_OK;
+}
+
+// Every check in the order of pa_b200.h, on the host before any device call.  dims (n_dims > 0):
+// pa_reduce_dims' checks as well, its geometry into *geo
 static pa_status reduce_checks(const pa_pencil* pencil, int n_extra, const int64_t* extra_dims,
                                pa_comm* comm, int dtype, int map, int op, const void* pred_value,
-                               const void* a, const void* b, void* result, i64* n_local) {
-  const char* who = "pa_reduce";
+                               const void* a, const void* b, void* result, i64* n_local,
+                               int n_dims = 0, const int* dims = nullptr, DimsGeom* geo = nullptr) {
+  const char* who = geo ? "pa_reduce_dims" : "pa_reduce";
   if (!pencil) {
     set_error("%s: null pencil", who);
     return PA_EINVAL;
   }
   int rt = 0;
-  pa_status s = pa_reduce_result_type(dtype, map, op, &rt);
-  if (s != PA_OK) return s;
+  const char* why = "";
+  rt = red::result_dtype(dtype, map, op, &why);
+  if (rt < 0) {
+    set_error("%s: dtype %d, map %d, op %d: %s", who, dtype, map, op, why);
+    return PA_EINVAL;
+  }
   const Pencil& Pn = *pencil->p;
   if (n_extra < 0 || (n_extra > 0 && !extra_dims) || Pn.N + n_extra > PA_MAX_DIMS) {
     set_error("%s: %d extra dims on a %d-d pencil (at most %d dims in all)", who, n_extra, Pn.N,
@@ -1360,6 +1421,8 @@ static pa_status reduce_checks(const pa_pencil* pencil, int n_extra, const int64
     n *= extra_dims[i];
     nglobal *= extra_dims[i];
   }
+  i64 nout = 1, nred_global = nglobal, nout_max = 1;
+  if (geo) RC(dims_geom(Pn, n_extra, extra_dims, n_dims, dims, geo, &nout, &nred_global, &nout_max));
   if (map == PA_MAP_DOT ? (n > 0 && !b) : b != nullptr) {
     set_error(map == PA_MAP_DOT ? "%s: PA_MAP_DOT reduces two arrays: `b` is missing"
                                 : "%s: a second array `b` goes with PA_MAP_DOT only", who);
@@ -1376,7 +1439,7 @@ static pa_status reduce_checks(const pa_pencil* pencil, int n_extra, const int64
   }
   // (the kernels store the result whole: 16-byte stores for ComplexF64, 8-byte for ComplexF32)
   const uintptr_t ral = (uintptr_t)elem_bytes(rt);
-  if (!result || (uintptr_t)result % ral) {
+  if ((!result && nout > 0) || (uintptr_t)result % ral) {  // (an empty local result: may be NULL)
     set_error("%s: `result` must be a device pointer aligned to %d bytes", who, (int)ral);
     return PA_EINVAL;
   }
@@ -1386,12 +1449,18 @@ static pa_status reduce_checks(const pa_pencil* pencil, int n_extra, const int64
     return PA_EINVAL;
   }
   const int base = op & 15;
-  if (nglobal == 0 && (base == PA_OP_MAX || base == PA_OP_MIN)) {
+  if (nred_global == 0 && (base == PA_OP_MAX || base == PA_OP_MIN)) {
     set_error("%s: reducing over an empty collection is not allowed (maximum / minimum of an "
               "empty array)", who);
     return PA_EINVAL;
   }
   const int nranks = Pn.topo->size;
+  if (geo && nranks > 1 && nout_max * REDUCE_SLOT_BYTES > (i64)REDUCE_AREA_BYTES) {
+    set_error("%s: a rank's partial result of %lld elements exceeds the flag window's partial area "
+              "(%lld 16-byte accumulators)", who, (long long)nout_max,
+              (long long)(REDUCE_AREA_BYTES / REDUCE_SLOT_BYTES));
+    return PA_EINVAL;
+  }
   if (comm ? comm_size(comm->p) != nranks : nranks > 1) {
     set_error(comm ? "%s: the topology has %d ranks, the communicator %d"
                    : "%s: a topology of %d ranks needs a communicator", who, nranks,
@@ -1413,6 +1482,27 @@ pa_status pa_reduce(const pa_pencil* pencil, int n_extra, const int64_t* extra_d
     s = need_gpu();
     if (s != PA_OK) return s;
     return reduce(comm ? comm->p : nullptr, dtype, map, op, pred_value, n, a, b, result, stream);
+  })
+}
+
+pa_status pa_reduce_dims(const pa_pencil* pencil, int n_extra, const int64_t* extra_dims,
+                         pa_comm* comm, int dtype, int map, int op, const void* pred_value,
+                         const void* a, const void* b, int n_dims, const int* dims, void* result,
+                         void* stream) {
+  GUARD({
+    i64 n = 0;
+    DimsGeom geo;
+    pa_status s = reduce_checks(pencil, n_extra, extra_dims, comm, dtype, map, op, pred_value, a, b,
+                                result, &n, n_dims, dims, &geo);
+    if (s != PA_OK) return s;
+    s = need_gpu();
+    if (s != PA_OK) return s;
+    bool every = true;
+    for (int i = 0; i < geo.nd; ++i) every = every && geo.red[i];
+    if (every)  // one element: pa_reduce's
+      return reduce(comm ? comm->p : nullptr, dtype, map, op, pred_value, n, a, b, result, stream);
+    return reduce_dims(comm ? comm->p : nullptr, dtype, map, op, pred_value, geo, a, b, result,
+                       stream);
   })
 }
 

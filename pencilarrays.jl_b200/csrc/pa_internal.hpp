@@ -255,6 +255,9 @@ pa_status comm_flags_import(Comm* c, int rank, const void* handle64, i64 offset)
 // words of kind FK_REDUCE and, behind all the words, two sets (the parity of the call) of one
 // 16-byte slot per source rank.
 constexpr int REDUCE_SLOT_BYTES = 16;
+// pa_reduce_dims: behind the slots, two sets (the parity of the call) of this rank's own partial
+// area, one 16-byte accumulator per local output element; group members read it in place
+constexpr size_t REDUCE_AREA_BYTES = 8u << 20;
 struct ReduceState;  // workspace + serialising event of the reductions on one communicator
 struct ReduceWindow {
   int nranks = 1, rank = 0;
@@ -272,14 +275,32 @@ int comm_size(const Comm* c);
 // ncclAllGather of `bytes` per rank (the reductions' fallback without a flag window)
 pa_status comm_allgather(Comm* c, const void* send, void* recv, size_t bytes, void* stream);
 // a communicator's reduction state, made with the communicator (synchronous); its window tables
-// uploaded once the flag window is mapped everywhere
+// uploaded once the flag window is mapped everywhere.  areas[r]: rank r's partial area as mapped
+// here (areas[rank]: the local one)
 pa_status reduce_state_create(int nranks, ReduceState** out);
 pa_status reduce_state_set_tables(ReduceState* s, int nranks, unsigned long long* const* remote_words,
-                                  unsigned char* const* peer_slots);
+                                  unsigned char* const* peer_slots, unsigned char* const* areas);
 void reduce_state_destroy(ReduceState* s);
 // the reduction itself (reduce.cu); every argument has been checked.  comm NULL: one rank
 pa_status reduce(Comm* comm, int dtype, int map, int op, const void* pred_value, i64 n,
                  const void* a, const void* b, void* result, void* stream);
+
+// pa_reduce_dims' local geometry, checked by capi.cpp: the parent's dims in memory order (extra
+// dims last) with their local extents and whether each is reduced, and the grid: a rank combines
+// with the ranks whose coordinates agree with its own on every grid dim in keep_grid (the grid
+// dims that decompose a kept dim)
+struct DimsGeom {
+  int nd = 0;
+  i64 ext[PA_MAX_DIMS] = {0};
+  bool red[PA_MAX_DIMS] = {false};
+  int topo_M = 0;
+  i64 topo_dims[PA_MAX_TOPO] = {0};
+  i64 coords[PA_MAX_TOPO] = {0};
+  unsigned keep_grid = 0;
+};
+// the reduction along dims (reduce.cu); every argument has been checked
+pa_status reduce_dims(Comm* comm, int dtype, int map, int op, const void* pred_value,
+                      const DimsGeom& geo, const void* a, const void* b, void* result, void* stream);
 
 // What a fused line kernel computes: from the lines it gathers on the receive side of a
 // transposition (unpack_fused, get_fft) or from the source lines it loads on the send side

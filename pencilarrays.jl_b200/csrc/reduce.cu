@@ -235,6 +235,265 @@ __global__ void __launch_bounds__(RT, R_CTAS_PER_SM) k_reduce(const RArgs g) {
   *(typename Rd::R*)g.result = Rd::finish(acc);
 }
 
+// ---- reductions along dims (pa_reduce_dims, DESIGN §3l) -----------------------------------------
+// The local parent's dims (memory order, extra dims last), extent-1 dims dropped and neighbours of
+// the same class merged, are kept (K) and reduced (R) runs.  Output o (column-major over the K
+// runs, which is the result's layout) folds the elements koff(o) + roff(r) + i: r over the "rows"
+// (the outer R runs, an odometer), i over the inner run -- the fastest run when it is reduced and
+// long enough (the row regime: contiguous, 16-byte units when aligned), else length 1 (the column
+// regime: consecutive threads own consecutive outputs).  A team of Wi x Wr threads folds one
+// output: Wi lanes interleaved along each row's units, Wr contiguous blocks of rows; the CTA holds
+// Oc teams (Wi * Wr * Oc = RT).  With few outputs the rows x units of each output tile are split
+// over S = Sr x Si CTAs; their partials go to the workspace and the tile's last CTA (ticket) folds
+// them.  With P > 1 each tile's rank partials go to this rank's own area of the flag window, and the
+// last tile to finish (a second ticket) runs the combine.
+constexpr int D_RUNS = PA_MAX_DIMS / 2;  // K runs and R runs alternate: at most 4 of each
+// resident CTAs per SM the kernel is compiled for: 3 (at most 85 registers); 4 (64 registers)
+// spills 24-224 bytes per thread in every instantiation
+constexpr int D_CTAS_PER_SM = 3;
+
+struct DArgs {
+  const void* a;
+  const void* b;
+  i64 nout;                        // local outputs
+  int nk, nr;                      // K runs; outer R runs (the rows' odometer)
+  i64 ke[D_RUNS], ks[D_RUNS];      // extents and element strides, fastest first
+  i64 re[D_RUNS], rs[D_RUNS];
+  i64 nrows;                       // product of re (0: the reduced range is empty)
+  i64 lu;                          // units per row (16-byte units when vec, else elements)
+  int vec;
+  int Wi, Wr, Oc;
+  int S, Sr;                       // splits per tile (S = Sr * Si): Sr along rows, Si along units
+  i64 rchunk, uchunk;              // rows / units per split
+  i64 tiles;                       // output tiles (at least 1)
+  int pred;
+  alignas(16) unsigned char ref[16];
+  unsigned* tickets;               // [tiles] when S > 1, then the all-tiles ticket
+  unsigned char* part;             // [tiles][S][Oc] 16-byte partials
+  int nranks, rank;
+  ull seq;
+  ull* local_words;
+  int word_stride;
+  ull* const* remote_words;        // device table [nranks]
+  unsigned char* const* areas;     // device table [nranks]: every rank's partial area as mapped here
+  size_t area_off;                 // the parity set's offset in an area
+  int topo_M;                      // the combine group: the ranks whose coordinates agree with
+  int topo_dims[PA_MAX_TOPO];      //   mine on every grid dim of keep_grid
+  int coords[PA_MAX_TOPO];
+  unsigned keep_grid;
+  ull timeout_ns;
+  int* err;
+  void* result;
+};
+
+__device__ __forceinline__ bool in_group(const DArgs& g, int q) {
+  for (int i = g.topo_M - 1; i >= 0; --i) {  // row-major rank numbering: the last coordinate fastest
+    const int c = q % g.topo_dims[i];
+    q /= g.topo_dims[i];
+    if (((g.keep_grid >> i) & 1) && c != g.coords[i]) return false;
+  }
+  return true;
+}
+
+// tree over the W members of each team (sh[t] holds member t's value): member m takes m + h for
+// h = W/2 .. 1; the team's value ends in member 0.  Every thread of the CTA calls it.
+template <class Rd>
+__device__ __forceinline__ typename Rd::A team_reduce(typename Rd::A v, typename Rd::A* sh,
+                                                      const DArgs& g, int m, int oc) {
+  const int W = g.Wi * g.Wr;
+  auto tid = [&](int mm) { return ((mm / g.Wi) * g.Oc + oc) * g.Wi + mm % g.Wi; };
+  __syncthreads();  // (sh may still be read from an earlier tree)
+  sh[threadIdx.x] = v;
+  __syncthreads();
+  for (int h = W / 2; h > 0; h >>= 1) {
+    if (m < h) sh[threadIdx.x] = Rd::comb(sh[threadIdx.x], sh[tid(m + h)]);
+    __syncthreads();
+  }
+  return sh[tid(0)];
+}
+
+template <class E, int M, int O>
+__global__ void __launch_bounds__(RT, D_CTAS_PER_SM) k_reduce_dims(const DArgs g) {
+  using Rd = Red<E, M, O>;
+  using T = typename Rd::T;
+  using A = typename Rd::A;
+  constexpr int V = 16 / sizeof(E);
+  __shared__ A sh[RT];
+  __shared__ int last;
+  const E* a = (const E*)g.a;
+  const E* b = M == M_DOT ? (const E*)g.b : a;
+  T ref;
+  memcpy(&ref, g.ref, sizeof(T));
+  const int t = threadIdx.x;
+  const int wi = t % g.Wi, oc = (t / g.Wi) % g.Oc, wr = t / (g.Wi * g.Oc);
+  const int m = wr * g.Wi + wi, W = g.Wi * g.Wr;
+  const i64 tile = blockIdx.x / g.S;
+  const int s = blockIdx.x % g.S;
+  const i64 o = tile * g.Oc + oc;
+  const int vx = g.vec ? V : 1;
+
+  A acc = Rd::neutral();
+  if (o < g.nout) {
+    i64 koff = 0, q = o;
+#pragma unroll
+    for (int k = 0; k < D_RUNS; ++k)
+      if (k < g.nk) {
+        koff += (q % g.ke[k]) * g.ks[k];
+        q /= g.ke[k];
+      }
+    const int sr = s % g.Sr, si = s / g.Sr;
+    const i64 R0 = (i64)sr * g.rchunk, R1 = min(g.nrows, R0 + g.rchunk);
+    const i64 nb = R1 > R0 ? (R1 - R0 + g.Wr - 1) / g.Wr : 0;
+    i64 r = R0 + wr * nb;
+    const i64 rend = min(R1, r + nb);
+    const i64 U0 = (i64)si * g.uchunk, U1 = min(g.lu, U0 + g.uchunk);
+    i64 u = U0 + wi;
+    if (r < rend && u < U1) {
+      i64 c[D_RUNS], roff = 0, rq = r;
+#pragma unroll
+      for (int k = 0; k < D_RUNS; ++k)
+        if (k < g.nr) {
+          c[k] = rq % g.re[k];
+          roff += c[k] * g.rs[k];
+          rq /= g.re[k];
+        }
+      const E* pa0 = a + koff;
+      const E* pb0 = b + koff;
+      bool more = true;
+      while (more) {
+        E xa[RU][V], xb[RU][V];
+        i64 off[RU];
+        int nin = 0;
+#pragma unroll
+        for (int k = 0; k < RU; ++k) {
+          if (!more) break;
+          off[k] = roff + u * vx;
+          nin = k + 1;
+          u += g.Wi;  // next item: the next unit of the row, else the next row (odometer)
+          if (u >= U1) {
+            u = U0 + wi;
+            if (++r >= rend) {
+              more = false;
+            } else {
+#pragma unroll
+              for (int j = 0; j < D_RUNS; ++j)
+                if (j < g.nr) {
+                  roff += g.rs[j];
+                  if (++c[j] < g.re[j]) break;
+                  roff -= g.re[j] * g.rs[j];
+                  c[j] = 0;
+                }
+            }
+          }
+        }
+#pragma unroll
+        for (int k = 0; k < RU; ++k)
+          if (k < nin) {
+            if (g.vec) {
+              ld_unit(pa0 + off[k], true, xa[k]);
+              if (M == M_DOT) ld_unit(pb0 + off[k], true, xb[k]);
+            } else {
+              xa[k][0] = ld1(pa0 + off[k]);
+              if (M == M_DOT) xb[k][0] = ld1(pb0 + off[k]);
+            }
+          }
+#pragma unroll
+        for (int k = 0; k < RU; ++k)
+          if (k < nin) {
+#pragma unroll
+            for (int j = 0; j < V; ++j)
+              if (j < vx) acc = Rd::comb(acc, Rd::elem(xa[k][j], M == M_DOT ? xb[k][j] : xa[k][j], ref, g.pred));
+          }
+      }
+    }
+  }
+  acc = team_reduce<Rd>(acc, sh, g, m, oc);
+
+  if (g.S > 1) {  // the tile's last CTA folds its S partials (members take s = m, m + W, ...)
+    unsigned char* part = g.part + (size_t)tile * g.S * g.Oc * 16;
+    if (m == 0 && o < g.nout) {
+      st16(part + ((size_t)s * g.Oc + oc) * 16, acc);
+      __threadfence();
+    }
+    __syncthreads();
+    if (t == 0) last = atomicAdd(g.tickets + tile, 1u) == (unsigned)g.S - 1;
+    __syncthreads();
+    if (!last) return;
+    __threadfence();
+    acc = Rd::neutral();
+    if (o < g.nout)
+      for (int i = m; i < g.S; i += W) acc = Rd::comb(acc, ld16_cg<A>(part + ((size_t)i * g.Oc + oc) * 16));
+    acc = team_reduce<Rd>(acc, sh, g, m, oc);
+    if (t == 0) g.tickets[tile] = 0;  // the next call (ordered after this one) starts from zero
+  }
+
+  typename Rd::R* res = (typename Rd::R*)g.result;
+  if (g.nranks == 1) {
+    if (m == 0 && o < g.nout) res[o] = Rd::finish(acc);
+    return;
+  }
+  // P > 1: the tile's rank partials into my own area; the last tile runs the combine
+  const int P = g.nranks, me = g.rank;
+  if (m == 0 && o < g.nout) {
+    st16(g.areas[me] + g.area_off + (size_t)o * 16, acc);
+    __threadfence_system();
+  }
+  __syncthreads();
+  unsigned* all = g.tickets + (g.S > 1 ? g.tiles : 0);
+  if (t == 0) last = atomicAdd(all, 1u) == (unsigned)(g.tiles - 1);
+  __syncthreads();
+  if (!last) return;
+  __threadfence_system();
+  if (t == 0) {
+    *all = 0;
+    for (int k = 1; k < P; ++k) flag_signal(g.remote_words[(me + k) % P], g.seq);
+    for (int k = 1; k < P; ++k) {  // every peer, not only the group: see DESIGN §3l
+      const int q = (me + P - k) % P;
+      flag_wait(g.local_words + (size_t)q * g.word_stride, g.seq, g.timeout_ns, g.err);
+    }
+  }
+  // the group's areas, in rank order, listed once per call (up to RT members in shared memory)
+  __shared__ const unsigned char* grp[RT];
+  __shared__ int ng;
+  if (t == 0) {
+    int n = 0;
+    for (int q = 0; q < P; ++q)
+      if (in_group(g, q)) {
+        if (n < RT) grp[n] = g.areas[q] + g.area_off;
+        ++n;
+      }
+    ng = n;
+  }
+  __syncthreads();
+  if (ng > RT) {  // (a group of more than RT ranks: test membership per rank)
+    for (i64 oo = t; oo < g.nout; oo += RT) {
+      A v = Rd::neutral();
+      for (int q = 0; q < P; ++q)
+        if (in_group(g, q)) v = Rd::comb(v, ld16_cv<A>(g.areas[q] + g.area_off + (size_t)oo * 16));
+      res[oo] = Rd::finish(v);
+    }
+    return;
+  }
+  // RU outputs per thread at once: their loads from one member are independent
+  for (i64 o0 = t; o0 < g.nout; o0 += (i64)RT * RU) {
+    A v[RU];
+#pragma unroll
+    for (int k = 0; k < RU; ++k) v[k] = Rd::neutral();
+    for (int i = 0; i < ng; ++i) {
+      A x[RU];
+#pragma unroll
+      for (int k = 0; k < RU; ++k)
+        if (o0 + (i64)k * RT < g.nout) x[k] = ld16_cv<A>(grp[i] + (size_t)(o0 + (i64)k * RT) * 16);
+#pragma unroll
+      for (int k = 0; k < RU; ++k)
+        if (o0 + (i64)k * RT < g.nout) v[k] = Rd::comb(v[k], x[k]);
+    }
+#pragma unroll
+    for (int k = 0; k < RU; ++k)
+      if (o0 + (i64)k * RT < g.nout) res[o0 + (i64)k * RT] = Rd::finish(v[k]);
+  }
+}
+
 // the NCCL fallback's second kernel: fold the P gathered partials in rank order
 template <class E, int M, int O>
 __global__ void k_reduce_fold(const unsigned char* slots, int P, void* result) {
@@ -250,8 +509,10 @@ struct ReduceState {
   unsigned* ticket = nullptr;
   unsigned char* part = nullptr;    // G_max partials
   unsigned char* gather = nullptr;  // [0]: the rank partial; [1 + r]: gathered partials (fallback)
-  void** tables = nullptr;          // remote_words[nranks], peer_slots[nranks] (flag window)
+  void** tables = nullptr;          // remote_words[nranks], peer_slots[nranks], areas[nranks]
   bool tables_ready = false;
+  unsigned* dtickets = nullptr;     // pa_reduce_dims: G_max + 1 tickets and G_max * RT partials,
+  unsigned char* dpart = nullptr;   //   made by the first such call (stream-ordered)
   cudaEvent_t done = nullptr;       // the previous reduction's last kernel
   ull seq = 0;
   // held from the wait on `done` to its record: host threads calling at once cannot both order
@@ -269,6 +530,8 @@ void reduce_state_destroy(ReduceState* s) {
   cudaFree(s->part);
   cudaFree(s->gather);
   cudaFree(s->tables);
+  cudaFree(s->dtickets);
+  cudaFree(s->dpart);
   cudaGetLastError();
   delete s;
 }
@@ -291,7 +554,7 @@ static pa_status make_state(int nranks, cudaStream_t stream, bool ordered, Reduc
   CU(cudaMemsetAsync(s->ticket, 0, sizeof(unsigned), stream));
   CU(alloc((void**)&s->part, (size_t)s->G_max * 16));
   CU(alloc((void**)&s->gather, (size_t)(nranks + 1) * 16));
-  if (nranks > 1) CU(alloc((void**)&s->tables, 2 * sizeof(void*) * (size_t)nranks));
+  if (nranks > 1) CU(alloc((void**)&s->tables, 3 * sizeof(void*) * (size_t)nranks));
   CU(cudaEventCreateWithFlags(&s->done, cudaEventDisableTiming));
   if (!ordered) CU(cudaStreamSynchronize(stream));
   *out = s.release();
@@ -303,11 +566,12 @@ pa_status reduce_state_create(int nranks, ReduceState** out) {
 }
 
 pa_status reduce_state_set_tables(ReduceState* s, int nranks, unsigned long long* const* remote_words,
-                                  unsigned char* const* peer_slots) {
-  std::vector<void*> tab(2 * (size_t)nranks);
+                                  unsigned char* const* peer_slots, unsigned char* const* areas) {
+  std::vector<void*> tab(3 * (size_t)nranks);
   for (int r = 0; r < nranks; ++r) {
     tab[r] = remote_words[r];
     tab[nranks + r] = peer_slots[r];
+    tab[2 * nranks + r] = areas[r];
   }
   CU(cudaMemcpy(s->tables, tab.data(), tab.size() * sizeof(void*), cudaMemcpyHostToDevice));
   s->tables_ready = true;
@@ -324,10 +588,14 @@ struct Launch {
   cudaStream_t stream;
   const unsigned char* gathered;  // C_GATHER: the fold kernel's input (NULL: no fold)
   int nranks;
+  const DArgs* d;                 // pa_reduce_dims (k_reduce_dims instead of k_reduce)
 };
 
 template <class E, int M, int O> static pa_status run(const Launch& L) {
-  k_reduce<E, M, O><<<L.g.G, RT, 0, L.stream>>>(L.g);
+  if (L.d)
+    k_reduce_dims<E, M, O><<<(unsigned)(L.d->tiles * L.d->S), RT, 0, L.stream>>>(*L.d);
+  else
+    k_reduce<E, M, O><<<L.g.G, RT, 0, L.stream>>>(L.g);
   count_launch();
   CU(cudaGetLastError());
   return PA_OK;
@@ -384,6 +652,29 @@ static int dtype_size(int dtype) {
   return 0;
 }
 
+// the state serving a call: the communicator's, or the device's one-rank state (made here)
+static pa_status state_of(Comm* comm, const ReduceWindow& w, void* stream, ReduceState** out) {
+  if (comm) {
+    *out = *w.state;  // made with the communicator
+    return PA_OK;
+  }
+  int dev = 0;
+  CU(cudaGetDevice(&dev));
+  std::lock_guard<std::mutex> lock(g_local_mu);
+  ReduceState*& s0 = g_local_states[dev];
+  if (!s0) RC(make_state(1, (cudaStream_t)stream, true, &s0));
+  *out = s0;
+  return PA_OK;
+}
+
+static void set_pred(RArgs* g, int dtype, int map, int op, const void* pred_value, int es) {
+  g->pred = op >> 4;
+  if (pred_value) {
+    int vs = (map == M_ID) ? es : (dtype == D_C64 ? 8 : dtype == D_C32 ? 4 : es);  // the mapped value
+    memcpy(g->ref, pred_value, (size_t)vs);
+  }
+}
+
 pa_status reduce(Comm* comm, int dtype, int map, int op, const void* pred_value, i64 n,
                  const void* a, const void* b, void* result, void* stream) {
   ReduceWindow w;
@@ -397,19 +688,7 @@ pa_status reduce(Comm* comm, int dtype, int map, int op, const void* pred_value,
     return PA_ESTATE;
   }
   ReduceState* st = nullptr;
-  if (comm) {
-    st = *w.state;  // made with the communicator
-  } else {
-    int dev = 0;
-    CU(cudaGetDevice(&dev));
-    std::lock_guard<std::mutex> lock(g_local_mu);
-    ReduceState*& s0 = g_local_states[dev];
-    if (!s0) {
-      pa_status s = make_state(1, (cudaStream_t)stream, true, &s0);
-      if (s != PA_OK) return s;
-    }
-    st = s0;
-  }
+  RC(state_of(comm, w, stream, &st));
   std::lock_guard<std::mutex> serial(st->mu);
   const bool flags = P > 1 && w.flags;
   if (flags && !st->tables_ready) {
@@ -438,11 +717,7 @@ pa_status reduce(Comm* comm, int dtype, int map, int op, const void* pred_value,
   g.chunk = (g.nunits + g.G - 1) / g.G;
   g.a = a;
   g.b = map == M_DOT ? b : a;
-  g.pred = op >> 4;
-  if (pred_value) {
-    int vs = (map == M_ID) ? es : (dtype == D_C64 ? 8 : dtype == D_C32 ? 4 : es);  // the mapped value
-    memcpy(g.ref, pred_value, (size_t)vs);
-  }
+  set_pred(&g, dtype, map, op, pred_value, es);
   g.ticket = st->ticket;
   g.part = st->part;
   g.result = result;
@@ -474,6 +749,134 @@ pa_status reduce(Comm* comm, int dtype, int map, int op, const void* pred_value,
     if (s != PA_OK) return s;
   }
   CU(cudaEventRecord(st->done, L.stream));
+  return PA_OK;
+}
+
+static i64 pow2_ceil(i64 x) {
+  i64 p = 1;
+  while (p < x) p <<= 1;
+  return p;
+}
+
+pa_status reduce_dims(Comm* comm, int dtype, int map, int op, const void* pred_value,
+                      const DimsGeom& geo, const void* a, const void* b, void* result, void* stream) {
+  ReduceWindow w;
+  if (comm) RC(comm_reduce_window(comm, &w));
+  const int P = w.nranks;
+  if (P > 1 && !w.flags) {
+    set_error("pa_reduce_dims: the combine runs through the communicator's flag window, and this "
+              "communicator has none (NCCL without the window, or the nccl_fences tunable)");
+    return PA_ESTATE;
+  }
+  ReduceState* st = nullptr;
+  RC(state_of(comm, w, stream, &st));
+  std::lock_guard<std::mutex> serial(st->mu);
+  if (P > 1 && !st->tables_ready) {
+    set_error("reduction: the flag window's tables were not uploaded (pa_comm_flags_import)");
+    return PA_ESTATE;
+  }
+  const cudaStream_t cs = (cudaStream_t)stream;
+  if (!st->dtickets) {  // stream-ordered: the first call does not synchronise the host either
+    CU(cudaMallocAsync((void**)&st->dtickets, (size_t)(st->G_max + 1) * sizeof(unsigned), cs));
+    CU(cudaMemsetAsync(st->dtickets, 0, (size_t)(st->G_max + 1) * sizeof(unsigned), cs));
+    CU(cudaMallocAsync((void**)&st->dpart, (size_t)st->G_max * RT * 16, cs));
+  }
+
+  DArgs d;
+  memset(&d, 0, sizeof d);
+  const int es = dtype_size(dtype), V = 16 / es;
+  // runs: extent-1 dims dropped, neighbours of the same class merged
+  bool rred[PA_MAX_DIMS];
+  i64 rext[PA_MAX_DIMS], rstr[PA_MAX_DIMS], stride = 1, nred = 1;
+  int nruns = 0;
+  d.nout = 1;
+  for (int i = 0; i < geo.nd; ++i) {
+    (geo.red[i] ? nred : d.nout) *= geo.ext[i];
+    if (geo.ext[i] != 1) {
+      if (nruns > 0 && rred[nruns - 1] == geo.red[i]) {
+        rext[nruns - 1] *= geo.ext[i];
+      } else {
+        rred[nruns] = geo.red[i];
+        rext[nruns] = geo.ext[i];
+        rstr[nruns++] = stride;
+      }
+    }
+    stride *= geo.ext[i];
+  }
+  // the row regime: the fastest run is reduced and at least 64 bytes long
+  const bool row = nruns > 0 && rred[0] && rext[0] * es >= 64;
+  const i64 L = row ? rext[0] : 1;
+  for (int i = row ? 1 : 0; i < nruns; ++i) {
+    if (rred[i]) {
+      d.re[d.nr] = rext[i];
+      d.rs[d.nr++] = rstr[i];
+    } else {
+      d.ke[d.nk] = rext[i];
+      d.ks[d.nk++] = rstr[i];
+    }
+  }
+  d.nrows = nred / L;
+  d.vec = row && (uintptr_t)a % 16 == 0 && (map != M_DOT || (uintptr_t)b % 16 == 0) &&
+          (L * es) % 16 == 0;
+  d.lu = d.vec ? L / V : L;
+  // teams: along the row's units first, then fewer outputs per CTA when there are few outputs
+  int Wi = row ? (int)std::min<i64>(32, pow2_ceil(d.lu)) : 1, Wr = 1, Oc = RT / Wi;
+  while (Oc > 1 && Oc / 2 >= d.nout) {
+    Oc /= 2;
+    if (row && d.nrows < 2 * (i64)Wr && d.lu > Wi) Wi *= 2;
+    else Wr *= 2;
+  }
+  d.Wi = Wi;
+  d.Wr = Wr;
+  d.Oc = Oc;
+  d.tiles = std::max<i64>(1, (d.nout + Oc - 1) / Oc);
+  // splits: only when the tiles leave SMs idle and each member keeps >= 64 items; depends on the
+  // geometry and the device only
+  i64 S = 1;
+  if (d.nout > 0 && d.tiles < st->G_max)
+    S = std::max<i64>(1, std::min<i64>(st->G_max / d.tiles, d.nrows * d.lu / ((i64)Wi * Wr * 64)));
+  const i64 Sr = std::min<i64>(S, std::max<i64>(1, d.nrows / Wr));
+  const i64 Si = std::max<i64>(1, std::min<i64>(S / Sr, d.lu / Wi));
+  d.Sr = (int)Sr;
+  d.S = (int)(Sr * Si);
+  d.rchunk = std::max<i64>(1, (d.nrows + Sr - 1) / Sr);
+  d.uchunk = std::max<i64>(1, (d.lu + Si - 1) / Si);
+  d.a = a;
+  d.b = map == M_DOT ? b : a;
+  RArgs pr;
+  memset(&pr, 0, sizeof pr);
+  set_pred(&pr, dtype, map, op, pred_value, es);
+  d.pred = pr.pred;
+  memcpy(d.ref, pr.ref, 16);
+  d.tickets = st->dtickets;
+  d.part = st->dpart;
+  d.result = result;
+  d.nranks = P;
+  d.rank = w.rank;
+  if (P > 1) {
+    d.seq = ++st->seq;  // one sequence with pa_reduce: the parity sets alternate across both
+    d.local_words = w.local_words;
+    d.word_stride = w.word_stride;
+    d.remote_words = (ull* const*)st->tables;
+    d.areas = (unsigned char* const*)(st->tables + 2 * P);
+    d.area_off = (size_t)(d.seq & 1) * REDUCE_AREA_BYTES;
+    d.topo_M = geo.topo_M;
+    for (int i = 0; i < geo.topo_M; ++i) {
+      d.topo_dims[i] = (int)geo.topo_dims[i];
+      d.coords[i] = (int)geo.coords[i];
+    }
+    d.keep_grid = geo.keep_grid;
+    d.timeout_ns = w.timeout_ns;
+    d.err = w.err;
+  }
+
+  Launch Ln;
+  memset(&Ln, 0, sizeof Ln);
+  Ln.stream = cs;
+  Ln.d = &d;
+  CU(cudaStreamWaitEvent(cs, st->done, 0));
+  RC(dispatch(dtype, map, op, false, Ln));
+  CU(cudaEventRecord(st->done, cs));
   return PA_OK;
 }
 

@@ -246,12 +246,16 @@ struct Comm {
   ReduceState* reduce = nullptr;         // the reductions' workspace and event (reduce.cu)
 };
 
-// the window: the words [source rank][kind], then the reductions' slots [parity][source rank]
+// the window: the words [source rank][kind], then the reductions' slots [parity][source rank],
+// then pa_reduce_dims' two parity sets of this rank's own partial area (REDUCE_AREA_BYTES each)
 static size_t reduce_slots_offset(int nranks) {
   return (sizeof(ull) * (size_t)nranks * FK_KINDS + 15) / 16 * 16;
 }
-static size_t window_bytes(int nranks) {
+static size_t reduce_area_offset(int nranks) {
   return reduce_slots_offset(nranks) + 2 * (size_t)nranks * REDUCE_SLOT_BYTES;
+}
+static size_t window_bytes(int nranks) {
+  return reduce_area_offset(nranks) + 2 * REDUCE_AREA_BYTES;
 }
 
 static ull* remote_word(Comm* c, int peer_rank, int kind) {
@@ -362,7 +366,7 @@ pa_status comm_flags_export(Comm* c, void* handle64, i64* offset) {
   if (!c->flags) {
     // (a whole 2 MiB block of its own: small cudaMalloc allocations share a block, and
     //  a block can be opened only once per importing process)
-    const size_t bytes = std::max<size_t>(window_bytes(c->nranks), IPC_BLOCK);
+    const size_t bytes = (window_bytes(c->nranks) + IPC_BLOCK - 1) / IPC_BLOCK * IPC_BLOCK;
     CU(cudaMalloc((void**)&c->flags, bytes));
     CU(cudaMemset(c->flags, 0, bytes));
     CU(cudaHostAlloc((void**)&c->fence_err, sizeof(int), cudaHostAllocMapped));
@@ -391,16 +395,19 @@ pa_status comm_flags_import(Comm* c, int rank, const void* handle64, i64 offset)
   for (int r = 0; r < c->nranks; ++r)
     if (r != c->rank && !c->peer_flags[r]) all = false;
   c->flags_ready = all;
-  if (all && c->nranks > 1) {  // the reductions' peer words and slots (reduce.cu)
-    const size_t so = reduce_slots_offset(c->nranks);
+  if (all && c->nranks > 1) {  // the reductions' peer words, slots and areas (reduce.cu)
+    const size_t so = reduce_slots_offset(c->nranks), ao = reduce_area_offset(c->nranks);
     std::vector<ull*> words(c->nranks, nullptr);
-    std::vector<unsigned char*> slots(c->nranks, nullptr);
-    for (int r = 0; r < c->nranks; ++r)
+    std::vector<unsigned char*> slots(c->nranks, nullptr), areas(c->nranks, nullptr);
+    for (int r = 0; r < c->nranks; ++r) {
+      const ull* win = r == c->rank ? c->flags : c->peer_flags[r];
+      areas[r] = (unsigned char*)win + ao;
       if (r != c->rank) {
         words[r] = remote_word(c, r, FK_REDUCE);
         slots[r] = (unsigned char*)c->peer_flags[r] + so;
       }
-    RC(reduce_state_set_tables(c->reduce, c->nranks, words.data(), slots.data()));
+    }
+    RC(reduce_state_set_tables(c->reduce, c->nranks, words.data(), slots.data(), areas.data()));
   }
   return PA_OK;
 }

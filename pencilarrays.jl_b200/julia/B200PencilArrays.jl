@@ -703,4 +703,54 @@ for (fn, code) in ((:any, 3), (:all, 4))
     end
 end
 
+# ---- reductions along dims (pa_reduce_dims, DESIGN §3l) -----------------------------------------
+# mapreduce_dims(f, op, u[, v]; dims): `dims` are LOGICAL dims (1..N spatial, N+1.. extra, as
+# ndims(u) counts them).  Returns this rank's CuArray, laid out like parent(u) with extent 1 along
+# the reduced dims: the reduction over their global ranges at this rank's kept indices, combined
+# over the ranks that share them.  Base.mapreduce(...; dims) keeps the reference's method, which
+# counts memory-order dims and Allreduces over all ranks (right only when every decomposed dim is
+# reduced).  For any / all pass op = any or all and f = a predicate pa_pred recognises.
+function mapreduce_dims(f::F, op::OP, u::CuPencilArray{T}, etc::Vararg{CuPencilArray{T}};
+                        dims) where {F,OP,T<:PA_ELTYPES}
+    length(etc) <= 1 || throw(ArgumentError("mapreduce_dims takes one or two arrays"))
+    v = isempty(etc) ? nothing : etc[1]
+    v === nothing || PencilArrays._check_compatible_arrays(u, v)
+    if op === any || op === all
+        p = pa_pred(f)
+        (p !== nothing && (p[2] === nothing || exact_in(T, p[2]))) ||
+            throw(ArgumentError("mapreduce_dims: predicate $f is not one the library runs"))
+        map, code, value = Cint(0), Cint(op === any ? 3 : 4) | p[1], p[2]
+    else
+        map, code, value = pa_map(f), pa_op(op), nothing
+        (map !== nothing && code !== nothing && (v !== nothing) == (map == 3)) ||
+            throw(ArgumentError("mapreduce_dims: ($f, $op) is not a reduction the library runs"))
+    end
+    H = handles(topology(pencil(u)))
+    dt = PA_DTYPE[T]
+    rt = Ref{Cint}()
+    check(ccall((:pa_reduce_result_type, libpa), Cint, (Cint, Cint, Cint, Ptr{Cint}), dt, map, code, rt))
+    ds = Cint[d for d in dims]
+    N = ndims(pencil(u))
+    pp = permutation(pencil(u))
+    perm = isidentity(pp) ? Tuple(1:N) : Tuple(pp)  # memory dim m holds logical dim perm[m]
+    shape = collect(size(parent(u)))
+    for d in ds
+        1 <= d <= length(shape) || throw(ArgumentError("dim $d out of range 1..$(length(shape))"))
+        shape[d <= N ? findfirst(==(d), perm) : d] = 1
+    end
+    result = CuArray{PA_RESULT[rt[]]}(undef, shape...)
+    VT = map == 0 ? T : real(T)
+    ref = value === nothing ? C_NULL : Ref{VT}(convert(VT, value))
+    ex = Int64[extra_dims(u)...]
+    ptr_or_null(A) = isempty(A) ? C_NULL : devptr(A)
+    GC.@preserve ref ds check(ccall((:pa_reduce_dims, libpa), Cint,
+        (Ptr{Cvoid}, Cint, Ptr{Int64}, Ptr{Cvoid}, Cint, Cint, Cint, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid},
+         Cint, Ptr{Cint}, Ptr{Cvoid}, Ptr{Cvoid}),
+        pencil_handle(H, pencil(u)), length(ex), ex, H.comm, dt, map, code,
+        ref === C_NULL ? C_NULL : Base.unsafe_convert(Ptr{Cvoid}, ref), ptr_or_null(parent(u)),
+        v === nothing ? C_NULL : ptr_or_null(parent(v)), length(ds), ds, ptr_or_null(result),
+        stream_ptr()))
+    result
+end
+
 end # module

@@ -12,6 +12,13 @@ against ``value`` (which must be exactly representable in the mapped element typ
 comparison runs in that type), or ``"isnan"`` / ``"isfinite"``.  The result's type comes from the library
 (``pa_reduce_result_type``): sum of int32 gives int64, abs / abs2 / realdot of complex values
 the real type, any / all bool.
+
+Every function takes ``dims``: ``None`` (the default) reduces over everything, as above; a dim or
+a collection of 1-based LOGICAL dims (``1..N`` the pencil's spatial dims, ``N+1..`` its extra
+dims) reduces over those only (``pa_reduce_dims``, DESIGN §3l).  The result is then a tensor of
+``u.data.shape`` with every reduced position set to 1: along each kept dim it holds this rank's
+local range, combined over the ranks that share it, so ``u.data - mean`` broadcasts with no
+further exchange.
 """
 from __future__ import annotations
 
@@ -25,6 +32,7 @@ import torch
 from . import _lib
 from ._lib import lib, check, i64arr, ArgumentError
 from .arrays import PencilArray
+from .permutations import as_tuple
 from .transpositions import _stream_ptr
 
 
@@ -96,7 +104,33 @@ def _exact(value, vt):
     return t
 
 
-def _reduce(code_map, code_op, u: PencilArray, vs, value=None):
+def result_shape(u: PencilArray, dims):
+    """The checked ``dims`` as a tuple of 1-based logical dims, and the torch shape of the result
+    of a reduction of ``u`` along them: ``u.data.shape`` with the reduced positions set to 1."""
+    if isinstance(dims, int) and not isinstance(dims, bool):
+        dims = (dims,)
+    try:
+        dims = tuple(dims)
+    except TypeError:
+        raise ArgumentError(_lib.PA_EINVAL, f"dims {dims!r} is not a dim or a collection of dims") from None
+    N, nd = len(u.space_dims), u.data.dim()
+    if not dims:
+        raise ArgumentError(_lib.PA_EINVAL, "dims must name at least one dim")
+    for d in dims:
+        if not isinstance(d, int) or isinstance(d, bool) or not 1 <= d <= nd:
+            raise ArgumentError(_lib.PA_EINVAL, f"dim {d!r} out of range 1..{nd} ({N} spatial dims, "
+                                f"then {nd - N} extra)")
+    if len(set(dims)) != len(dims):
+        raise ArgumentError(_lib.PA_EINVAL, f"dims {dims} name a dim twice")
+    perm = as_tuple(u.pencil.perm, N)  # memory dim m holds logical dim perm[m]
+    shape = list(u.data.shape)
+    for d in dims:
+        m = perm.index(d) if d <= N else d - 1
+        shape[nd - 1 - m] = 1
+    return dims, tuple(shape)
+
+
+def _reduce(code_map, code_op, u: PencilArray, vs, value=None, dims=None):
     if len(vs) > 1:
         raise ArgumentError(_lib.PA_EINVAL, f"mapreduce takes one or two arrays: got {1 + len(vs)}")
     for v in vs:  # _check_compatible_arrays (arrays.jl:499-504), plus what the kernel reads
@@ -114,52 +148,58 @@ def _reduce(code_map, code_op, u: PencilArray, vs, value=None):
     if value is not None:  # one value of the mapped type
         vt = u.dtype if code_map == _lib.PA_MAP_IDENTITY else _REAL.get(u.dtype, u.dtype)
         pred = _exact(value, vt)
-    result = torch.empty((), dtype=_TORCH[out.value], device=u.data.device)
     comm = u.pencil.topology.comm
     ex = u.extra_dims
+    args = (u.pencil._h, len(ex), i64arr(ex), comm.handle, dt, code_map, code_op,
+            C.c_void_p(pred.data_ptr()) if pred is not None else None,
+            C.c_void_p(u.data_ptr() or None), C.c_void_p(vs[0].data_ptr() or None) if vs else None)
+    if dims is None:
+        result = torch.empty((), dtype=_TORCH[out.value], device=u.data.device)
+        with torch.cuda.device(u.data.device):
+            check(lib.pa_reduce(*args, C.c_void_p(result.data_ptr()), _stream_ptr()))
+        return result
+    dims, shape = result_shape(u, dims)
+    result = torch.empty(shape, dtype=_TORCH[out.value], device=u.data.device)
     with torch.cuda.device(u.data.device):
-        check(lib.pa_reduce(u.pencil._h, len(ex), i64arr(ex), comm.handle, dt, code_map, code_op,
-                            C.c_void_p(pred.data_ptr()) if pred is not None else None,
-                            C.c_void_p(u.data_ptr() or None),
-                            C.c_void_p(vs[0].data_ptr() or None) if vs else None,
-                            C.c_void_p(result.data_ptr()), _stream_ptr()))
+        check(lib.pa_reduce_dims(*args, len(dims), (C.c_int * len(dims))(*dims),
+                                 C.c_void_p(result.data_ptr() or None), _stream_ptr()))
     return result
 
 
-def mapreduce(f, op, u: PencilArray, *vs: PencilArray):
-    """``mapreduce(f, op, u, vs...)`` over all ranks; ``f`` of two arrays is :func:`realdot`."""
-    return _reduce(_lookup(_MAPS, f, "function"), _lookup(_OPS, op, "op"), u, vs)
+def mapreduce(f, op, u: PencilArray, *vs: PencilArray, dims=None):
+    """``mapreduce(f, op, u, vs...; dims)`` over all ranks; ``f`` of two arrays is :func:`realdot`."""
+    return _reduce(_lookup(_MAPS, f, "function"), _lookup(_OPS, op, "op"), u, vs, dims=dims)
 
 
-def sum(u: PencilArray, f=None):
-    """``sum(f, u)``."""
-    return mapreduce(f, "+", u)
+def sum(u: PencilArray, f=None, dims=None):
+    """``sum(f, u; dims)``."""
+    return mapreduce(f, "+", u, dims=dims)
 
 
-def maximum(u: PencilArray, f=None):
-    """``maximum(f, u)``; a NaN anywhere gives NaN.  Refused for a globally empty array."""
-    return mapreduce(f, "max", u)
+def maximum(u: PencilArray, f=None, dims=None):
+    """``maximum(f, u; dims)``; a NaN anywhere gives NaN.  Refused for a globally empty range."""
+    return mapreduce(f, "max", u, dims=dims)
 
 
-def minimum(u: PencilArray, f=None):
-    """``minimum(f, u)``; a NaN anywhere gives NaN.  Refused for a globally empty array."""
-    return mapreduce(f, "min", u)
+def minimum(u: PencilArray, f=None, dims=None):
+    """``minimum(f, u; dims)``; a NaN anywhere gives NaN.  Refused for a globally empty range."""
+    return mapreduce(f, "min", u, dims=dims)
 
 
-def _pred(op, u, pred, value, f):
+def _pred(op, u, pred, value, f, dims):
     p = _lookup(_PREDS, pred, "predicate")
     if p in (_lib.PA_PRED_ISNAN, _lib.PA_PRED_ISFINITE):
         value = None
     elif value is None:
         raise ArgumentError(_lib.PA_EINVAL, f"the predicate {pred!r} compares against `value`")
-    return _reduce(_lookup(_MAPS, f, "function"), op | p, u, (), value)
+    return _reduce(_lookup(_MAPS, f, "function"), op | p, u, (), value, dims)
 
 
-def any(u: PencilArray, pred, value=None, f=None):
-    """``any(x -> pred(f(x), value), u)``, e.g. ``any(u, ">", 0)`` or ``any(u, "isnan")``."""
-    return _pred(_lib.PA_OP_ANY, u, pred, value, f)
+def any(u: PencilArray, pred, value=None, f=None, dims=None):
+    """``any(x -> pred(f(x), value), u; dims)``, e.g. ``any(u, ">", 0)`` or ``any(u, "isnan")``."""
+    return _pred(_lib.PA_OP_ANY, u, pred, value, f, dims)
 
 
-def all(u: PencilArray, pred, value=None, f=None):
-    """``all(x -> pred(f(x), value), u)``, e.g. ``all(u, "isfinite")``."""
-    return _pred(_lib.PA_OP_ALL, u, pred, value, f)
+def all(u: PencilArray, pred, value=None, f=None, dims=None):
+    """``all(x -> pred(f(x), value), u; dims)``, e.g. ``all(u, "isfinite")``."""
+    return _pred(_lib.PA_OP_ALL, u, pred, value, f, dims)
