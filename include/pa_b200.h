@@ -622,6 +622,49 @@ pa_status pa_reduce_dims(const pa_pencil* pencil, int n_extra, const int64_t* ex
                          const void* a, const void* b, int n_dims, const int* dims, void* result,
                          void* stream);
 
+/* Shell-binned spectrum of complex PencilArrays whose spatial dims are the modes of an unnormalised
+ * DFT: E(b) = sum over the modes k with bin(|k|) == b of w(k) * f(x), f = abs2 of `a`
+ * (PA_MAP_ABS2) or real(a * conj(b)) (PA_MAP_DOT, a co-spectrum); extra dims (vector components)
+ * add into the same bins.  `result` receives nbins values of pa_reduce_result_type(dtype, map,
+ * PA_OP_SUM) (Float64 / Float32): the GLOBAL spectrum, the same bits on every rank.  Geometry
+ * (reduce_core.hpp, DESIGN §3m), along logical dim d of global extent N_d at global 0-based index i:
+ *   wavenumber  n = i if i < (N_d + 1) / 2 else i - N_d (numpy's fftfreq order); along the r2c dim
+ *               (rfft_dim, 1-based; 0: none) n = i, that dim holding M = rfft_n / 2 + 1 bins of a
+ *               real length rfft_n (0: the default 2 (M - 1); any rfft_n with rfft_n / 2 + 1 == M);
+ *   weight      w = 2 along the r2c dim except at i = 0 and (rfft_n even) i = rfft_n / 2, else 1;
+ *   bin         k_d = scales[d - 1] * n_d (scales NULL: all 1), q = k_1 * k_1 + k_2 * k_2 + ... in
+ *               logical-dim order, b = floor(sqrt(q) / width + 0.5), each operation one correctly
+ *               rounded fp64 operation (NumPy's elementwise result bit for bit); modes with
+ *               b >= nbins are dropped.
+ * Contributions are computed as pa_reduce computes the map and summed in fp64 (Float32 results
+ * rounded once), a NaN poisons its own bin only; the order of every sum depends on the geometry, the
+ * arguments, the device and the base addresses modulo 16 only.  ONE kernel per rank and call,
+ * ordered on `stream`, collective over the communicator (ranks owning nothing take part), the host
+ * is not synchronised; shares pa_reduce's serialisation.  nbins is at most PA_SPECTRUM_MAX_BINS:
+ * each of a CTA's four warps keeps a histogram of nbins doubles in shared memory (128 KiB at the
+ * cap).  Refused on the host, in this order, identically on every rank (error texts start with
+ * "pa_shell_spectrum:"), PA_EINVAL: a NULL pencil; dtype not complex or map not PA_MAP_ABS2 /
+ * PA_MAP_DOT; `b` given for PA_MAP_ABS2 or missing for PA_MAP_DOT (NULL arrays are fine where the
+ * local array is empty); bad extra dims; rfft_dim outside
+ * 0..N; rfft_n inconsistent with the r2c dim's extent (or given without one); a scale or the width
+ * not finite and positive; nbins outside 1..PA_SPECTRUM_MAX_BINS; NULL arrays for a non-empty local
+ * array; arrays not aligned to their real component; a NULL `result` or one not aligned to the
+ * result type.  PA_EINCOMPAT: the topology's rank count is not the communicator's (or comm == NULL
+ * with more than one rank).  Then without a device PA_ENOGPU.  PA_ESTATE: more than one rank on a
+ * communicator without a flag window.                                                             */
+#define PA_SPECTRUM_MAX_BINS 4096
+pa_status pa_shell_spectrum(const pa_pencil* pencil, int n_extra, const int64_t* extra_dims,
+                            pa_comm* comm, int dtype, int map, const void* a, const void* b,
+                            int rfft_dim, int64_t rfft_n, const double* scales, double width,
+                            int nbins, void* result, void* stream);
+/* The default nbins of pa_shell_spectrum: the bin of the extreme mode (the largest |wavenumber|
+ * along every dim) plus one, from the same geometry functions; it may exceed
+ * PA_SPECTRUM_MAX_BINS, which pa_shell_spectrum then refuses.  Refused like pa_shell_spectrum (a
+ * NULL pencil, then its rfft_dim / rfft_n / scales / width checks), or when the bin does not fit an
+ * int.  Host-only.                                                                                 */
+pa_status pa_shell_spectrum_nbins(const pa_pencil* pencil, int rfft_dim, int64_t rfft_n,
+                                  const double* scales, double width, int* nbins);
+
 /* ---- host chains -----------------------------------------------------------
  * A sequence of transpositions applied to HOST arrays (plan i+1 consumes what
  * plan i produces): one submit = upload of `host_src`, every transpose! on the

@@ -29,6 +29,7 @@ from .transpositions import (Transposition, transpose_, transpose_bang, Waitall,
 
 from . import reductions
 from .reductions import mapreduce, sum, maximum, minimum, any, all, abs2, realdot
+from .reductions import shell_spectrum, spectrum_nbins
 
 
 from . import pencilio as PencilIO

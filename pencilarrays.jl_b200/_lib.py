@@ -39,6 +39,7 @@ PA_RODFT10 = 9
 PA_FLOAT64, PA_FLOAT32, PA_COMPLEXF64, PA_COMPLEXF32, PA_INT32, PA_INT64, PA_BOOL = range(7)
 PA_MAP_IDENTITY, PA_MAP_ABS, PA_MAP_ABS2, PA_MAP_DOT = range(4)
 PA_OP_SUM, PA_OP_MAX, PA_OP_MIN, PA_OP_ANY, PA_OP_ALL = range(5)
+PA_SPECTRUM_MAX_BINS = 4096
 (PA_PRED_EQ, PA_PRED_NE, PA_PRED_LT, PA_PRED_LE, PA_PRED_GT, PA_PRED_GE, PA_PRED_ISNAN,
  PA_PRED_ISFINITE) = (k << 4 for k in range(1, 9))
 
@@ -171,6 +172,9 @@ SIGNATURES = {
     "pa_reduce_result_type": (C.c_int, [C.c_int, C.c_int, C.c_int, _IP]),
     "pa_reduce_dims": (C.c_int, [_P, C.c_int, _I64P, _P, C.c_int, C.c_int, C.c_int, _P, _P, _P,
                                  C.c_int, _IP, _P, _P]),
+    "pa_shell_spectrum": (C.c_int, [_P, C.c_int, _I64P, _P, C.c_int, C.c_int, _P, _P, C.c_int,
+                                    C.c_int64, _P, C.c_double, C.c_int, _P, _P]),
+    "pa_shell_spectrum_nbins": (C.c_int, [_P, C.c_int, C.c_int64, _P, C.c_double, _IP]),
     "pa_plan_timings": (C.c_int, [_P, C.POINTER(Timings)]),
     "pa_plan_enable_timing": (C.c_int, [_P, C.c_int]),
 }

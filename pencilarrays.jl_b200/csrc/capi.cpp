@@ -1506,6 +1506,169 @@ pa_status pa_reduce_dims(const pa_pencil* pencil, int n_extra, const int64_t* ex
   })
 }
 
+// ---- shell-binned spectra ------------------------------------------------------------------------
+// The geometry checks shared by pa_shell_spectrum and pa_shell_spectrum_nbins, in the header's
+// order from rfft_dim on; *n_real = the r2c dim's real length.  Every message starts with `who`.
+static pa_status spectrum_geometry(const Pencil& Pn, int rfft_dim, int64_t rfft_n,
+                                   const double* scales, double width, i64* n_real) {
+  const char* who = "pa_shell_spectrum";
+  if (rfft_dim < 0 || rfft_dim > Pn.N) {
+    set_error("%s: rfft_dim %d out of range 0..%d (0: no r2c dim)", who, rfft_dim, Pn.N);
+    return PA_EINVAL;
+  }
+  *n_real = 0;
+  if (rfft_dim > 0) {
+    const i64 M = Pn.size_global[rfft_dim - 1];
+    const i64 n = rfft_n == 0 ? std::max<i64>(0, 2 * (M - 1)) : rfft_n;
+    if (rfft_n < 0 || (M > 0 && n / 2 + 1 != M) || (M == 0 && rfft_n != 0)) {
+      set_error("%s: rfft_n %lld does not fit the r2c dim's %lld bins (n / 2 + 1 must be %lld)", who,
+                (long long)rfft_n, (long long)M, (long long)M);
+      return PA_EINVAL;
+    }
+    *n_real = n;
+  } else if (rfft_n != 0) {
+    set_error("%s: rfft_n %lld given without an r2c dim", who, (long long)rfft_n);
+    return PA_EINVAL;
+  }
+  for (int d = 0; d < Pn.N; ++d) {
+    const double s = scales ? scales[d] : 1.0;
+    if (!(s > 0.0) || !std::isfinite(s)) {
+      set_error("%s: scale %g of dim %d is not finite and positive", who, s, d + 1);
+      return PA_EINVAL;
+    }
+  }
+  if (!(width > 0.0) || !std::isfinite(width)) {
+    set_error("%s: width %g is not finite and positive", who, width);
+    return PA_EINVAL;
+  }
+  return PA_OK;
+}
+
+// the bin of the extreme mode plus one: |k| grows with every |wavenumber|, so the corner of the
+// largest |wavenumber| along each dim holds the last bin (every dim of extent 0 or 1 adds 0)
+static i64 spectrum_default_bins(const Pencil& Pn, int rfft_dim, const double* scales, double width) {
+  double q = 0.0;
+  for (int d = 0; d < Pn.N; ++d) {
+    const i64 n = Pn.size_global[d];
+    const i64 top = n == 0 ? 0 : d + 1 == rfft_dim ? n - 1 : n / 2;
+    const double k = red::spec_k(scales ? scales[d] : 1.0, top);
+    q = red::add(q, red::mul(k, k));
+  }
+  const double b = red::spec_shell(q, width);
+  return b + 1.0 > (double)INT32_MAX ? (i64)INT32_MAX + 1 : (i64)b + 1;
+}
+
+pa_status pa_shell_spectrum_nbins(const pa_pencil* pencil, int rfft_dim, int64_t rfft_n,
+                                  const double* scales, double width, int* nbins) {
+  GUARD({
+    if (!pencil) {
+      set_error("pa_shell_spectrum: null pencil");
+      return PA_EINVAL;
+    }
+    i64 n_real = 0;
+    RC(spectrum_geometry(*pencil->p, rfft_dim, rfft_n, scales, width, &n_real));
+    const i64 b = spectrum_default_bins(*pencil->p, rfft_dim, scales, width);
+    if (b > INT32_MAX) {
+      set_error("pa_shell_spectrum: the extreme mode's bin does not fit an int");
+      return PA_EINVAL;
+    }
+    if (nbins) *nbins = (int)b;
+    return PA_OK;
+  })
+}
+
+// pa_shell_spectrum: every check in the order of pa_b200.h, then the kernel
+static pa_status spectrum_call(const pa_pencil* pencil, int n_extra, const int64_t* extra_dims,
+                               pa_comm* comm, int dtype, int map, const void* a, const void* b,
+                               int rfft_dim, int64_t rfft_n, const double* scales, double width,
+                               int nbins, void* result, void* stream) {
+  const char* who = "pa_shell_spectrum";
+  if (!pencil) {
+    set_error("%s: null pencil", who);
+    return PA_EINVAL;
+  }
+  if ((dtype != PA_COMPLEXF64 && dtype != PA_COMPLEXF32) ||
+      (map != PA_MAP_ABS2 && map != PA_MAP_DOT)) {
+    set_error("%s: dtype %d, map %d: a spectrum is of ComplexF64 / ComplexF32 arrays under "
+              "PA_MAP_ABS2 (one array) or PA_MAP_DOT (two)", who, dtype, map);
+    return PA_EINVAL;
+  }
+  const Pencil& Pn = *pencil->p;
+  i64 lo[PA_MAX_DIMS], hi[PA_MAX_DIMS];
+  Pn.range_local(lo, hi);
+  i64 n_spatial = 1;  // (a rank owning nothing may pass NULL arrays)
+  for (int d = 0; d < Pn.N; ++d) n_spatial *= hi[d] - lo[d];
+  if (map == PA_MAP_DOT ? (n_spatial > 0 && !b) : b != nullptr) {
+    set_error(map == PA_MAP_DOT ? "%s: PA_MAP_DOT bins two arrays: `b` is missing"
+                                : "%s: a second array `b` goes with PA_MAP_DOT only", who);
+    return PA_EINVAL;
+  }
+  if (n_extra < 0 || (n_extra > 0 && !extra_dims) || Pn.N + n_extra > PA_MAX_DIMS) {
+    set_error("%s: %d extra dims on a %d-d pencil (at most %d dims in all)", who, n_extra, Pn.N,
+              PA_MAX_DIMS);
+    return PA_EINVAL;
+  }
+  SpecGeom g;
+  g.n = n_spatial;
+  for (int i = 0; i < n_extra; ++i) {
+    if (extra_dims[i] < 0) {
+      set_error("%s: negative extra dim", who);
+      return PA_EINVAL;
+    }
+    g.n *= extra_dims[i];
+  }
+  RC(spectrum_geometry(Pn, rfft_dim, rfft_n, scales, width, &g.rfft_n));
+  if (nbins < 1 || nbins > PA_SPECTRUM_MAX_BINS) {
+    set_error("%s: nbins %d out of range 1..%d", who, nbins, PA_SPECTRUM_MAX_BINS);
+    return PA_EINVAL;
+  }
+  if (g.n > 0 && (!a || (map == PA_MAP_DOT && !b))) {
+    set_error("%s: null array pointer for a non-empty local array", who);
+    return PA_EINVAL;
+  }
+  const uintptr_t al = (uintptr_t)component_bytes(dtype);
+  if (((uintptr_t)a | (uintptr_t)b) % al) {
+    set_error("%s: arrays must be aligned to %d bytes (their real component)", who, (int)al);
+    return PA_EINVAL;
+  }
+  const uintptr_t ral = dtype == PA_COMPLEXF64 ? 8 : 4;
+  if (!result || (uintptr_t)result % ral) {
+    set_error("%s: `result` must be a device pointer aligned to %d bytes", who, (int)ral);
+    return PA_EINVAL;
+  }
+  const int nranks = Pn.topo->size;
+  if (comm ? comm_size(comm->p) != nranks : nranks > 1) {
+    set_error(comm ? "%s: the topology has %d ranks, the communicator %d"
+                   : "%s: a topology of %d ranks needs a communicator", who, nranks,
+              comm ? comm_size(comm->p) : 0);
+    return PA_EINCOMPAT;
+  }
+  RC(need_gpu());
+  g.N = Pn.N;
+  for (int m = 0; m < Pn.N; ++m) {
+    const int l = Pn.perm[m];  // memory dim m holds logical dim l
+    g.ext[m] = hi[l] - lo[l];
+    g.lo[m] = lo[l];
+    g.ng[m] = Pn.size_global[l];
+    g.s[m] = scales ? scales[l] : 1.0;
+    g.lpos[l] = m;
+    if (l + 1 == rfft_dim) g.r2c = m;
+  }
+  g.width = width;
+  g.nbins = nbins;
+  return shell_spectrum(comm ? comm->p : nullptr, dtype, map, g, a, b, result, stream);
+}
+
+pa_status pa_shell_spectrum(const pa_pencil* pencil, int n_extra, const int64_t* extra_dims,
+                            pa_comm* comm, int dtype, int map, const void* a, const void* b,
+                            int rfft_dim, int64_t rfft_n, const double* scales, double width,
+                            int nbins, void* result, void* stream) {
+  GUARD({
+    return spectrum_call(pencil, n_extra, extra_dims, comm, dtype, map, a, b, rfft_dim, rfft_n,
+                         scales, width, nbins, result, stream);
+  })
+}
+
 pa_status pa_plan_timings(pa_plan* plan, pa_timings* t) {
   if (!plan || !t) return PA_EINVAL;
   return plan_timings(plan->p, t);

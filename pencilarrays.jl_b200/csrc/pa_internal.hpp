@@ -302,6 +302,24 @@ struct DimsGeom {
 pa_status reduce_dims(Comm* comm, int dtype, int map, int op, const void* pred_value,
                       const DimsGeom& geo, const void* a, const void* b, void* result, void* stream);
 
+// pa_shell_spectrum's geometry, checked by capi.cpp: the spatial dims in memory order with their
+// local extents, the global index of the first local element and the global extents; the scales;
+// the memory dim of each logical dim; the r2c dim (memory dim, -1: none) and its real length
+struct SpecGeom {
+  int N = 0;
+  i64 ext[PA_MAX_DIMS] = {0}, lo[PA_MAX_DIMS] = {0}, ng[PA_MAX_DIMS] = {0};
+  double s[PA_MAX_DIMS] = {0};
+  int lpos[PA_MAX_DIMS] = {0};
+  int r2c = -1;
+  i64 rfft_n = 0;
+  double width = 1.0;
+  int nbins = 1;
+  i64 n = 0;  // local elements, extra dims included
+};
+// the spectrum (reduce.cu); every argument has been checked.  comm NULL: one rank
+pa_status shell_spectrum(Comm* comm, int dtype, int map, const SpecGeom& geo, const void* a,
+                         const void* b, void* result, void* stream);
+
 // What a fused line kernel computes: from the lines it gathers on the receive side of a
 // transposition (unpack_fused, get_fft) or from the source lines it loads on the send side
 // (put_fft).  A plan moves the elements of one side; the array on the other side of the transform

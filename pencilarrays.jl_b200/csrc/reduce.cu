@@ -252,6 +252,34 @@ constexpr int D_RUNS = PA_MAX_DIMS / 2;  // K runs and R runs alternate: at most
 // spills 24-224 bytes per thread in every instantiation
 constexpr int D_CTAS_PER_SM = 3;
 
+// The combine of a replicated or sliced result across ranks (P > 1): every rank has stored its
+// nout partials (16-byte accumulators) into its own partial area of the flag window; the caller's
+// last CTA signals every peer, waits for every peer and folds the group's areas in rank order.
+struct GroupCombine {
+  int nranks, rank;
+  ull seq;
+  ull* local_words;
+  int word_stride;
+  ull* const* remote_words;        // device table [nranks]
+  unsigned char* const* areas;     // device table [nranks]: every rank's partial area as mapped here
+  size_t area_off;                 // the parity set's offset in an area
+  int topo_M;                      // the combine group: the ranks whose coordinates agree with
+  int topo_dims[PA_MAX_TOPO];      //   mine on every grid dim of keep_grid (0: every rank)
+  int coords[PA_MAX_TOPO];
+  unsigned keep_grid;
+  ull timeout_ns;
+  int* err;
+};
+
+__device__ __forceinline__ bool in_group(const GroupCombine& g, int q) {
+  for (int i = g.topo_M - 1; i >= 0; --i) {  // row-major rank numbering: the last coordinate fastest
+    const int c = q % g.topo_dims[i];
+    q /= g.topo_dims[i];
+    if (((g.keep_grid >> i) & 1) && c != g.coords[i]) return false;
+  }
+  return true;
+}
+
 struct DArgs {
   const void* a;
   const void* b;
@@ -270,29 +298,64 @@ struct DArgs {
   alignas(16) unsigned char ref[16];
   unsigned* tickets;               // [tiles] when S > 1, then the all-tiles ticket
   unsigned char* part;             // [tiles][S][Oc] 16-byte partials
-  int nranks, rank;
-  ull seq;
-  ull* local_words;
-  int word_stride;
-  ull* const* remote_words;        // device table [nranks]
-  unsigned char* const* areas;     // device table [nranks]: every rank's partial area as mapped here
-  size_t area_off;                 // the parity set's offset in an area
-  int topo_M;                      // the combine group: the ranks whose coordinates agree with
-  int topo_dims[PA_MAX_TOPO];      //   mine on every grid dim of keep_grid
-  int coords[PA_MAX_TOPO];
-  unsigned keep_grid;
-  ull timeout_ns;
-  int* err;
+  GroupCombine cb;
   void* result;
 };
 
-__device__ __forceinline__ bool in_group(const DArgs& g, int q) {
-  for (int i = g.topo_M - 1; i >= 0; --i) {  // row-major rank numbering: the last coordinate fastest
-    const int c = q % g.topo_dims[i];
-    q /= g.topo_dims[i];
-    if (((g.keep_grid >> i) & 1) && c != g.coords[i]) return false;
+// The last CTA's half of the combine (NT threads, every one calls it): signal every peer, wait for
+// every peer, then res[o] = the group's partials of output o folded in rank order, read in place
+// from each member's area.  Every member folds the same values in the same order.
+template <class Rd, int NT>
+__device__ __forceinline__ void group_combine(const GroupCombine& g, i64 nout, typename Rd::R* res) {
+  using A = typename Rd::A;
+  const int t = threadIdx.x, P = g.nranks, me = g.rank;
+  if (t == 0) {
+    for (int k = 1; k < P; ++k) flag_signal(g.remote_words[(me + k) % P], g.seq);
+    for (int k = 1; k < P; ++k) {  // every peer, not only the group: see DESIGN §3l
+      const int q = (me + P - k) % P;
+      flag_wait(g.local_words + (size_t)q * g.word_stride, g.seq, g.timeout_ns, g.err);
+    }
   }
-  return true;
+  // the group's areas, in rank order, listed once per call (up to NT members in shared memory)
+  __shared__ const unsigned char* grp[NT];
+  __shared__ int ng;
+  if (t == 0) {
+    int n = 0;
+    for (int q = 0; q < P; ++q)
+      if (in_group(g, q)) {
+        if (n < NT) grp[n] = g.areas[q] + g.area_off;
+        ++n;
+      }
+    ng = n;
+  }
+  __syncthreads();
+  if (ng > NT) {  // (a group of more than NT ranks: test membership per rank)
+    for (i64 oo = t; oo < nout; oo += NT) {
+      A v = Rd::neutral();
+      for (int q = 0; q < P; ++q)
+        if (in_group(g, q)) v = Rd::comb(v, ld16_cv<A>(g.areas[q] + g.area_off + (size_t)oo * 16));
+      res[oo] = Rd::finish(v);
+    }
+    return;
+  }
+  // RU outputs per thread at once: their loads from one member are independent
+  for (i64 o0 = t; o0 < nout; o0 += (i64)NT * RU) {
+    A v[RU];
+#pragma unroll
+    for (int k = 0; k < RU; ++k) v[k] = Rd::neutral();
+    for (int i = 0; i < ng; ++i) {
+      A x[RU];
+#pragma unroll
+      for (int k = 0; k < RU; ++k)
+        if (o0 + (i64)k * NT < nout) x[k] = ld16_cv<A>(grp[i] + (size_t)(o0 + (i64)k * NT) * 16);
+#pragma unroll
+      for (int k = 0; k < RU; ++k)
+        if (o0 + (i64)k * NT < nout) v[k] = Rd::comb(v[k], x[k]);
+    }
+#pragma unroll
+    for (int k = 0; k < RU; ++k)
+      if (o0 + (i64)k * NT < nout) res[o0 + (i64)k * NT] = Rd::finish(v[k]);
+  }
 }
 
 // tree over the W members of each team (sh[t] holds member t's value): member m takes m + h for
@@ -428,14 +491,13 @@ __global__ void __launch_bounds__(RT, D_CTAS_PER_SM) k_reduce_dims(const DArgs g
   }
 
   typename Rd::R* res = (typename Rd::R*)g.result;
-  if (g.nranks == 1) {
+  if (g.cb.nranks == 1) {
     if (m == 0 && o < g.nout) res[o] = Rd::finish(acc);
     return;
   }
   // P > 1: the tile's rank partials into my own area; the last tile runs the combine
-  const int P = g.nranks, me = g.rank;
   if (m == 0 && o < g.nout) {
-    st16(g.areas[me] + g.area_off + (size_t)o * 16, acc);
+    st16(g.cb.areas[g.cb.rank] + g.cb.area_off + (size_t)o * 16, acc);
     __threadfence_system();
   }
   __syncthreads();
@@ -444,54 +506,8 @@ __global__ void __launch_bounds__(RT, D_CTAS_PER_SM) k_reduce_dims(const DArgs g
   __syncthreads();
   if (!last) return;
   __threadfence_system();
-  if (t == 0) {
-    *all = 0;
-    for (int k = 1; k < P; ++k) flag_signal(g.remote_words[(me + k) % P], g.seq);
-    for (int k = 1; k < P; ++k) {  // every peer, not only the group: see DESIGN §3l
-      const int q = (me + P - k) % P;
-      flag_wait(g.local_words + (size_t)q * g.word_stride, g.seq, g.timeout_ns, g.err);
-    }
-  }
-  // the group's areas, in rank order, listed once per call (up to RT members in shared memory)
-  __shared__ const unsigned char* grp[RT];
-  __shared__ int ng;
-  if (t == 0) {
-    int n = 0;
-    for (int q = 0; q < P; ++q)
-      if (in_group(g, q)) {
-        if (n < RT) grp[n] = g.areas[q] + g.area_off;
-        ++n;
-      }
-    ng = n;
-  }
-  __syncthreads();
-  if (ng > RT) {  // (a group of more than RT ranks: test membership per rank)
-    for (i64 oo = t; oo < g.nout; oo += RT) {
-      A v = Rd::neutral();
-      for (int q = 0; q < P; ++q)
-        if (in_group(g, q)) v = Rd::comb(v, ld16_cv<A>(g.areas[q] + g.area_off + (size_t)oo * 16));
-      res[oo] = Rd::finish(v);
-    }
-    return;
-  }
-  // RU outputs per thread at once: their loads from one member are independent
-  for (i64 o0 = t; o0 < g.nout; o0 += (i64)RT * RU) {
-    A v[RU];
-#pragma unroll
-    for (int k = 0; k < RU; ++k) v[k] = Rd::neutral();
-    for (int i = 0; i < ng; ++i) {
-      A x[RU];
-#pragma unroll
-      for (int k = 0; k < RU; ++k)
-        if (o0 + (i64)k * RT < g.nout) x[k] = ld16_cv<A>(grp[i] + (size_t)(o0 + (i64)k * RT) * 16);
-#pragma unroll
-      for (int k = 0; k < RU; ++k)
-        if (o0 + (i64)k * RT < g.nout) v[k] = Rd::comb(v[k], x[k]);
-    }
-#pragma unroll
-    for (int k = 0; k < RU; ++k)
-      if (o0 + (i64)k * RT < g.nout) res[o0 + (i64)k * RT] = Rd::finish(v[k]);
-  }
+  if (t == 0) *all = 0;
+  group_combine<Rd, RT>(g.cb, g.nout, res);
 }
 
 // the NCCL fallback's second kernel: fold the P gathered partials in rank order
@@ -501,6 +517,225 @@ __global__ void k_reduce_fold(const unsigned char* slots, int P, void* result) {
   typename Rd::A acc = Rd::neutral();
   for (int q = 0; q < P; ++q) acc = Rd::comb(acc, ld16_cg<typename Rd::A>(slots + (size_t)q * 16));
   *(typename Rd::R*)result = Rd::finish(acc);
+}
+
+// ---- shell-binned spectra (pa_shell_spectrum, DESIGN §3m) ---------------------------------------
+// E(b) = sum over the modes of bin b of w * f(x).  G CTAs of ST threads own contiguous chunks of
+// 16-byte units (k_reduce's split: head, units, tail).  Each thread walks its elements with an
+// odometer over the spatial memory dims (no index tensor): its first element's coordinates by
+// division, then steps of ST * V elements added digit by digit.  Per step every lane of a warp has
+// one (bin, contribution) pair: the lanes of equal bins (__match_any_sync) are summed in lane order
+// by the lowest one, which adds the sum into the warp's histogram in shared memory (distinct bins
+// per step: no atomics).  The SW warp histograms are folded in warp order into the CTA's partial;
+// the last CTA (fence + ticket) folds the G partials in CTA order; with P > 1 the rank partial goes
+// to this rank's partial area and group_combine folds every rank's in rank order.
+constexpr int ST = 128;               // threads per CTA
+constexpr int SW = ST / 32;           // warps per CTA: one histogram each
+constexpr int S_CTAS_PER_SM = 4;      // grid cap per SM (512 threads); shared memory may allow fewer
+
+struct SArgs {
+  const void* a;
+  const void* b;
+  i64 head, tail, nunits, chunk;      // as RArgs
+  int G;
+  int vec_a, vec_b;
+  int N;                              // spatial dims
+  int ext[PA_MAX_DIMS];               // memory dim m: local extent,
+  int lo[PA_MAX_DIMS];                //   global index of the first local element,
+  int ng[PA_MAX_DIMS];                //   global extent,
+  double s[PA_MAX_DIMS];              //   scale,
+  int step[PA_MAX_DIMS];              //   digit of ST * V elements
+  int lpos[PA_MAX_DIMS];              // logical dim l is memory dim lpos[l]
+  int r2c;                            // memory dim of the r2c dim, -1: none
+  i64 rfft_n;
+  double width;
+  int nbins;
+  unsigned* ticket;
+  double* part;                       // [G][nbins]
+  GroupCombine cb;
+  void* result;
+};
+
+// coordinates (memory order) of local element i
+__device__ __forceinline__ void spec_coords(const SArgs& g, i64 i, int (&c)[PA_MAX_DIMS]) {
+#pragma unroll
+  for (int m = 0; m < PA_MAX_DIMS; ++m)
+    if (m < g.N) {
+      c[m] = (int)(i % g.ext[m]);
+      i /= g.ext[m];
+    }
+}
+// c += d (digits), the carry out of the last spatial dim dropped (extra dims do not bin)
+__device__ __forceinline__ void spec_advance(const SArgs& g, int (&c)[PA_MAX_DIMS], const int* d) {
+  int carry = 0;
+#pragma unroll
+  for (int m = 0; m < PA_MAX_DIMS; ++m)
+    if (m < g.N) {
+      c[m] += d[m] + carry;
+      carry = c[m] >= g.ext[m];
+      if (carry) c[m] -= g.ext[m];
+    }
+}
+__device__ __forceinline__ void spec_inc(const SArgs& g, int (&c)[PA_MAX_DIMS]) {
+#pragma unroll
+  for (int m = 0; m < PA_MAX_DIMS; ++m)
+    if (m < g.N) {
+      if (++c[m] < g.ext[m]) return;
+      c[m] = 0;
+    }
+}
+// the bin of the mode at c (-1: dropped) and its weight
+__device__ __forceinline__ int spec_mode(const SArgs& g, const int (&c)[PA_MAX_DIMS], int* w) {
+  double k2[PA_MAX_DIMS];
+  *w = 1;
+#pragma unroll
+  for (int m = 0; m < PA_MAX_DIMS; ++m)
+    if (m < g.N) {
+      const int i = g.lo[m] + c[m];
+      const double k = spec_k(g.s[m], spec_wavenumber(i, g.ng[m], m == g.r2c));
+      k2[m] = mul(k, k);
+      if (m == g.r2c) *w = spec_weight(i, g.rfft_n);
+    }
+  double q = 0.0;  // in logical-dim order
+#pragma unroll
+  for (int l = 0; l < PA_MAX_DIMS; ++l)
+    if (l < g.N) {
+      double v = k2[0];
+#pragma unroll
+      for (int m = 1; m < PA_MAX_DIMS; ++m)
+        if (m < g.N && g.lpos[l] == m) v = k2[m];
+      q = add(q, v);
+    }
+  return spec_bin(q, g.width, g.nbins);
+}
+
+template <class E, int M>
+__global__ void __launch_bounds__(ST, S_CTAS_PER_SM) k_spectrum(const SArgs g) {
+  using Rd = Red<E, M, O_SUM>;
+  using A = typename Rd::A;  // double
+  constexpr int V = 16 / sizeof(E);
+  extern __shared__ double hist[];  // [SW][nbins]
+  __shared__ double sv[SW][32];
+  __shared__ int last;
+  const E* a = (const E*)g.a;
+  const E* b = M == M_DOT ? (const E*)g.b : a;
+  const int t = threadIdx.x, c = blockIdx.x, lane = t & 31, wp = t >> 5;
+  const int nb = g.nbins;
+  for (int i = t; i < SW * nb; i += ST) hist[i] = 0.0;
+  __syncthreads();
+  double* h = hist + (size_t)wp * nb;
+  // one warp step: lane's (bin, contribution) into the warp's histogram
+  auto put = [&](int bin, A v) {
+    const unsigned grp = __match_any_sync(~0u, bin);
+    sv[wp][lane] = v;
+    __syncwarp();
+    if (bin >= 0 && (grp & ((1u << lane) - 1)) == 0) {
+      A sum = v;
+      for (unsigned r = grp & (grp - 1); r; r &= r - 1) sum = add(sum, sv[wp][__ffs(r) - 1]);
+      h[bin] = add(h[bin], sum);
+    }
+    __syncwarp();
+  };
+  auto contrib = [&](const E& x, const E& y, const int (&cc)[PA_MAX_DIMS], int* bin) {
+    int w;
+    *bin = spec_mode(g, cc, &w);
+    const A v = Rd::elem(x, y, typename Rd::T(), 0);
+    return w == 2 ? mul(2.0, v) : v;  // an exact doubling
+  };
+
+  int cc[PA_MAX_DIMS] = {0};
+  if (c == 0 && t < 32) {  // head: warp 0, one element per lane
+    int bin = -1;
+    A v = 0.0;
+    if (t < g.head) {
+      spec_coords(g, t, cc);
+      v = contrib(ld1(a + t), ld1(b + t), cc, &bin);
+    }
+    put(bin, v);
+  }
+  const E* ua = a + g.head;
+  const E* ub = b + g.head;
+  const i64 u0 = (i64)c * g.chunk, u1 = min(u0 + g.chunk, g.nunits);
+  if (u0 + t < u1) spec_coords(g, g.head + (u0 + t) * V, cc);
+  for (i64 ubase = u0; ubase < u1; ubase += (i64)ST * RU) {  // the same trip count in every warp
+    E xa[RU][V], xb[RU][V];
+#pragma unroll
+    for (int k = 0; k < RU; ++k) {
+      const i64 u = ubase + t + (i64)k * ST;
+      if (u < u1) {
+        ld_unit(ua + u * V, g.vec_a, xa[k]);
+        if (M == M_DOT) ld_unit(ub + u * V, g.vec_b, xb[k]);
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < RU; ++k) {
+      const bool in = ubase + t + (i64)k * ST < u1;
+      int ce[PA_MAX_DIMS];
+#pragma unroll
+      for (int m = 0; m < PA_MAX_DIMS; ++m) ce[m] = cc[m];
+#pragma unroll
+      for (int j = 0; j < V; ++j) {
+        int bin = -1;
+        A v = 0.0;
+        if (in) v = contrib(xa[k][j], M == M_DOT ? xb[k][j] : xa[k][j], ce, &bin);
+        put(bin, v);
+        if (j + 1 < V) spec_inc(g, ce);
+      }
+      if (in) spec_advance(g, cc, g.step);
+    }
+  }
+  if (c == g.G - 1 && t < 32) {  // tail: warp 0 of the last CTA
+    int bin = -1;
+    A v = 0.0;
+    if (t < g.tail) {
+      const i64 i = g.head + g.nunits * V + t;
+      spec_coords(g, i, cc);
+      v = contrib(ld1(a + i), ld1(b + i), cc, &bin);
+    }
+    put(bin, v);
+  }
+  __syncthreads();
+
+  // the CTA's partial (warps in order), then the last CTA folds the G partials in CTA order
+  for (int i = t; i < nb; i += ST) {
+    A v = hist[i];
+#pragma unroll
+    for (int w = 1; w < SW; ++w) v = add(v, hist[(size_t)w * nb + i]);
+    g.part[(size_t)c * nb + i] = v;
+  }
+  __threadfence();
+  __syncthreads();
+  if (t == 0) last = atomicAdd(g.ticket, 1u) == (unsigned)g.G - 1;
+  __syncthreads();
+  if (!last) return;
+  __threadfence();
+  if (t == 0) *g.ticket = 0;  // the next call (ordered after this one) starts from zero
+  typename Rd::R* res = (typename Rd::R*)g.result;
+  for (int i0 = t; i0 < nb; i0 += ST * RU) {  // RU bins per thread: independent loads
+    A v[RU];
+#pragma unroll
+    for (int k = 0; k < RU; ++k)
+      if (i0 + k * ST < nb) v[k] = __ldcg(g.part + i0 + k * ST);
+    for (int q = 1; q < g.G; ++q) {
+      A x[RU];
+#pragma unroll
+      for (int k = 0; k < RU; ++k)
+        if (i0 + k * ST < nb) x[k] = __ldcg(g.part + (size_t)q * nb + i0 + k * ST);
+#pragma unroll
+      for (int k = 0; k < RU; ++k)
+        if (i0 + k * ST < nb) v[k] = add(v[k], x[k]);
+    }
+#pragma unroll
+    for (int k = 0; k < RU; ++k)
+      if (i0 + k * ST < nb) {
+        if (g.cb.nranks == 1) res[i0 + k * ST] = Rd::finish(v[k]);
+        else st16(g.cb.areas[g.cb.rank] + g.cb.area_off + (size_t)(i0 + k * ST) * 16, v[k]);
+      }
+  }
+  if (g.cb.nranks == 1) return;
+  __threadfence_system();
+  __syncthreads();
+  group_combine<Rd, ST>(g.cb, nb, res);
 }
 
 // ---- state: workspace, window tables and the event serialising the calls ----------------------
@@ -513,6 +748,9 @@ struct ReduceState {
   bool tables_ready = false;
   unsigned* dtickets = nullptr;     // pa_reduce_dims: G_max + 1 tickets and G_max * RT partials,
   unsigned char* dpart = nullptr;   //   made by the first such call (stream-ordered)
+  unsigned* sticket = nullptr;      // pa_shell_spectrum: one ticket and G x nbins partials, made
+  double* spart = nullptr;          //   and grown by the calls (stream-ordered)
+  size_t spart_n = 0;
   cudaEvent_t done = nullptr;       // the previous reduction's last kernel
   ull seq = 0;
   // held from the wait on `done` to its record: host threads calling at once cannot both order
@@ -532,6 +770,8 @@ void reduce_state_destroy(ReduceState* s) {
   cudaFree(s->tables);
   cudaFree(s->dtickets);
   cudaFree(s->dpart);
+  cudaFree(s->sticket);
+  cudaFree(s->spart);
   cudaGetLastError();
   delete s;
 }
@@ -752,6 +992,22 @@ pa_status reduce(Comm* comm, int dtype, int map, int op, const void* pred_value,
   return PA_OK;
 }
 
+// the combine's arguments for a call on a communicator with a flag window; the group is every rank
+// until the caller narrows it (keep_grid)
+static void combine_args(const ReduceWindow& w, ReduceState* st, GroupCombine* cb) {
+  const int P = w.nranks;
+  cb->nranks = P;
+  cb->rank = w.rank;
+  cb->seq = ++st->seq;  // one sequence with pa_reduce: the parity sets alternate across all calls
+  cb->local_words = w.local_words;
+  cb->word_stride = w.word_stride;
+  cb->remote_words = (ull* const*)st->tables;
+  cb->areas = (unsigned char* const*)(st->tables + 2 * P);
+  cb->area_off = (size_t)(cb->seq & 1) * REDUCE_AREA_BYTES;
+  cb->timeout_ns = w.timeout_ns;
+  cb->err = w.err;
+}
+
 static i64 pow2_ceil(i64 x) {
   i64 p = 1;
   while (p < x) p <<= 1;
@@ -851,24 +1107,17 @@ pa_status reduce_dims(Comm* comm, int dtype, int map, int op, const void* pred_v
   d.tickets = st->dtickets;
   d.part = st->dpart;
   d.result = result;
-  d.nranks = P;
-  d.rank = w.rank;
   if (P > 1) {
-    d.seq = ++st->seq;  // one sequence with pa_reduce: the parity sets alternate across both
-    d.local_words = w.local_words;
-    d.word_stride = w.word_stride;
-    d.remote_words = (ull* const*)st->tables;
-    d.areas = (unsigned char* const*)(st->tables + 2 * P);
-    d.area_off = (size_t)(d.seq & 1) * REDUCE_AREA_BYTES;
-    d.topo_M = geo.topo_M;
+    combine_args(w, st, &d.cb);
+    d.cb.topo_M = geo.topo_M;
     for (int i = 0; i < geo.topo_M; ++i) {
-      d.topo_dims[i] = (int)geo.topo_dims[i];
-      d.coords[i] = (int)geo.coords[i];
+      d.cb.topo_dims[i] = (int)geo.topo_dims[i];
+      d.cb.coords[i] = (int)geo.coords[i];
     }
-    d.keep_grid = geo.keep_grid;
-    d.timeout_ns = w.timeout_ns;
-    d.err = w.err;
+    d.cb.keep_grid = geo.keep_grid;
   }
+  d.cb.nranks = P;
+  d.cb.rank = w.rank;
 
   Launch Ln;
   memset(&Ln, 0, sizeof Ln);
@@ -876,6 +1125,108 @@ pa_status reduce_dims(Comm* comm, int dtype, int map, int op, const void* pred_v
   Ln.d = &d;
   CU(cudaStreamWaitEvent(cs, st->done, 0));
   RC(dispatch(dtype, map, op, false, Ln));
+  CU(cudaEventRecord(st->done, cs));
+  return PA_OK;
+}
+
+// ---- pa_shell_spectrum ---------------------------------------------------------------------------
+template <class E, int M> static pa_status run_spectrum(const SArgs& g, size_t smem, cudaStream_t s) {
+  CU(cudaFuncSetAttribute(k_spectrum<E, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  k_spectrum<E, M><<<g.G, ST, smem, s>>>(g);
+  count_launch();
+  CU(cudaGetLastError());
+  return PA_OK;
+}
+template <class E, int M> static pa_status spectrum_occupancy(size_t smem, int* occ) {
+  CU(cudaFuncSetAttribute(k_spectrum<E, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(occ, k_spectrum<E, M>, ST, smem));
+  return PA_OK;
+}
+
+pa_status shell_spectrum(Comm* comm, int dtype, int map, const SpecGeom& sg, const void* a,
+                         const void* b, void* result, void* stream) {
+  ReduceWindow w;
+  if (comm) RC(comm_reduce_window(comm, &w));
+  const int P = w.nranks;
+  if (P > 1 && !w.flags) {
+    set_error("pa_shell_spectrum: the combine runs through the communicator's flag window, and this "
+              "communicator has none (NCCL without the window, or the nccl_fences tunable)");
+    return PA_ESTATE;
+  }
+  ReduceState* st = nullptr;
+  RC(state_of(comm, w, stream, &st));
+  std::lock_guard<std::mutex> serial(st->mu);
+  if (P > 1 && !st->tables_ready) {
+    set_error("reduction: the flag window's tables were not uploaded (pa_comm_flags_import)");
+    return PA_ESTATE;
+  }
+  const cudaStream_t cs = (cudaStream_t)stream;
+  const bool wide = dtype == D_C64, dot = map == M_DOT;
+  const size_t smem = (size_t)SW * sg.nbins * sizeof(double);
+  int occ = 0;
+  RC(wide ? (dot ? spectrum_occupancy<c64, M_DOT>(smem, &occ) : spectrum_occupancy<c64, M_ABS2>(smem, &occ))
+         : (dot ? spectrum_occupancy<c32, M_DOT>(smem, &occ) : spectrum_occupancy<c32, M_ABS2>(smem, &occ)));
+
+  SArgs g;
+  memset(&g, 0, sizeof g);
+  const int es = wide ? 16 : 8, V = 16 / es;
+  const i64 n = sg.n;
+  // k_reduce's split into head, 16-byte units and tail
+  const uintptr_t pa_ = (uintptr_t)a, pb = (uintptr_t)b;
+  const i64 head_bytes = (i64)((16 - (pa_ & 15)) & 15);
+  const bool vec = n > 0 && head_bytes % es == 0;
+  g.head = vec ? std::min<i64>(head_bytes / es, n) : 0;
+  g.nunits = (n - g.head) / V;
+  g.tail = n - g.head - g.nunits * V;
+  g.vec_a = vec;
+  g.vec_b = vec && dot && ((pb - pa_) & 15) == 0;
+  // the CTA count depends on n, nbins and the device only
+  const int sms = st->G_max / R_CTAS_PER_SM;
+  const i64 want = (n + (i64)V * ST * RU - 1) / ((i64)V * ST * RU);
+  g.G = (int)std::max<i64>(1, std::min<i64>(want, (i64)sms * std::max(1, std::min(occ, S_CTAS_PER_SM))));
+  g.chunk = (g.nunits + g.G - 1) / g.G;
+  g.a = a;
+  g.b = dot ? b : a;
+  g.N = sg.N;
+  i64 delta = (i64)ST * V;
+  for (int m = 0; m < sg.N; ++m) {
+    g.ext[m] = (int)sg.ext[m];
+    g.lo[m] = (int)sg.lo[m];
+    g.ng[m] = (int)sg.ng[m];
+    g.s[m] = sg.s[m];
+    g.lpos[m] = sg.lpos[m];
+    if (n > 0) {
+      g.step[m] = (int)(delta % sg.ext[m]);
+      delta /= sg.ext[m];
+    }
+  }
+  g.r2c = sg.r2c;
+  g.rfft_n = sg.rfft_n;
+  g.width = sg.width;
+  g.nbins = sg.nbins;
+  g.result = result;
+  if (P > 1) combine_args(w, st, &g.cb);
+  g.cb.nranks = P;
+  g.cb.rank = w.rank;
+
+  CU(cudaStreamWaitEvent(cs, st->done, 0));
+  // workspace, stream-ordered (after the previous reduction on this state, which may still use it)
+  const size_t need = (size_t)g.G * sg.nbins;
+  if (!st->sticket) {
+    CU(cudaMallocAsync((void**)&st->sticket, sizeof(unsigned), cs));
+    CU(cudaMemsetAsync(st->sticket, 0, sizeof(unsigned), cs));
+  }
+  if (st->spart_n < need) {
+    if (st->spart) CU(cudaFreeAsync(st->spart, cs));
+    st->spart = nullptr;
+    st->spart_n = 0;
+    CU(cudaMallocAsync((void**)&st->spart, need * sizeof(double), cs));
+    st->spart_n = need;
+  }
+  g.ticket = st->sticket;
+  g.part = st->spart;
+  RC(wide ? (dot ? run_spectrum<c64, M_DOT>(g, smem, cs) : run_spectrum<c64, M_ABS2>(g, smem, cs))
+         : (dot ? run_spectrum<c32, M_DOT>(g, smem, cs) : run_spectrum<c32, M_ABS2>(g, smem, cs)));
   CU(cudaEventRecord(st->done, cs));
   return PA_OK;
 }

@@ -355,5 +355,46 @@ inline int result_dtype(int dtype, int map, int op, const char** why) {
   return val;
 }
 
+// ---- shell-binned spectra (pa_shell_spectrum, DESIGN §3m) ---------------------------------------
+// The one place that knows the geometry of a spectrum; the kernel, the default bin count and the
+// CPU check (tests/spectrum_host_check.cpp) all call these.  Every floating operation is one
+// correctly rounded IEEE operation, so a mode's bin is bit for bit what NumPy computes.
+RHD double sqrt_rn(double x) {
+#ifdef __CUDA_ARCH__
+  return __dsqrt_rn(x);
+#else
+  return sqrt(x);
+#endif
+}
+RHD double div_rn(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __ddiv_rn(a, b);
+#else
+  return a / b;
+#endif
+}
+
+// integer wavenumber of global index i along a dim of global extent n (numpy's fftfreq order);
+// along the r2c dim the index is the wavenumber
+RHD long long spec_wavenumber(long long i, long long n, bool r2c) {
+  return r2c || i < (n + 1) / 2 ? i : i - n;
+}
+// Hermitian weight along the r2c dim of a real length n: 1 at i = 0 and (n even) i = n / 2, else 2
+RHD int spec_weight(long long i, long long n) {
+  return i == 0 || (n % 2 == 0 && i == n / 2) ? 1 : 2;
+}
+// k_d = s_d * wavenumber, and its square (the term of q)
+RHD double spec_k(double s, long long nt) { return mul(s, (double)nt); }
+// the shell of q = k_1^2 + k_2^2 + ... (summed in logical-dim order): floor(sqrt(q) / width + 0.5)
+// as a double (it may exceed every integer type); width == 1 divides exactly
+RHD double spec_shell(double q, double width) {
+  return floor(add(div_rn(sqrt_rn(q), width), 0.5));
+}
+// the bin of a mode, or -1 when it is at or beyond nbins
+RHD int spec_bin(double q, double width, int nbins) {
+  const double b = spec_shell(q, width);
+  return b < (double)nbins ? (int)b : -1;
+}
+
 }  // namespace red
 }  // namespace pa

@@ -753,4 +753,41 @@ function mapreduce_dims(f::F, op::OP, u::CuPencilArray{T}, etc::Vararg{CuPencilA
     result
 end
 
+# ---- shell-binned spectra (pa_shell_spectrum, DESIGN §3m) ----------------------------------------
+# shell_spectrum(abs2, û; ...) and shell_spectrum(realdot, û, v̂; ...): E(b) = Σ over the modes
+# with bin(|k|) == b of w · abs2(û) (or w · real(û · conj(v̂))), the global spectrum as a CuVector
+# of nbins values (Float64, or Float32 for ComplexF32 arrays), the same bits on every rank.
+# rfft_dim: the logical dim holding the n ÷ 2 + 1 bins of a real-to-complex transform of length
+# rfft_n (default 2 (M - 1)); scales: one per spatial dim (2π / L_d; default 1); width: the shell
+# width; nbins: default the bin of the extreme mode plus one (pa_shell_spectrum_nbins).
+function shell_spectrum(f::F, u::CuPencilArray{T}, etc::Vararg{CuPencilArray{T}};
+                        rfft_dim::Integer = 0, rfft_n::Integer = 0, scales = nothing,
+                        width::Real = 1.0, nbins = nothing) where {F,T<:Union{ComplexF64,ComplexF32}}
+    length(etc) <= 1 || throw(ArgumentError("shell_spectrum takes one or two arrays"))
+    v = isempty(etc) ? nothing : etc[1]
+    v === nothing || PencilArrays._check_compatible_arrays(u, v)
+    map = pa_map(f)
+    (map == 2 && v === nothing) || (map == 3 && v !== nothing) ||
+        throw(ArgumentError("shell_spectrum: abs2 of one array or realdot of two, not $f"))
+    H = handles(topology(pencil(u)))
+    N = ndims(pencil(u))
+    sc = scales === nothing ? C_NULL : Float64[s for s in scales]
+    sc === C_NULL || length(sc) == N || throw(ArgumentError("shell_spectrum: one scale per dim"))
+    nb = Ref{Cint}()
+    GC.@preserve sc check(ccall((:pa_shell_spectrum_nbins, libpa), Cint,
+        (Ptr{Cvoid}, Cint, Int64, Ptr{Float64}, Cdouble, Ptr{Cint}),
+        pencil_handle(H, pencil(u)), rfft_dim, rfft_n, sc, width, nb))
+    n = nbins === nothing ? Int(nb[]) : Int(nbins)
+    result = CuVector{real(T)}(undef, max(n, 1))
+    ex = Int64[extra_dims(u)...]
+    ptr_or_null(A) = isempty(A) ? C_NULL : devptr(A)
+    GC.@preserve sc check(ccall((:pa_shell_spectrum, libpa), Cint,
+        (Ptr{Cvoid}, Cint, Ptr{Int64}, Ptr{Cvoid}, Cint, Cint, Ptr{Cvoid}, Ptr{Cvoid}, Cint, Int64,
+         Ptr{Float64}, Cdouble, Cint, Ptr{Cvoid}, Ptr{Cvoid}),
+        pencil_handle(H, pencil(u)), length(ex), ex, H.comm, PA_DTYPE[T], map,
+        ptr_or_null(parent(u)), v === nothing ? C_NULL : ptr_or_null(parent(v)), rfft_dim, rfft_n,
+        sc, width, n, devptr(result), stream_ptr()))
+    result
+end
+
 end # module

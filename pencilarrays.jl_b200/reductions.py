@@ -203,3 +203,81 @@ def any(u: PencilArray, pred, value=None, f=None, dims=None):
 def all(u: PencilArray, pred, value=None, f=None, dims=None):
     """``all(x -> pred(f(x), value), u; dims)``, e.g. ``all(u, "isfinite")``."""
     return _pred(_lib.PA_OP_ALL, u, pred, value, f, dims)
+
+
+def _spectrum_geometry(u: PencilArray, rfft_dim, rfft_n, scales, width):
+    N = len(u.space_dims)
+    rd = 0 if rfft_dim is None else rfft_dim
+    if not isinstance(rd, int) or isinstance(rd, bool):
+        raise ArgumentError(_lib.PA_EINVAL, f"rfft_dim {rfft_dim!r} is not a dim")
+    rn = 0 if rfft_n is None else rfft_n
+    if not isinstance(rn, int) or isinstance(rn, bool):
+        raise ArgumentError(_lib.PA_EINVAL, f"rfft_n {rfft_n!r} is not an integer")
+    sc = None
+    if scales is not None:
+        try:
+            sc = tuple(float(x) for x in scales)
+        except (TypeError, ValueError):
+            raise ArgumentError(_lib.PA_EINVAL, f"scales {scales!r} are not {N} numbers") from None
+        if len(sc) != N:
+            raise ArgumentError(_lib.PA_EINVAL, f"scales {scales!r}: one per spatial dim ({N})")
+        sc = (C.c_double * N)(*sc)
+    try:
+        width = float(width)
+    except (TypeError, ValueError):
+        raise ArgumentError(_lib.PA_EINVAL, f"width {width!r} is not a number") from None
+    return rd, rn, sc, width
+
+
+def spectrum_nbins(u: PencilArray, *, rfft_dim=None, rfft_n=None, scales=None, width=1.0):
+    """The default bin count of :func:`shell_spectrum`: the bin of the extreme mode plus one, as
+    the library computes it (``pa_shell_spectrum_nbins``)."""
+    rd, rn, sc, width = _spectrum_geometry(u, rfft_dim, rfft_n, scales, width)
+    out = C.c_int()
+    check(lib.pa_shell_spectrum_nbins(u.pencil._h, rd, rn, sc, width, C.byref(out)))
+    return out.value
+
+
+def shell_spectrum(u: PencilArray, v: PencilArray = None, *, rfft_dim=None, rfft_n=None,
+                   scales=None, width=1.0, nbins=None):
+    """Shell-binned spectrum ``E(b) = sum over bin(|k|) == b of w * abs2(u)`` (with ``v``: of
+    ``w * real(u * conj(v))``, a co-spectrum) of complex arrays whose spatial dims hold the modes
+    of an unnormalised DFT (``pa_shell_spectrum``, DESIGN §3m).  ``rfft_dim``: the 1-based logical
+    dim holding the ``n // 2 + 1`` bins of a real-to-complex transform of length ``rfft_n``
+    (default ``2 (M - 1)``), whose interior bins count twice; ``scales``: one wavenumber scale per
+    spatial dim (``2 pi / L``; default 1); ``width``: the shell width; ``nbins``: default
+    :func:`spectrum_nbins`.  Extra dims add into the same bins.  Returns the global spectrum (the
+    same bits on every rank), a 1-d tensor of ``nbins`` float64 (float32 for complex64 arrays) on
+    ``u``'s device, computed on torch's current stream in one kernel per rank."""
+    if not isinstance(u, PencilArray):
+        raise ArgumentError(_lib.PA_EINVAL, "shell_spectrum takes PencilArrays")
+    if v is not None:
+        if not isinstance(v, PencilArray) or v.pencil is not u.pencil:
+            raise ArgumentError(_lib.PA_EINVAL, "arrays are not compatible: not on the same pencil")
+        if v.extra_dims != u.extra_dims:
+            raise ArgumentError(_lib.PA_EINVAL, "arrays are not compatible: extra dims "
+                                f"{v.extra_dims} != {u.extra_dims}")
+        if v.dtype != u.dtype:
+            raise ArgumentError(_lib.PA_EINVAL, f"arrays are not compatible: {v.dtype} != {u.dtype}")
+    if u.dtype not in _REAL:
+        raise ArgumentError(_lib.PA_EINVAL, f"a spectrum is of complex arrays, not {u.dtype}")
+    rd, rn, sc, width = _spectrum_geometry(u, rfft_dim, rfft_n, scales, width)
+    out = C.c_int()  # (the geometry's checks, before anything is allocated)
+    check(lib.pa_shell_spectrum_nbins(u.pencil._h, rd, rn, sc, width, C.byref(out)))
+    if nbins is None:
+        nbins = out.value
+    if not isinstance(nbins, int) or isinstance(nbins, bool) or \
+            not 1 <= nbins <= _lib.PA_SPECTRUM_MAX_BINS:
+        raise ArgumentError(_lib.PA_EINVAL, f"pa_shell_spectrum: nbins {nbins!r} out of range "
+                            f"1..{_lib.PA_SPECTRUM_MAX_BINS}")
+    code_map = _lib.PA_MAP_ABS2 if v is None else _lib.PA_MAP_DOT
+    dt = _DTYPES[u.dtype]
+    result = torch.empty(nbins, dtype=_REAL[u.dtype], device=u.data.device)
+    ex = u.extra_dims
+    with torch.cuda.device(u.data.device):
+        check(lib.pa_shell_spectrum(u.pencil._h, len(ex), i64arr(ex), u.pencil.topology.comm.handle,
+                                    dt, code_map, C.c_void_p(u.data_ptr() or None),
+                                    C.c_void_p(v.data_ptr() or None) if v is not None else None,
+                                    rd, rn, sc, width, nbins, C.c_void_p(result.data_ptr() or None),
+                                    _stream_ptr()))
+    return result
