@@ -665,6 +665,49 @@ pa_status pa_shell_spectrum(const pa_pencil* pencil, int n_extra, const int64_t*
 pa_status pa_shell_spectrum_nbins(const pa_pencil* pencil, int rfft_dim, int64_t rfft_n,
                                   const double* scales, double width, int* nbins);
 
+/* The spectrum of pa_shell_spectrum over chosen dims, each logical dim given one role (DESIGN §3n):
+ *   bin dims   bin_dims[0 .. n_bin-1]: 1-based SPATIAL dims (at least one, no repeats); |k| is formed
+ *              from these only (q summed over them in logical-dim order, every operation one
+ *              correctly rounded fp64 operation as in pa_shell_spectrum);
+ *   kept dims  keep_dims[0 .. n_keep-1]: 1-based logical dims (1..N spatial, N+1..N+n_extra extra),
+ *              none of them a bin dim, no repeats (n_keep 0: none); each rank gets its local range;
+ *   every other dim, spatial or extra, is summed into the bins.
+ * The wavenumbers, weights and bins are pa_shell_spectrum's, whatever role the r2c dim has: along a
+ * kept r2c dim index i holds modes i and -i together (weight 2 in the interior), so the sum over
+ * the bins and over the kept indices of every rank is Parseval's total.  scales: one per spatial
+ * dim (all checked, only the bin dims' used).  `result` receives, as pa_reduce_result_type(dtype,
+ * map, PA_OP_SUM) values, result[b + nbins * o]: o the column-major index over the local extents of
+ * the kept dims in the parent's memory order (extra dims last), as in pa_reduce_dims' result.  A
+ * rank combines with the ranks whose grid coordinates agree with its own on every grid dim that
+ * decomposes a kept dim, folding their partials in rank order; every member gets the same bits
+ * (with no kept dim decomposed: every rank).  Every spatial dim binned and nothing kept is
+ * pa_shell_spectrum, bit for bit.  ONE kernel per rank and call, ordered on `stream`, collective
+ * over the communicator (ranks owning nothing take part), the host is not synchronised; shares
+ * pa_reduce's serialisation.  Refused on the host, in this order, identically on every rank (error
+ * texts start with "pa_shell_spectrum_dims:"), PA_EINVAL: a NULL pencil; dtype not complex or map
+ * not PA_MAP_ABS2 / PA_MAP_DOT; `b` given for PA_MAP_ABS2 or missing for PA_MAP_DOT; bad extra
+ * dims; bad bin dims (none, NULL, outside 1..N, or one given twice); bad kept dims (n_keep < 0, NULL
+ * with n_keep > 0, outside 1..N+n_extra, given twice, or a bin dim); rfft_dim outside 0..N; rfft_n
+ * inconsistent with the r2c dim; a scale or the width not finite and positive; nbins outside
+ * 1..PA_SPECTRUM_MAX_BINS; NULL arrays for a non-empty local array; arrays not aligned to their
+ * real component; `result` NULL (allowed when the local result is empty) or not aligned to the
+ * result type; with more than one rank, nbins x the kept outputs of the rank with the most above
+ * the flag window's partial area (524288 accumulators), decided from the global geometry.
+ * PA_EINCOMPAT: the topology's rank count is not the communicator's (or comm == NULL with more than
+ * one rank).  Then without a device PA_ENOGPU.  PA_ESTATE: more than one rank on a communicator
+ * without a flag window.                                                                          */
+pa_status pa_shell_spectrum_dims(const pa_pencil* pencil, int n_extra, const int64_t* extra_dims,
+                                 pa_comm* comm, int dtype, int map, const void* a, const void* b,
+                                 int rfft_dim, int64_t rfft_n, const double* scales, double width,
+                                 int nbins, int n_bin, const int* bin_dims, int n_keep,
+                                 const int* keep_dims, void* result, void* stream);
+/* The default nbins of pa_shell_spectrum_dims: the bin of the extreme mode over the bin dims plus
+ * one.  Refused (texts start with "pa_shell_spectrum_dims:") for a NULL pencil, bad bin dims, then
+ * pa_shell_spectrum_nbins' checks.  Host-only.                                                    */
+pa_status pa_shell_spectrum_dims_nbins(const pa_pencil* pencil, int rfft_dim, int64_t rfft_n,
+                                       const double* scales, double width, int n_bin,
+                                       const int* bin_dims, int* nbins);
+
 /* ---- host chains -----------------------------------------------------------
  * A sequence of transpositions applied to HOST arrays (plan i+1 consumes what
  * plan i produces): one submit = upload of `host_src`, every transpose! on the

@@ -175,6 +175,11 @@ SIGNATURES = {
     "pa_shell_spectrum": (C.c_int, [_P, C.c_int, _I64P, _P, C.c_int, C.c_int, _P, _P, C.c_int,
                                     C.c_int64, _P, C.c_double, C.c_int, _P, _P]),
     "pa_shell_spectrum_nbins": (C.c_int, [_P, C.c_int, C.c_int64, _P, C.c_double, _IP]),
+    "pa_shell_spectrum_dims": (C.c_int, [_P, C.c_int, _I64P, _P, C.c_int, C.c_int, _P, _P, C.c_int,
+                                         C.c_int64, _P, C.c_double, C.c_int, C.c_int, _IP, C.c_int,
+                                         _IP, _P, _P]),
+    "pa_shell_spectrum_dims_nbins": (C.c_int, [_P, C.c_int, C.c_int64, _P, C.c_double, C.c_int, _IP,
+                                               _IP]),
     "pa_plan_timings": (C.c_int, [_P, C.POINTER(Timings)]),
     "pa_plan_enable_timing": (C.c_int, [_P, C.c_int]),
 }

@@ -1509,9 +1509,8 @@ pa_status pa_reduce_dims(const pa_pencil* pencil, int n_extra, const int64_t* ex
 // ---- shell-binned spectra ------------------------------------------------------------------------
 // The geometry checks shared by pa_shell_spectrum and pa_shell_spectrum_nbins, in the header's
 // order from rfft_dim on; *n_real = the r2c dim's real length.  Every message starts with `who`.
-static pa_status spectrum_geometry(const Pencil& Pn, int rfft_dim, int64_t rfft_n,
+static pa_status spectrum_geometry(const char* who, const Pencil& Pn, int rfft_dim, int64_t rfft_n,
                                    const double* scales, double width, i64* n_real) {
-  const char* who = "pa_shell_spectrum";
   if (rfft_dim < 0 || rfft_dim > Pn.N) {
     set_error("%s: rfft_dim %d out of range 0..%d (0: no r2c dim)", who, rfft_dim, Pn.N);
     return PA_EINVAL;
@@ -1544,45 +1543,83 @@ static pa_status spectrum_geometry(const Pencil& Pn, int rfft_dim, int64_t rfft_
   return PA_OK;
 }
 
-// the bin of the extreme mode plus one: |k| grows with every |wavenumber|, so the corner of the
-// largest |wavenumber| along each dim holds the last bin (every dim of extent 0 or 1 adds 0)
-static i64 spectrum_default_bins(const Pencil& Pn, int rfft_dim, const double* scales, double width) {
-  double q = 0.0;
-  for (int d = 0; d < Pn.N; ++d) {
-    const i64 n = Pn.size_global[d];
-    const i64 top = n == 0 ? 0 : d + 1 == rfft_dim ? n - 1 : n / 2;
-    const double k = red::spec_k(scales ? scales[d] : 1.0, top);
-    q = red::add(q, red::mul(k, k));
+// the bin of the extreme mode plus one over the bin dims (reduce_core.hpp)
+static i64 spectrum_default_bins(const Pencil& Pn, int rfft_dim, const double* scales, double width,
+                                 unsigned mask) {
+  long long n[PA_MAX_DIMS] = {0};
+  for (int d = 0; d < Pn.N; ++d) n[d] = Pn.size_global[d];
+  return red::spec_default_bins(Pn.N, n, rfft_dim, scales, width, mask);
+}
+
+// pa_shell_spectrum_dims: the bin dims (1-based spatial dims, at least one, no repeats) as a mask
+static pa_status bin_mask(const char* who, int N, int n_bin, const int* bin_dims, unsigned* mask) {
+  if (n_bin < 1 || !bin_dims) {
+    set_error("%s: `dims` must name at least one bin dim", who);
+    return PA_EINVAL;
   }
-  const double b = red::spec_shell(q, width);
-  return b + 1.0 > (double)INT32_MAX ? (i64)INT32_MAX + 1 : (i64)b + 1;
+  *mask = 0;
+  for (int i = 0; i < n_bin; ++i) {
+    const int d = bin_dims[i];
+    if (d < 1 || d > N) {
+      set_error("%s: bin dim %d out of range 1..%d (the spatial dims)", who, d, N);
+      return PA_EINVAL;
+    }
+    if ((*mask >> (d - 1)) & 1) {
+      set_error("%s: bin dim %d given twice", who, d);
+      return PA_EINVAL;
+    }
+    *mask |= 1u << (d - 1);
+  }
+  return PA_OK;
+}
+
+static pa_status spectrum_nbins(const char* who, const pa_pencil* pencil, int rfft_dim,
+                                int64_t rfft_n, const double* scales, double width, int n_bin,
+                                const int* bin_dims, int* nbins) {
+  if (!pencil) {
+    set_error("%s: null pencil", who);
+    return PA_EINVAL;
+  }
+  const Pencil& Pn = *pencil->p;
+  unsigned mask = (1u << Pn.N) - 1;
+  if (n_bin >= 0) RC(bin_mask(who, Pn.N, n_bin, bin_dims, &mask));
+  i64 n_real = 0;
+  RC(spectrum_geometry(who, Pn, rfft_dim, rfft_n, scales, width, &n_real));
+  const i64 b = spectrum_default_bins(Pn, rfft_dim, scales, width, mask);
+  if (b > INT32_MAX) {
+    set_error("%s: the extreme mode's bin does not fit an int", who);
+    return PA_EINVAL;
+  }
+  if (nbins) *nbins = (int)b;
+  return PA_OK;
 }
 
 pa_status pa_shell_spectrum_nbins(const pa_pencil* pencil, int rfft_dim, int64_t rfft_n,
                                   const double* scales, double width, int* nbins) {
   GUARD({
-    if (!pencil) {
-      set_error("pa_shell_spectrum: null pencil");
-      return PA_EINVAL;
-    }
-    i64 n_real = 0;
-    RC(spectrum_geometry(*pencil->p, rfft_dim, rfft_n, scales, width, &n_real));
-    const i64 b = spectrum_default_bins(*pencil->p, rfft_dim, scales, width);
-    if (b > INT32_MAX) {
-      set_error("pa_shell_spectrum: the extreme mode's bin does not fit an int");
-      return PA_EINVAL;
-    }
-    if (nbins) *nbins = (int)b;
-    return PA_OK;
+    return spectrum_nbins("pa_shell_spectrum", pencil, rfft_dim, rfft_n, scales, width, -1, nullptr,
+                          nbins);
   })
 }
 
-// pa_shell_spectrum: every check in the order of pa_b200.h, then the kernel
+pa_status pa_shell_spectrum_dims_nbins(const pa_pencil* pencil, int rfft_dim, int64_t rfft_n,
+                                       const double* scales, double width, int n_bin,
+                                       const int* bin_dims, int* nbins) {
+  GUARD({
+    return spectrum_nbins("pa_shell_spectrum_dims", pencil, rfft_dim, rfft_n, scales, width, n_bin,
+                          bin_dims, nbins);
+  })
+}
+
+// pa_shell_spectrum (n_bin < 0: every spatial dim binned, nothing kept) and pa_shell_spectrum_dims:
+// every check in the order of pa_b200.h, then the kernel
 static pa_status spectrum_call(const pa_pencil* pencil, int n_extra, const int64_t* extra_dims,
                                pa_comm* comm, int dtype, int map, const void* a, const void* b,
                                int rfft_dim, int64_t rfft_n, const double* scales, double width,
-                               int nbins, void* result, void* stream) {
-  const char* who = "pa_shell_spectrum";
+                               int nbins, int n_bin, const int* bin_dims, int n_keep,
+                               const int* keep_dims, void* result, void* stream) {
+  const bool sub = n_bin >= 0;
+  const char* who = sub ? "pa_shell_spectrum_dims" : "pa_shell_spectrum";
   if (!pencil) {
     set_error("%s: null pencil", who);
     return PA_EINVAL;
@@ -1608,7 +1645,8 @@ static pa_status spectrum_call(const pa_pencil* pencil, int n_extra, const int64
               PA_MAX_DIMS);
     return PA_EINVAL;
   }
-  SpecGeom g;
+  SpecDimsGeom G;
+  SpecGeom& g = G.sp;
   g.n = n_spatial;
   for (int i = 0; i < n_extra; ++i) {
     if (extra_dims[i] < 0) {
@@ -1617,7 +1655,35 @@ static pa_status spectrum_call(const pa_pencil* pencil, int n_extra, const int64
     }
     g.n *= extra_dims[i];
   }
-  RC(spectrum_geometry(Pn, rfft_dim, rfft_n, scales, width, &g.rfft_n));
+  // the roles: bin dims (spatial), kept dims (any), the rest summed
+  const int nl = Pn.N + n_extra;
+  G.bin_mask = (1u << Pn.N) - 1;
+  unsigned keep = 0;
+  if (sub) {
+    RC(bin_mask(who, Pn.N, n_bin, bin_dims, &G.bin_mask));
+    if (n_keep < 0 || (n_keep > 0 && !keep_dims)) {
+      set_error("%s: %d kept dims%s", who, n_keep, n_keep < 0 ? "" : " and no `keep_dims`");
+      return PA_EINVAL;
+    }
+    for (int i = 0; i < n_keep; ++i) {
+      const int d = keep_dims[i];
+      if (d < 1 || d > nl) {
+        set_error("%s: kept dim %d out of range 1..%d (%d spatial dims, then %d extra)", who, d, nl,
+                  Pn.N, n_extra);
+        return PA_EINVAL;
+      }
+      if ((keep >> (d - 1)) & 1) {
+        set_error("%s: kept dim %d given twice", who, d);
+        return PA_EINVAL;
+      }
+      if ((G.bin_mask >> (d - 1)) & 1) {
+        set_error("%s: dim %d is both a bin dim and a kept dim", who, d);
+        return PA_EINVAL;
+      }
+      keep |= 1u << (d - 1);
+    }
+  }
+  RC(spectrum_geometry(who, Pn, rfft_dim, rfft_n, scales, width, &g.rfft_n));
   if (nbins < 1 || nbins > PA_SPECTRUM_MAX_BINS) {
     set_error("%s: nbins %d out of range 1..%d", who, nbins, PA_SPECTRUM_MAX_BINS);
     return PA_EINVAL;
@@ -1631,12 +1697,24 @@ static pa_status spectrum_call(const pa_pencil* pencil, int n_extra, const int64
     set_error("%s: arrays must be aligned to %d bytes (their real component)", who, (int)al);
     return PA_EINVAL;
   }
+  // the layout and the group of pa_reduce_dims with every unkept dim reduced (never none: a bin dim)
+  int red[PA_MAX_DIMS], nred = 0;
+  for (int l = 0; l < nl; ++l)
+    if (!((keep >> l) & 1)) red[nred++] = l + 1;
+  i64 nred_global = 0, nout_max = 0;
+  RC(dims_geom(Pn, n_extra, extra_dims, nred, red, &G.dg, &G.nout, &nred_global, &nout_max));
   const uintptr_t ral = dtype == PA_COMPLEXF64 ? 8 : 4;
-  if (!result || (uintptr_t)result % ral) {
+  if ((!result && G.nout > 0) || (uintptr_t)result % ral) {  // (an empty local result: may be NULL)
     set_error("%s: `result` must be a device pointer aligned to %d bytes", who, (int)ral);
     return PA_EINVAL;
   }
   const int nranks = Pn.topo->size;
+  if (nranks > 1 && nout_max * nbins * REDUCE_SLOT_BYTES > (i64)REDUCE_AREA_BYTES) {
+    set_error("%s: a rank's partial result of %lld bins x %lld kept outputs exceeds the flag window's "
+              "partial area (%lld 16-byte accumulators)", who, (long long)nbins, (long long)nout_max,
+              (long long)(REDUCE_AREA_BYTES / REDUCE_SLOT_BYTES));
+    return PA_EINVAL;
+  }
   if (comm ? comm_size(comm->p) != nranks : nranks > 1) {
     set_error(comm ? "%s: the topology has %d ranks, the communicator %d"
                    : "%s: a topology of %d ranks needs a communicator", who, nranks,
@@ -1656,7 +1734,9 @@ static pa_status spectrum_call(const pa_pencil* pencil, int n_extra, const int64
   }
   g.width = width;
   g.nbins = nbins;
-  return shell_spectrum(comm ? comm->p : nullptr, dtype, map, g, a, b, result, stream);
+  if (keep == 0 && G.bin_mask == (1u << Pn.N) - 1)  // every spatial dim binned: pa_shell_spectrum
+    return shell_spectrum(comm ? comm->p : nullptr, dtype, map, g, a, b, result, stream);
+  return shell_spectrum_dims(comm ? comm->p : nullptr, dtype, map, G, a, b, result, stream);
 }
 
 pa_status pa_shell_spectrum(const pa_pencil* pencil, int n_extra, const int64_t* extra_dims,
@@ -1665,7 +1745,19 @@ pa_status pa_shell_spectrum(const pa_pencil* pencil, int n_extra, const int64_t*
                             int nbins, void* result, void* stream) {
   GUARD({
     return spectrum_call(pencil, n_extra, extra_dims, comm, dtype, map, a, b, rfft_dim, rfft_n,
-                         scales, width, nbins, result, stream);
+                         scales, width, nbins, -1, nullptr, 0, nullptr, result, stream);
+  })
+}
+
+pa_status pa_shell_spectrum_dims(const pa_pencil* pencil, int n_extra, const int64_t* extra_dims,
+                                 pa_comm* comm, int dtype, int map, const void* a, const void* b,
+                                 int rfft_dim, int64_t rfft_n, const double* scales, double width,
+                                 int nbins, int n_bin, const int* bin_dims, int n_keep,
+                                 const int* keep_dims, void* result, void* stream) {
+  GUARD({
+    return spectrum_call(pencil, n_extra, extra_dims, comm, dtype, map, a, b, rfft_dim, rfft_n,
+                         scales, width, nbins, std::max(n_bin, 0), bin_dims, n_keep, keep_dims,
+                         result, stream);
   })
 }
 

@@ -320,6 +320,18 @@ struct SpecGeom {
 pa_status shell_spectrum(Comm* comm, int dtype, int map, const SpecGeom& geo, const void* a,
                          const void* b, void* result, void* stream);
 
+// pa_shell_spectrum_dims' geometry, checked by capi.cpp: the spatial geometry of SpecGeom; every
+// dim of the parent in memory order (extra dims last) with its local extent, red[m] false for the
+// kept dims, and the combine group (DimsGeom); the bin dims (bit l: logical dim l + 1)
+struct SpecDimsGeom {
+  SpecGeom sp;
+  DimsGeom dg;
+  unsigned bin_mask = 0;
+  i64 nout = 0;  // the local kept outputs (product of the kept dims' local extents)
+};
+pa_status shell_spectrum_dims(Comm* comm, int dtype, int map, const SpecDimsGeom& geo,
+                              const void* a, const void* b, void* result, void* stream);
+
 // What a fused line kernel computes: from the lines it gathers on the receive side of a
 // transposition (unpack_fused, get_fft) or from the source lines it loads on the send side
 // (put_fft).  A plan moves the elements of one side; the array on the other side of the transform

@@ -738,6 +738,251 @@ __global__ void __launch_bounds__(ST, S_CTAS_PER_SM) k_spectrum(const SArgs g) {
   group_combine<Rd, ST>(g.cb, nb, res);
 }
 
+// ---- spectra over chosen dims (pa_shell_spectrum_dims, DESIGN §3n) ------------------------------
+// Every dim of the parent (memory order, extra dims last) is kept, binned or summed.  Output o
+// (column-major over the kept dims' local extents) owns the slab of the other dims: nslab items j
+// (column-major over the slab dims).  A CTA owns a tile of Kc consecutive outputs and a split of
+// its slab (S splits of jchunk items); lane = kc + Kc * r takes output kc of the tile and items
+// j = J0 + r + Rw * (warp + SW * step), Rw = 32 / Kc.  Kc = 1 unless the fastest memory dim is kept:
+// then Kc consecutive kept indices are consecutive elements and the lanes' loads coalesce.  Each
+// warp bins into its own histogram of Kc x nbins doubles with k_spectrum's match / lane-order step
+// (key kc * nbins + bin; a key held by all 32 lanes is summed by a shuffle tree instead of the
+// lane-order chain: a bin dim slow in memory keeps one bin over long runs of items), the warps are folded in warp order, the S splits of a tile in split order by
+// the tile's last CTA (fence + ticket); with P > 1 every tile's rank partial goes to the partial
+// area and the last tile (a second ticket) runs group_combine.
+constexpr int SD_KC = 8;                         // most outputs per tile (8 x 16 bytes: a line)
+constexpr size_t SD_SMEM = 48u << 10;            // warp histograms at Kc > 1: 4 CTAs per SM
+
+struct SDArgs {
+  const void* a;
+  const void* b;
+  int vec;                            // whole-element loads (the bases aligned to the element)
+  int nd, N;                          // memory dims (extra dims included); spatial dims
+  int kept[PA_MAX_DIMS];              // memory dim m: kept (1) or in the slab (0),
+  int ext[PA_MAX_DIMS];               //   local extent,
+  i64 str[PA_MAX_DIMS];               //   element stride,
+  int sstep[PA_MAX_DIMS];             //   digit of Rw * SW slab items (0 for kept dims)
+  int lo[PA_MAX_DIMS];                // spatial memory dim m: global index of the first local element,
+  int ng[PA_MAX_DIMS];                //   global extent,
+  double s[PA_MAX_DIMS];              //   scale
+  int lpos[PA_MAX_DIMS];              // logical dim l is memory dim lpos[l]
+  unsigned mask;                      // bin dims (logical)
+  int r2c;                            // memory dim of the r2c dim, -1: none
+  i64 rfft_n;
+  double width;
+  int nbins, Kc, Rw, S;
+  i64 nout, nslab, jchunk, tiles;
+  unsigned* tickets;                  // [tiles] when S > 1, then the all-tiles ticket
+  double* part;                       // [tiles][S][Kc * nbins] when S > 1
+  GroupCombine cb;
+  void* result;
+};
+
+__device__ __forceinline__ c64 ld_elem(const c64* p, bool vec) {
+  if (vec) {
+    const double2 w = __ldcs((const double2*)p);
+    return c64{w.x, w.y};
+  }
+  return ld1(p);
+}
+__device__ __forceinline__ c32 ld_elem(const c32* p, bool vec) {
+  if (vec) {
+    const float2 w = __ldcs((const float2*)p);
+    return c32{w.x, w.y};
+  }
+  return ld1(p);
+}
+
+// c += the slab digits d (kept dims skipped), *off updated; the carry out of the last dim dropped
+__device__ __forceinline__ void sd_advance(const SDArgs& g, int (&c)[PA_MAX_DIMS], i64* off) {
+  int carry = 0;
+#pragma unroll
+  for (int m = 0; m < PA_MAX_DIMS; ++m)
+    if (m < g.nd && !g.kept[m]) {
+      const int d = g.sstep[m] + carry;
+      c[m] += d;
+      *off += (i64)d * g.str[m];
+      carry = c[m] >= g.ext[m];
+      if (carry) {
+        c[m] -= g.ext[m];
+        *off -= (i64)g.ext[m] * g.str[m];
+      }
+    }
+}
+// the bin of the mode at c (-1: dropped) and its weight; only the bin dims enter q
+__device__ __forceinline__ int sd_mode(const SDArgs& g, const int (&c)[PA_MAX_DIMS], int* w) {
+  double km[PA_MAX_DIMS], k[PA_MAX_DIMS];
+  *w = 1;
+#pragma unroll
+  for (int m = 0; m < PA_MAX_DIMS; ++m)
+    if (m < g.N) {
+      const int i = g.lo[m] + c[m];
+      km[m] = spec_k(g.s[m], spec_wavenumber(i, g.ng[m], m == g.r2c));
+      if (m == g.r2c) *w = spec_weight(i, g.rfft_n);
+    }
+#pragma unroll
+  for (int l = 0; l < PA_MAX_DIMS; ++l)
+    if (l < g.N) {
+      double v = km[0];
+#pragma unroll
+      for (int m = 1; m < PA_MAX_DIMS; ++m)
+        if (m < g.N && g.lpos[l] == m) v = km[m];
+      k[l] = v;
+    } else {
+      k[l] = 0.0;
+    }
+  return spec_bin(spec_q(g.N, k, g.mask), g.width, g.nbins);
+}
+
+template <class E, int M>
+__global__ void __launch_bounds__(ST, S_CTAS_PER_SM) k_spectrum_dims(const SDArgs g) {
+  using Rd = Red<E, M, O_SUM>;
+  using A = typename Rd::A;  // double
+  extern __shared__ double hist[];  // [SW][Kc * nbins]
+  __shared__ double sv[SW][32];
+  __shared__ int last;
+  const E* a = (const E*)g.a;
+  const E* b = M == M_DOT ? (const E*)g.b : a;
+  const int t = threadIdx.x, lane = t & 31, wp = t >> 5;
+  const int nb = g.nbins, KN = g.Kc * nb;
+  const i64 tile = blockIdx.x / g.S;
+  const int s = blockIdx.x % g.S;
+  for (int i = t; i < SW * KN; i += ST) hist[i] = 0.0;
+  __syncthreads();
+  double* h = hist + (size_t)wp * KN;
+  const int kc = lane % g.Kc, r = lane / g.Kc;
+  const i64 o = tile * g.Kc + kc;
+  const bool own = o < g.nout;
+
+  // the lane's first item: kept coordinates from o, slab coordinates from j
+  const i64 J0 = (i64)s * g.jchunk, J1 = min(g.nslab, J0 + g.jchunk);
+  const i64 jstep = (i64)g.Rw * SW;
+  int cc[PA_MAX_DIMS] = {0};
+  i64 off = 0;
+  if (own && g.nslab > 0) {  // (no extent is 0)
+    i64 q = o, j = J0 + (i64)wp * g.Rw + r;
+#pragma unroll
+    for (int m = 0; m < PA_MAX_DIMS; ++m)
+      if (m < g.nd) {
+        const i64 e = g.ext[m];
+        if (g.kept[m]) {
+          cc[m] = (int)(q % e);
+          q /= e;
+        } else {
+          cc[m] = (int)(j % e);
+          j /= e;
+        }
+        off += (i64)cc[m] * g.str[m];
+      }
+  }
+  auto put = [&](int key, A v) {
+    const unsigned grp = __match_any_sync(~0u, key);
+    if (grp == ~0u) {  // one key in the whole warp (a bin constant along the items): a shuffle tree
+      if (key < 0) return;
+#pragma unroll
+      for (int d = 16; d > 0; d >>= 1) v = add(v, __shfl_down_sync(~0u, v, d));
+      if (lane == 0) h[key] = add(h[key], v);
+      __syncwarp();
+      return;
+    }
+    sv[wp][lane] = v;
+    __syncwarp();
+    if (key >= 0 && (grp & ((1u << lane) - 1)) == 0) {
+      A sum = v;
+      for (unsigned rr = grp & (grp - 1); rr; rr &= rr - 1) sum = add(sum, sv[wp][__ffs(rr) - 1]);
+      h[key] = add(h[key], sum);
+    }
+    __syncwarp();
+  };
+
+  int co[PA_MAX_DIMS];  // the load odometer runs RU steps ahead of the binning one
+  i64 offl = off;
+#pragma unroll
+  for (int m = 0; m < PA_MAX_DIMS; ++m) co[m] = cc[m];
+  for (i64 jb = J0 + (i64)wp * g.Rw; jb < J1; jb += jstep * RU) {  // uniform over the warp
+    E xa[RU], xb[RU];
+#pragma unroll
+    for (int k = 0; k < RU; ++k)
+      if (own && jb + r + k * jstep < J1) {
+        xa[k] = ld_elem(a + offl, g.vec);
+        if (M == M_DOT) xb[k] = ld_elem(b + offl, g.vec);
+        sd_advance(g, co, &offl);
+      }
+#pragma unroll
+    for (int k = 0; k < RU; ++k) {
+      const bool in = own && jb + r + k * jstep < J1;
+      int key = -1;
+      A v = 0.0;
+      if (in) {
+        int w;
+        const int bin = sd_mode(g, cc, &w);
+        v = Rd::elem(xa[k], M == M_DOT ? xb[k] : xa[k], typename Rd::T(), 0);
+        if (w == 2) v = mul(2.0, v);  // an exact doubling
+        key = bin < 0 ? -1 : kc * nb + bin;
+        sd_advance(g, cc, &off);
+      }
+      put(key, v);
+    }
+  }
+  __syncthreads();
+
+  // the CTA's partial (warps in order); with S > 1 the tile's last CTA folds the S partials in order
+  typename Rd::R* res = (typename Rd::R*)g.result;
+  const i64 nv = min((i64)KN, (g.nout - tile * g.Kc) * nb);  // the tile's values
+  if (g.S > 1) {
+    double* part = g.part + (size_t)tile * g.S * KN;
+    for (int i = t; i < nv; i += ST) {
+      A v = hist[i];
+#pragma unroll
+      for (int w = 1; w < SW; ++w) v = add(v, hist[(size_t)w * KN + i]);
+      part[(size_t)s * KN + i] = v;
+    }
+    __threadfence();
+    __syncthreads();
+    if (t == 0) last = atomicAdd(g.tickets + tile, 1u) == (unsigned)g.S - 1;
+    __syncthreads();
+    if (!last) return;
+    __threadfence();
+    if (t == 0) g.tickets[tile] = 0;  // the next call (ordered after this one) starts from zero
+  }
+  for (int i0 = t; i0 < nv; i0 += ST * RU) {  // RU values per thread: independent loads
+    A v[RU];
+#pragma unroll
+    for (int k = 0; k < RU; ++k) {
+      const int i = i0 + k * ST;
+      if (i < nv) {
+        if (g.S > 1) {
+          const double* part = g.part + (size_t)tile * g.S * KN + i;
+          v[k] = __ldcg(part);
+          for (int q = 1; q < g.S; ++q) v[k] = add(v[k], __ldcg(part + (size_t)q * KN));
+        } else {
+          v[k] = hist[i];
+#pragma unroll
+          for (int w = 1; w < SW; ++w) v[k] = add(v[k], hist[(size_t)w * KN + i]);
+        }
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < RU; ++k) {
+      const i64 i = tile * KN + i0 + k * ST;  // = b + nbins * o
+      if (i0 + k * ST < nv) {
+        if (g.cb.nranks == 1) res[i] = Rd::finish(v[k]);
+        else st16(g.cb.areas[g.cb.rank] + g.cb.area_off + (size_t)i * 16, v[k]);
+      }
+    }
+  }
+  if (g.cb.nranks == 1) return;
+  __threadfence_system();
+  __syncthreads();
+  unsigned* all = g.tickets + (g.S > 1 ? g.tiles : 0);
+  if (t == 0) last = atomicAdd(all, 1u) == (unsigned)(g.tiles - 1);
+  __syncthreads();
+  if (!last) return;
+  __threadfence_system();
+  if (t == 0) *all = 0;
+  group_combine<Rd, ST>(g.cb, g.nout * nb, res);
+}
+
 // ---- state: workspace, window tables and the event serialising the calls ----------------------
 struct ReduceState {
   int device = 0, G_max = 1;
@@ -749,8 +994,9 @@ struct ReduceState {
   unsigned* dtickets = nullptr;     // pa_reduce_dims: G_max + 1 tickets and G_max * RT partials,
   unsigned char* dpart = nullptr;   //   made by the first such call (stream-ordered)
   unsigned* sticket = nullptr;      // pa_shell_spectrum: one ticket and G x nbins partials, made
-  double* spart = nullptr;          //   and grown by the calls (stream-ordered)
-  size_t spart_n = 0;
+  double* spart = nullptr;          //   and grown by the calls (stream-ordered); the partials are
+  size_t spart_n = 0;               //   shared with pa_shell_spectrum_dims
+  unsigned* sdtickets = nullptr;    // pa_shell_spectrum_dims: G_max + 1 tickets
   cudaEvent_t done = nullptr;       // the previous reduction's last kernel
   ull seq = 0;
   // held from the wait on `done` to its record: host threads calling at once cannot both order
@@ -772,6 +1018,7 @@ void reduce_state_destroy(ReduceState* s) {
   cudaFree(s->dpart);
   cudaFree(s->sticket);
   cudaFree(s->spart);
+  cudaFree(s->sdtickets);
   cudaGetLastError();
   delete s;
 }
@@ -1130,6 +1377,18 @@ pa_status reduce_dims(Comm* comm, int dtype, int map, int op, const void* pred_v
 }
 
 // ---- pa_shell_spectrum ---------------------------------------------------------------------------
+// the spectra's partials hold at least `need` doubles (stream-ordered: after the previous
+// reduction on this state, which may still read them)
+static pa_status grow_spart(ReduceState* st, size_t need, cudaStream_t cs) {
+  if (st->spart_n >= need) return PA_OK;
+  if (st->spart) CU(cudaFreeAsync(st->spart, cs));
+  st->spart = nullptr;
+  st->spart_n = 0;
+  CU(cudaMallocAsync((void**)&st->spart, need * sizeof(double), cs));
+  st->spart_n = need;
+  return PA_OK;
+}
+
 template <class E, int M> static pa_status run_spectrum(const SArgs& g, size_t smem, cudaStream_t s) {
   CU(cudaFuncSetAttribute(k_spectrum<E, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   k_spectrum<E, M><<<g.G, ST, smem, s>>>(g);
@@ -1211,22 +1470,139 @@ pa_status shell_spectrum(Comm* comm, int dtype, int map, const SpecGeom& sg, con
 
   CU(cudaStreamWaitEvent(cs, st->done, 0));
   // workspace, stream-ordered (after the previous reduction on this state, which may still use it)
-  const size_t need = (size_t)g.G * sg.nbins;
   if (!st->sticket) {
     CU(cudaMallocAsync((void**)&st->sticket, sizeof(unsigned), cs));
     CU(cudaMemsetAsync(st->sticket, 0, sizeof(unsigned), cs));
   }
-  if (st->spart_n < need) {
-    if (st->spart) CU(cudaFreeAsync(st->spart, cs));
-    st->spart = nullptr;
-    st->spart_n = 0;
-    CU(cudaMallocAsync((void**)&st->spart, need * sizeof(double), cs));
-    st->spart_n = need;
-  }
+  RC(grow_spart(st, (size_t)g.G * sg.nbins, cs));
   g.ticket = st->sticket;
   g.part = st->spart;
   RC(wide ? (dot ? run_spectrum<c64, M_DOT>(g, smem, cs) : run_spectrum<c64, M_ABS2>(g, smem, cs))
          : (dot ? run_spectrum<c32, M_DOT>(g, smem, cs) : run_spectrum<c32, M_ABS2>(g, smem, cs)));
+  CU(cudaEventRecord(st->done, cs));
+  return PA_OK;
+}
+
+// ---- pa_shell_spectrum_dims ------------------------------------------------------------------------
+template <class E, int M> static pa_status run_spectrum_dims(const SDArgs& g, size_t smem, cudaStream_t s) {
+  CU(cudaFuncSetAttribute(k_spectrum_dims<E, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  k_spectrum_dims<E, M><<<(unsigned)(g.tiles * g.S), ST, smem, s>>>(g);
+  count_launch();
+  CU(cudaGetLastError());
+  return PA_OK;
+}
+template <class E, int M> static pa_status spectrum_dims_occupancy(size_t smem, int* occ) {
+  CU(cudaFuncSetAttribute(k_spectrum_dims<E, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(occ, k_spectrum_dims<E, M>, ST, smem));
+  return PA_OK;
+}
+
+pa_status shell_spectrum_dims(Comm* comm, int dtype, int map, const SpecDimsGeom& geo,
+                              const void* a, const void* b, void* result, void* stream) {
+  const SpecGeom& sg = geo.sp;
+  const DimsGeom& dg = geo.dg;
+  ReduceWindow w;
+  if (comm) RC(comm_reduce_window(comm, &w));
+  const int P = w.nranks;
+  if (P > 1 && !w.flags) {
+    set_error("pa_shell_spectrum_dims: the combine runs through the communicator's flag window, and "
+              "this communicator has none (NCCL without the window, or the nccl_fences tunable)");
+    return PA_ESTATE;
+  }
+  ReduceState* st = nullptr;
+  RC(state_of(comm, w, stream, &st));
+  std::lock_guard<std::mutex> serial(st->mu);
+  if (P > 1 && !st->tables_ready) {
+    set_error("reduction: the flag window's tables were not uploaded (pa_comm_flags_import)");
+    return PA_ESTATE;
+  }
+  const cudaStream_t cs = (cudaStream_t)stream;
+  const bool wide = dtype == D_C64, dot = map == M_DOT;
+  const int es = wide ? 16 : 8;
+
+  SDArgs g;
+  memset(&g, 0, sizeof g);
+  g.nd = dg.nd;
+  g.N = sg.N;
+  g.nout = geo.nout;
+  g.nslab = 1;
+  i64 stride = 1;
+  int fastest = -1;  // the fastest memory dim of extent > 1
+  for (int m = 0; m < dg.nd; ++m) {
+    g.kept[m] = !dg.red[m];
+    g.ext[m] = (int)dg.ext[m];
+    g.str[m] = stride;
+    stride *= dg.ext[m];
+    if (dg.red[m]) g.nslab *= dg.ext[m];
+    if (fastest < 0 && dg.ext[m] > 1) fastest = m;
+  }
+  for (int m = 0; m < sg.N; ++m) {
+    g.lo[m] = (int)sg.lo[m];
+    g.ng[m] = (int)sg.ng[m];
+    g.s[m] = sg.s[m];
+    g.lpos[m] = sg.lpos[m];
+  }
+  g.mask = geo.bin_mask;
+  g.r2c = sg.r2c;
+  g.rfft_n = sg.rfft_n;
+  g.width = sg.width;
+  g.nbins = sg.nbins;
+  // tiles of Kc outputs: Kc > 1 only when the fastest memory dim is kept (the lanes' loads are then
+  // consecutive elements), as long as the warp histograms fit SD_SMEM
+  int Kc = 1;
+  if (fastest >= 0 && g.kept[fastest]) {
+    Kc = SD_KC;
+    while (Kc > 1 && (Kc / 2 >= dg.ext[fastest] || (size_t)SW * Kc * sg.nbins * 8 > SD_SMEM)) Kc /= 2;
+  }
+  g.Kc = Kc;
+  g.Rw = 32 / Kc;
+  const size_t smem = (size_t)SW * Kc * sg.nbins * sizeof(double);
+  int occ = 0;
+  RC(wide ? (dot ? spectrum_dims_occupancy<c64, M_DOT>(smem, &occ) : spectrum_dims_occupancy<c64, M_ABS2>(smem, &occ))
+         : (dot ? spectrum_dims_occupancy<c32, M_DOT>(smem, &occ) : spectrum_dims_occupancy<c32, M_ABS2>(smem, &occ)));
+  g.tiles = std::max<i64>(1, (g.nout + Kc - 1) / Kc);
+  // splits of the slab: only when the tiles leave resident CTAs idle and each split keeps at least
+  // RU steps per warp; depends on the geometry, nbins and the device only
+  const int sms = st->G_max / R_CTAS_PER_SM;
+  const i64 G = (i64)sms * std::max(1, std::min(occ, S_CTAS_PER_SM));
+  i64 S = 1;
+  if (g.nout > 0 && g.tiles < G)
+    S = std::max<i64>(1, std::min<i64>(G / g.tiles, g.nslab / ((i64)g.Rw * SW * RU)));
+  g.jchunk = std::max<i64>(1, (g.nslab + S - 1) / S);
+  g.S = (int)S;
+  i64 delta = (i64)g.Rw * SW;
+  for (int m = 0; m < dg.nd; ++m)
+    if (dg.red[m] && g.nslab > 0) {
+      g.sstep[m] = (int)(delta % dg.ext[m]);
+      delta /= dg.ext[m];
+    }
+  const uintptr_t pa_ = (uintptr_t)a, pb = (uintptr_t)b;
+  g.vec = (pa_ % es == 0) && (!dot || pb % es == 0);
+  g.a = a;
+  g.b = dot ? b : a;
+  g.result = result;
+  if (P > 1) {
+    combine_args(w, st, &g.cb);
+    g.cb.topo_M = dg.topo_M;
+    for (int i = 0; i < dg.topo_M; ++i) {
+      g.cb.topo_dims[i] = (int)dg.topo_dims[i];
+      g.cb.coords[i] = (int)dg.coords[i];
+    }
+    g.cb.keep_grid = dg.keep_grid;
+  }
+  g.cb.nranks = P;
+  g.cb.rank = w.rank;
+
+  CU(cudaStreamWaitEvent(cs, st->done, 0));
+  if (!st->sdtickets) {  // (S > 1 only with fewer tiles than G <= G_max)
+    CU(cudaMallocAsync((void**)&st->sdtickets, (size_t)(st->G_max + 1) * sizeof(unsigned), cs));
+    CU(cudaMemsetAsync(st->sdtickets, 0, (size_t)(st->G_max + 1) * sizeof(unsigned), cs));
+  }
+  if (S > 1) RC(grow_spart(st, (size_t)g.tiles * S * Kc * sg.nbins, cs));
+  g.tickets = st->sdtickets;
+  g.part = st->spart;
+  RC(wide ? (dot ? run_spectrum_dims<c64, M_DOT>(g, smem, cs) : run_spectrum_dims<c64, M_ABS2>(g, smem, cs))
+         : (dot ? run_spectrum_dims<c32, M_DOT>(g, smem, cs) : run_spectrum_dims<c32, M_ABS2>(g, smem, cs)));
   CU(cudaEventRecord(st->done, cs));
   return PA_OK;
 }

@@ -396,5 +396,32 @@ RHD int spec_bin(double q, double width, int nbins) {
   return b < (double)nbins ? (int)b : -1;
 }
 
+// Spectra over chosen dims (pa_shell_spectrum_dims, DESIGN §3n): only the bin dims enter |k|.
+// mask bit d set: logical dim d + 1 is a bin dim (every bit of the N dims: pa_shell_spectrum).
+// q of a mode from its k_d in logical-dim order, the unbinned dims skipped
+RHD double spec_q(int N, const double (&k)[8], unsigned mask) {
+  double q = 0.0;
+#ifdef __CUDA_ARCH__
+#pragma unroll
+#endif
+  for (int d = 0; d < 8; ++d)
+    if (d < N && ((mask >> d) & 1)) q = add(q, mul(k[d], k[d]));
+  return q;
+}
+// the bin of the extreme mode plus one (the default nbins): |k| grows with every |wavenumber|, so
+// the corner of the largest |wavenumber| along each bin dim holds the last bin (a dim of extent 0
+// or 1 adds 0); n: global extents in logical order, rfft_dim 1-based (0: none).  Saturates at
+// 2^31 when the bin does not fit an int.
+inline long long spec_default_bins(int N, const long long* n, int rfft_dim, const double* scales,
+                                   double width, unsigned mask) {
+  double k[8] = {0};
+  for (int d = 0; d < N && d < 8; ++d) {
+    const long long top = n[d] == 0 ? 0 : d + 1 == rfft_dim ? n[d] - 1 : n[d] / 2;
+    k[d] = spec_k(scales ? scales[d] : 1.0, top);
+  }
+  const double b = spec_shell(spec_q(N, k, mask), width);
+  return b + 1.0 > (double)INT32_MAX ? (long long)INT32_MAX + 1 : (long long)b + 1;
+}
+
 }  // namespace red
 }  // namespace pa

@@ -760,9 +760,18 @@ end
 # rfft_dim: the logical dim holding the n ÷ 2 + 1 bins of a real-to-complex transform of length
 # rfft_n (default 2 (M - 1)); scales: one per spatial dim (2π / L_d; default 1); width: the shell
 # width; nbins: default the bin of the extreme mode plus one (pa_shell_spectrum_nbins).
+# dims / keep (pa_shell_spectrum_dims, DESIGN §3n): |k| over the bin dims `dims` only (spatial,
+# default all), the logical dims in `keep` (extra dims N+1.. included) kept, every other dim summed:
+# dims = (1, 3), keep = (2,) is E(k_h; y).  With `keep` the result has size(parent(u)) with every
+# non-kept position 1 and a leading nbins dim (bins fastest, as the C layout result[b + nbins * o]),
+# this rank's local range along each kept dim.
 function shell_spectrum(f::F, u::CuPencilArray{T}, etc::Vararg{CuPencilArray{T}};
                         rfft_dim::Integer = 0, rfft_n::Integer = 0, scales = nothing,
-                        width::Real = 1.0, nbins = nothing) where {F,T<:Union{ComplexF64,ComplexF32}}
+                        width::Real = 1.0, nbins = nothing, dims = nothing,
+                        keep = ()) where {F,T<:Union{ComplexF64,ComplexF32}}
+    (dims === nothing && isempty(keep)) ||
+        return shell_spectrum_dims(f, u, etc...; rfft_dim, rfft_n, scales, width, nbins,
+                                   dims = dims === nothing ? Tuple(1:ndims(pencil(u))) : dims, keep)
     length(etc) <= 1 || throw(ArgumentError("shell_spectrum takes one or two arrays"))
     v = isempty(etc) ? nothing : etc[1]
     v === nothing || PencilArrays._check_compatible_arrays(u, v)
@@ -787,6 +796,43 @@ function shell_spectrum(f::F, u::CuPencilArray{T}, etc::Vararg{CuPencilArray{T}}
         pencil_handle(H, pencil(u)), length(ex), ex, H.comm, PA_DTYPE[T], map,
         ptr_or_null(parent(u)), v === nothing ? C_NULL : ptr_or_null(parent(v)), rfft_dim, rfft_n,
         sc, width, n, devptr(result), stream_ptr()))
+    result
+end
+
+function shell_spectrum_dims(f::F, u::CuPencilArray{T}, etc::Vararg{CuPencilArray{T}};
+                             rfft_dim, rfft_n, scales, width, nbins, dims,
+                             keep) where {F,T<:Union{ComplexF64,ComplexF32}}
+    length(etc) <= 1 || throw(ArgumentError("shell_spectrum takes one or two arrays"))
+    v = isempty(etc) ? nothing : etc[1]
+    v === nothing || PencilArrays._check_compatible_arrays(u, v)
+    map = pa_map(f)
+    (map == 2 && v === nothing) || (map == 3 && v !== nothing) ||
+        throw(ArgumentError("shell_spectrum: abs2 of one array or realdot of two, not $f"))
+    H = handles(topology(pencil(u)))
+    N = ndims(pencil(u))
+    sc = scales === nothing ? C_NULL : Float64[s for s in scales]
+    sc === C_NULL || length(sc) == N || throw(ArgumentError("shell_spectrum: one scale per dim"))
+    bd = Cint[d for d in dims]
+    kd = Cint[d for d in keep]
+    nb = Ref{Cint}()
+    GC.@preserve sc bd check(ccall((:pa_shell_spectrum_dims_nbins, libpa), Cint,
+        (Ptr{Cvoid}, Cint, Int64, Ptr{Float64}, Cdouble, Cint, Ptr{Cint}, Ptr{Cint}),
+        pencil_handle(H, pencil(u)), rfft_dim, rfft_n, sc, width, length(bd), bd, nb))
+    n = nbins === nothing ? Int(nb[]) : Int(nbins)
+    # the result: parent(u)'s local extents with every non-kept position 1, bins first (fastest)
+    nl = ndims(parent(u))
+    pp = permutation(pencil(u))
+    perm = isidentity(pp) ? Tuple(1:N) : Tuple(pp)  # memory dim m holds logical dim perm[m]
+    sz = ntuple(m -> (m <= N ? perm[m] : m) in keep ? size(parent(u), m) : 1, nl)
+    result = CuArray{real(T)}(undef, max(n, 1), sz...)
+    ex = Int64[extra_dims(u)...]
+    ptr_or_null(A) = isempty(A) ? C_NULL : devptr(A)
+    GC.@preserve sc bd kd check(ccall((:pa_shell_spectrum_dims, libpa), Cint,
+        (Ptr{Cvoid}, Cint, Ptr{Int64}, Ptr{Cvoid}, Cint, Cint, Ptr{Cvoid}, Ptr{Cvoid}, Cint, Int64,
+         Ptr{Float64}, Cdouble, Cint, Cint, Ptr{Cint}, Cint, Ptr{Cint}, Ptr{Cvoid}, Ptr{Cvoid}),
+        pencil_handle(H, pencil(u)), length(ex), ex, H.comm, PA_DTYPE[T], map,
+        ptr_or_null(parent(u)), v === nothing ? C_NULL : ptr_or_null(parent(v)), rfft_dim, rfft_n,
+        sc, width, n, length(bd), bd, length(kd), kd, ptr_or_null(result), stream_ptr()))
     result
 end
 

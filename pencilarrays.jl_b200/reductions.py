@@ -229,17 +229,54 @@ def _spectrum_geometry(u: PencilArray, rfft_dim, rfft_n, scales, width):
     return rd, rn, sc, width
 
 
-def spectrum_nbins(u: PencilArray, *, rfft_dim=None, rfft_n=None, scales=None, width=1.0):
-    """The default bin count of :func:`shell_spectrum`: the bin of the extreme mode plus one, as
-    the library computes it (``pa_shell_spectrum_nbins``)."""
+def _dim_list(u: PencilArray, dims, what, spatial):
+    """``dims`` (a dim or a collection of 1-based logical dims) checked as :func:`result_shape`
+    checks them, as a tuple: spatial dims only for the bin dims, any dim for the kept ones."""
+    if isinstance(dims, int) and not isinstance(dims, bool):
+        dims = (dims,)
+    try:
+        dims = tuple(dims)
+    except TypeError:
+        raise ArgumentError(_lib.PA_EINVAL, f"{what} {dims!r} is not a dim or a collection of dims") from None
+    N, nd = len(u.space_dims), u.data.dim()
+    top = N if spatial else nd
+    for d in dims:
+        if not isinstance(d, int) or isinstance(d, bool) or not 1 <= d <= top:
+            raise ArgumentError(_lib.PA_EINVAL, f"{what}: dim {d!r} out of range 1..{top} "
+                                + ("(the spatial dims)" if spatial else
+                                   f"({N} spatial dims, then {nd - N} extra)"))
+    if len(set(dims)) != len(dims):
+        raise ArgumentError(_lib.PA_EINVAL, f"{what} {dims} name a dim twice")
+    return dims
+
+
+def _bin_dims(u: PencilArray, dims):
+    """The checked bin dims (None: every spatial dim)."""
+    if dims is None:
+        dims = tuple(range(1, len(u.space_dims) + 1))
+    dims = _dim_list(u, dims, "dims", True)
+    if not dims:
+        raise ArgumentError(_lib.PA_EINVAL, "dims must name at least one bin dim")
+    return dims
+
+
+def spectrum_nbins(u: PencilArray, *, rfft_dim=None, rfft_n=None, scales=None, width=1.0, dims=None):
+    """The default bin count of :func:`shell_spectrum`: the bin of the extreme mode over the bin
+    dims ``dims`` (default: every spatial dim) plus one, as the library computes it
+    (``pa_shell_spectrum_nbins`` / ``pa_shell_spectrum_dims_nbins``)."""
     rd, rn, sc, width = _spectrum_geometry(u, rfft_dim, rfft_n, scales, width)
     out = C.c_int()
-    check(lib.pa_shell_spectrum_nbins(u.pencil._h, rd, rn, sc, width, C.byref(out)))
+    if dims is None:
+        check(lib.pa_shell_spectrum_nbins(u.pencil._h, rd, rn, sc, width, C.byref(out)))
+    else:
+        bd = _bin_dims(u, dims)
+        check(lib.pa_shell_spectrum_dims_nbins(u.pencil._h, rd, rn, sc, width, len(bd),
+                                               (C.c_int * len(bd))(*bd), C.byref(out)))
     return out.value
 
 
 def shell_spectrum(u: PencilArray, v: PencilArray = None, *, rfft_dim=None, rfft_n=None,
-                   scales=None, width=1.0, nbins=None):
+                   scales=None, width=1.0, nbins=None, dims=None, keep=None):
     """Shell-binned spectrum ``E(b) = sum over bin(|k|) == b of w * abs2(u)`` (with ``v``: of
     ``w * real(u * conj(v))``, a co-spectrum) of complex arrays whose spatial dims hold the modes
     of an unnormalised DFT (``pa_shell_spectrum``, DESIGN §3m).  ``rfft_dim``: the 1-based logical
@@ -248,7 +285,16 @@ def shell_spectrum(u: PencilArray, v: PencilArray = None, *, rfft_dim=None, rfft
     spatial dim (``2 pi / L``; default 1); ``width``: the shell width; ``nbins``: default
     :func:`spectrum_nbins`.  Extra dims add into the same bins.  Returns the global spectrum (the
     same bits on every rank), a 1-d tensor of ``nbins`` float64 (float32 for complex64 arrays) on
-    ``u``'s device, computed on torch's current stream in one kernel per rank."""
+    ``u``'s device, computed on torch's current stream in one kernel per rank.
+
+    ``dims`` and ``keep`` (``pa_shell_spectrum_dims``, DESIGN §3n): ``|k|`` is formed from the bin
+    dims ``dims`` only (1-based spatial dims; default every one), each dim in ``keep`` (1-based
+    logical dims, extra dims ``N+1..`` included, none a bin dim) is kept, and every other dim is
+    summed into the bins: ``dims=(1, 3), keep=(2,)`` is E(k_h; y), ``dims=(1,)`` E(k_x), and
+    ``keep=(4,)`` on a 3-component field the per-component spectra.  With ``keep`` the result has
+    ``u.data.shape`` with every non-kept position set to 1 and a trailing ``nbins`` dim; along each
+    kept dim it holds this rank's local range, combined over the ranks that share it.  Without
+    ``keep`` it is ``(nbins,)``."""
     if not isinstance(u, PencilArray):
         raise ArgumentError(_lib.PA_EINVAL, "shell_spectrum takes PencilArrays")
     if v is not None:
@@ -261,23 +307,44 @@ def shell_spectrum(u: PencilArray, v: PencilArray = None, *, rfft_dim=None, rfft
             raise ArgumentError(_lib.PA_EINVAL, f"arrays are not compatible: {v.dtype} != {u.dtype}")
     if u.dtype not in _REAL:
         raise ArgumentError(_lib.PA_EINVAL, f"a spectrum is of complex arrays, not {u.dtype}")
+    sub = dims is not None or keep is not None
+    who = "pa_shell_spectrum_dims" if sub else "pa_shell_spectrum"
+    shape = None
+    if sub:
+        bd = _bin_dims(u, dims)
+        kd = () if keep is None else _dim_list(u, keep, "keep", False)
+        both = set(bd) & set(kd)
+        if both:
+            raise ArgumentError(_lib.PA_EINVAL, f"dim {min(both)} is both a bin dim and a kept dim")
+        if kd:
+            red = tuple(d for d in range(1, u.data.dim() + 1) if d not in kd)
+            shape = result_shape(u, red)[1]
     rd, rn, sc, width = _spectrum_geometry(u, rfft_dim, rfft_n, scales, width)
     out = C.c_int()  # (the geometry's checks, before anything is allocated)
-    check(lib.pa_shell_spectrum_nbins(u.pencil._h, rd, rn, sc, width, C.byref(out)))
+    if sub:
+        check(lib.pa_shell_spectrum_dims_nbins(u.pencil._h, rd, rn, sc, width, len(bd),
+                                               (C.c_int * len(bd))(*bd), C.byref(out)))
+    else:
+        check(lib.pa_shell_spectrum_nbins(u.pencil._h, rd, rn, sc, width, C.byref(out)))
     if nbins is None:
         nbins = out.value
     if not isinstance(nbins, int) or isinstance(nbins, bool) or \
             not 1 <= nbins <= _lib.PA_SPECTRUM_MAX_BINS:
-        raise ArgumentError(_lib.PA_EINVAL, f"pa_shell_spectrum: nbins {nbins!r} out of range "
+        raise ArgumentError(_lib.PA_EINVAL, f"{who}: nbins {nbins!r} out of range "
                             f"1..{_lib.PA_SPECTRUM_MAX_BINS}")
     code_map = _lib.PA_MAP_ABS2 if v is None else _lib.PA_MAP_DOT
     dt = _DTYPES[u.dtype]
-    result = torch.empty(nbins, dtype=_REAL[u.dtype], device=u.data.device)
+    result = torch.empty((nbins,) if shape is None else shape + (nbins,), dtype=_REAL[u.dtype],
+                         device=u.data.device)
     ex = u.extra_dims
+    args = (u.pencil._h, len(ex), i64arr(ex), u.pencil.topology.comm.handle, dt, code_map,
+            C.c_void_p(u.data_ptr() or None),
+            C.c_void_p(v.data_ptr() or None) if v is not None else None, rd, rn, sc, width, nbins)
     with torch.cuda.device(u.data.device):
-        check(lib.pa_shell_spectrum(u.pencil._h, len(ex), i64arr(ex), u.pencil.topology.comm.handle,
-                                    dt, code_map, C.c_void_p(u.data_ptr() or None),
-                                    C.c_void_p(v.data_ptr() or None) if v is not None else None,
-                                    rd, rn, sc, width, nbins, C.c_void_p(result.data_ptr() or None),
-                                    _stream_ptr()))
+        if sub:
+            check(lib.pa_shell_spectrum_dims(*args, len(bd), (C.c_int * len(bd))(*bd), len(kd),
+                                             (C.c_int * max(1, len(kd)))(*kd),
+                                             C.c_void_p(result.data_ptr() or None), _stream_ptr()))
+        else:
+            check(lib.pa_shell_spectrum(*args, C.c_void_p(result.data_ptr() or None), _stream_ptr()))
     return result
